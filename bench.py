@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- LF evaluations/second on the north-star workload (200 taxa x 2000 codons, MG94xREV, 4 omega classes).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
     N>1: python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 ... bench.py --gpus N ...
 
 A "step" is ONE full likelihood-function evaluation: every one of the B*C rate matrices handed over, exponentiated,
@@ -16,6 +16,9 @@ Multi-GPU (strong scaling of one alignment): ranks form (pattern shards) x (clas
 rank exponentiates another group's matrices, patterns for the remaining factor (hyphy_b200/sharding.py); one exchange
 per evaluation on the engine's own NCCL communicator.
 The oracle / reference binary under oracle/ is used only for cpu_baseline and --impl reference.
+--dump-outputs DIR: after the timed steps, the outputs of the last timed evaluation of each timed path as DIR/<name>.npy
+(float64): the lnL values, and the per-pattern log-likelihoods and scaling exponents of the resident path recomputed
+from the same resident state.  Inputs are seeded, so two builds run with the same arguments can be compared output by output.
 """
 from __future__ import annotations
 
@@ -43,11 +46,11 @@ def peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "fallback: H100 SXM data sheet"
 
 
 class ClockSampler:
-    """nvidia-smi sampling DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampling DURING the timed region: SM clock and throttle reasons."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -106,7 +109,7 @@ class ClockSampler:
 
 def algorithmic_work(w, S, word=8):
     """SURVEY.md §8(d) per-evaluation algorithmic work for S patterns (all classes); `word` = bytes per stored
-    conditional (8 on the fp64 path, 4 on the tcgen05 path)."""
+    conditional (8 on the fp64 path, 4 on the tensor-core path)."""
     L, I, D, C = w.tree.n_leaves, w.tree.n_internal, w.D, w.C
     B = L + I - 1
     flops = C * ((I - 1) * S * 2 * D * D + (L + B) * S * D + 2 * S * D)
@@ -192,6 +195,7 @@ def main():
     ap.add_argument("--class-groups", type=int, default=0, help="multi-GPU: force this many class groups (default: as many as divide both)")
     ap.add_argument("--no-class-groups", action="store_true", help="multi-GPU: shard patterns only (every rank exponentiates every class)")
     ap.add_argument("--emulate-shard", default="", help="debug: R/W -> run rank R's pattern shard of a W-rank job on one GPU, no collectives")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR", help="write the last timed evaluation's outputs as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -271,13 +275,15 @@ def main():
             lf.part.set_matrices(c, lf.all_nodes, q[c])
         return lf.compute()
 
+    last = {}
+
     def timed(step):
         for k in range(args.warmup):
             step(k)
         barrier()
         t0 = time.perf_counter()
         for k in range(args.steps):
-            step(k)
+            last[step.__name__] = step(k)
         barrier()
         return max_over_ranks((time.perf_counter() - t0) * 1e3 / args.steps)
 
@@ -309,6 +315,13 @@ def main():
     ms, stage, lnl_res = lf.part.time_resident(w.class_weights, w.pi, iters=args.steps)
     barrier()
     launches = lf.part.launch_count - launches0
+    dump = {}
+    if args.dump_outputs:
+        # per-pattern outputs of the resident state the timed loop evaluated (same matrices, nothing re-staged)
+        lnl_sites, site_l, site_s = lf.compute(want_sites=True)
+        dump = {"lnL_resident": np.array([lnl_res]), "lnL_e2e": np.array([last["e2e_step"]]),
+                "lnL_e2e_dense": np.array([last["e2e_dense_step"]]), "lnL_sites_eval": np.array([lnl_sites]),
+                "site_lnL": np.asarray(site_l, dtype=np.float64), "site_scale": np.asarray(site_s, dtype=np.float64)}
     # the timed region is a few tens of ms; keep the identical load running ~1 s so nvidia-smi (100 ms period) sees it.
     # The repeat count is derived from the rank-reduced time so every rank issues the same number of all-reduces.
     extra = int(min(200, max(1, round(1000.0 / max(max_over_ranks(ms) * args.steps, 1e-3)))))
@@ -342,12 +355,13 @@ def main():
         lnl5 = lf5.compute()
         lf5.part.time_resident(w5.class_weights, w5.pi, iters=3)
         barrier()
-        ms5, stage5, lnl5r = lf5.part.time_resident(w5.class_weights, w5.pi, iters=max(5, args.steps // 2))
+        ms5, stage5, lnl5r = lf5.part.time_resident(w5.class_weights, w5.pi, iters=args.steps)
         barrier()
         ms5 = max_over_ranks(ms5)
         stage5 = [max_over_ranks(float(x)) for x in stage5]
         lf5.close()
         golden5 = -1160063.8295306289                 # unmodified reference binary (tests/golden/c5_mg94_500x5000_c4.npz)
+        dump["lnL_c5_resident"] = np.array([lnl5r])
         c5 = {"workload": "MG94xREV 500 taxa x 5000 codons, 4 omega classes (BASELINE.json configs[4])", "patterns": w5.S,
               "value": 1000.0 / ms5, "unit": "evals/s", "ms_per_step": ms5, "stage_ms": {"expm": stage5[0], "pruning": stage5[1], "root": stage5[2]},
               "layout": f"patterns/{lay5['shards']} x classes/{lay5['groups']}", "lnL": lnl5, "lnL_reference": golden5,
@@ -366,7 +380,8 @@ def main():
             lfs.set_all_compiled()
             lfs.compute()
             lfs.part.time_resident(ws.class_weights, ws.pi, iters=3)
-            mss, sts, lnls = lfs.part.time_resident(ws.class_weights, ws.pi, iters=10)
+            mss, sts, lnls = lfs.part.time_resident(ws.class_weights, ws.pi, iters=args.steps)
+            dump[f"lnL_{key}_resident"] = np.array([lnls])
             kern = lfs.part.pruning_kernel
             lfs.close()
             Ls, Is, Ss, Cs = ws.tree.n_leaves, ws.tree.n_internal, ws.S, ws.C
@@ -383,24 +398,13 @@ def main():
         prune_launches = stage_launches[1]
         prune_ms = stage[1]
         achieved_gbs = (byts / world) / (prune_ms * 1e-3) / 1e9
-        single_launch = prune_launches == 1
-        kname = {"prune64_tc_walk2_kernel": "prune64_tc_walk2_kernel (tcgen05 3xTF32 fused pruning pass, whole tree in one launch, two threads per pattern)",
-                 "prune64_tc_walk_kernel": "prune64_tc_walk_kernel (tcgen05 3xTF32 fused pruning pass, whole tree in one launch)",
-                 "prune64_tc_kernel": "prune64_tc_kernel (tcgen05 3xTF32 fused pruning update, one launch per tree level)",
+        kname = {"prune64_tc_walk2_kernel": "prune64_tc_walk2_kernel (wgmma 3xTF32 fused pruning pass, whole tree in one launch, two threads per pattern)",
+                 "prune64_tc_walk_kernel": "prune64_tc_walk_kernel (wgmma 3xTF32 fused pruning pass, whole tree in one launch)",
+                 "prune64_tc_kernel": "prune64_tc_kernel (wgmma 3xTF32 fused pruning update, one launch per tree level)",
                  "prune64_kernel": "prune64_kernel (fp64 fused pruning update, one launch per tree level)"}.get(prune_kernel, prune_kernel)
-        # DRAM traffic of that kernel from the committed `ncu --set full` capture of this same command (profiles/)
-        traffic, traffic_src = None, None
-        try:
-            prof = json.load(open(os.path.join(ROOT, "profiles", "walk_kernel_latest.json")))["kernels"][0]
-            if tc_mode and single_launch and world == 1:
-                unit = {"Mbyte": 1e6, "Gbyte": 1e9, "Kbyte": 1e3, "byte": 1.0}
-                traffic = sum(prof[k]["value"] * unit[prof[k]["unit"]] for k in ("dram__bytes_read.sum", "dram__bytes_write.sum"))
-                traffic_src = "profiles/walk_kernel_latest.json (ncu --set full, per launch)"
-        except Exception:
-            pass
         roofline = {"kernel": kname, "bound": "hbm",
                     "achieved": achieved_gbs, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": achieved_gbs / pk["hbm_gbs"],
-                    "traffic": traffic, "traffic_source": traffic_src, "peak_source": f"MEASURED_PEAKS.json ({pk_kind})",
+                    "peak_source": f"MEASURED_PEAKS.json ({pk_kind})",
                     "launches_per_eval": prune_launches, "stage_launches_per_eval": {"expm": stage_launches[0], "pruning": stage_launches[1], "root": stage_launches[2]}, "avg_launch_ms": prune_ms / max(prune_launches, 1),
                     "algorithmic_bytes_per_eval": byts, "algorithmic_flops_per_eval": flops,
                     "tflops_pruning": (flops / world) / (prune_ms * 1e-3) / 1e12,
@@ -412,7 +416,7 @@ def main():
         h2d_dense = int(w.C * w.tree.n_branches * w.D * w.D * 8 + w.C * w.tree.n_branches * 4 + (64 + w.C) * 8 + w.tree.n_internal * 4)
         line = {"metric": METRIC, "value": 1000.0 / ms, "unit": "evals/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
                 "ms_per_step": ms, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
-                "dtype": "tf32x3 (tcgen05, fp32 accumulate) pruning + f64 expm/root" if tc_mode else "f64",
+                "dtype": "tf32x3 (wgmma, fp32 accumulate) pruning + f64 expm/root" if tc_mode else "f64",
                 "data": "synthetic",
                 "config": config_dict(S, w.tree.n_branches, w.D, w.C),
                 "layout": f"patterns/{lay['shards']} x classes/{lay['groups']}",
@@ -422,16 +426,16 @@ def main():
                               "d2h_bytes_per_step": 12, "api": "hb2_set_matrices_packed x C + hb2_evaluate_classes", "lnL": lnl_dense},
                 "gpu_launches": int(launches), "clocks": clocks, "roofline": roofline, "lnL": lnl0, "lnL_resident": lnl_res,
                 "lnL_reference": -205416.12461664603, "root_exchange": root_path if world > 1 else None, "c5": c5, "small_states": small}
-        # the same evaluation stream through the PATCHED HyPhy binary (host/_build/hyphy: the reference's HBL interpreter,
+        # the same evaluation stream through the PATCHED HyPhy binary (oracle/_ref/host/hyphy: the reference's HBL interpreter,
         # formula evaluation and DetermineNodesForUpdate on the host, everything below ComputeBlock on the engine):
         # wall-clock evaluations/s of `LFCompute` as a user of the reference would see them
-        host_bin = os.path.join(ROOT, "host", "_build", "hyphy")
+        host_bin = os.path.join(ROOT, "oracle", "_ref", "host", "hyphy")
         if world == 1 and not args.no_host and os.path.isfile(host_bin):
             try:
                 from oracle import ref_harness as rh
-                hr = rh.run_reference(w, n_evals=max(args.steps, 10), n_warm=args.warmup, per_site=False, binary=host_bin,
+                hr = rh.run_reference(w, n_evals=args.steps, n_warm=args.warmup, per_site=False, binary=host_bin,
                                       env_extra={"HYPHY_B200_VERBOSE": "1", "HYPHY_B200_DEVICE": str(local_rank), "HYPHY_B200_TC": "1"})
-                line["host_e2e"] = {"value": max(args.steps, 10) / hr["loop_seconds"], "unit": "evals/s", "lnL": hr["lnL"],
+                line["host_e2e"] = {"value": args.steps / hr["loop_seconds"], "unit": "evals/s", "lnL": hr["lnL"],
                                     "api": "patched HyPhy binary: HBL LFCompute -> _LikelihoodFunction::ComputeBlock -> hb2_hooks -> C ABI (dense Q*t hand-over)",
                                     "engine": hr["engine"][-2:]}
             except Exception as e:
@@ -445,6 +449,11 @@ def main():
             except Exception as e:                   # the baseline is a report, never a reason to lose the bench line
                 line["cpu_baseline"] = {"value": None, "unit": "evals/s", "cores": 0, "kind": "unavailable", "sample": repr(e)}
         print(json.dumps(line), flush=True)
+    if args.dump_outputs:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        suffix = f"_rank{rank}" if world > 1 else ""
+        for name, arr in dump.items():
+            np.save(os.path.join(args.dump_outputs, name + suffix + ".npy"), np.ascontiguousarray(arr, dtype=np.float64))
     if dist is not None:
         dist.barrier()
         dist.destroy_process_group()

@@ -2,11 +2,11 @@
 """Builds the PATCHED host: copies the reference's sources into a scratch build tree and inserts the handful of hook calls
 that bind libhyphy_b200.so behind `_LikelihoodFunction::ComputeBlock` (SURVEY.md §8b; INTEGRATION.md walks through them).
 
-    python host/apply_hooks.py [--ref /root/reference] [--out host/_build]
+    python host/apply_hooks.py --ref <HyPhy source tree> [--out oracle/_ref/host]
 
 Every insertion is anchored on a short text fragment of the reference source (so a maintainer can find the place) and
 adds only calls into host/hb2_hyphy_hooks.{h,cpp} -- this repository contains the ADDED lines only, never reference
-code; the build tree (host/_build, git-ignored) is where the two meet.  The script fails loudly when an anchor is
+code; the build tree (oracle/_ref/host, git-ignored) is where the two meet.  The script fails loudly when an anchor is
 missing or ambiguous, i.e. when the reference has moved on and the binding needs a maintainer's eyes.
 """
 from __future__ import annotations
@@ -121,23 +121,34 @@ def apply(src_root: str) -> None:
         print(f"apply_hooks: {rel}: {len(hooks)} insertion(s)")
 
 
+def _writable(root: str) -> None:
+    """The reference tree may be read-only: its copies must not be, or they could be neither patched nor replaced."""
+    for d, _, files in os.walk(root):
+        os.chmod(d, 0o755)
+        for f in files:
+            os.chmod(os.path.join(d, f), 0o644)
+
+
+def _fresh_copy(src: str, dst: str) -> None:
+    if os.path.isdir(dst):
+        _writable(dst)
+        shutil.rmtree(dst)
+    shutil.copytree(src, dst, copy_function=shutil.copyfile)
+    _writable(dst)
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--ref", default="/root/reference")
-    ap.add_argument("--out", default=os.path.join(HERE, "_build"))
+    ap.add_argument("--ref", required=True)
+    ap.add_argument("--out", default=os.path.join(os.path.dirname(HERE), "oracle", "_ref", "host"))
     args = ap.parse_args()
     src = os.path.join(args.out, "src")
-    if os.path.isdir(src):
-        shutil.rmtree(src)
     os.makedirs(args.out, exist_ok=True)
-    shutil.copytree(os.path.join(args.ref, "src"), src)
+    _fresh_copy(os.path.join(args.ref, "src"), src)
     apply(src)
     # the reference's own batch-file library and regression tests, so that the patched binary can run them on the GPU box
     for sub, dst in (("res", "res"), ("tests/hbltests", "hbltests")):
-        d = os.path.join(args.out, dst)
-        if os.path.isdir(d):
-            shutil.rmtree(d)
-        shutil.copytree(os.path.join(args.ref, sub), d)
+        _fresh_copy(os.path.join(args.ref, sub), os.path.join(args.out, dst))
 
 
 if __name__ == "__main__":

@@ -18,10 +18,10 @@
 //   _LikelihoodFunction::ReconstructAncestors (likefunc2.cpp:308) -> hb2_hooks::materialize  device -> host copies for the
 //                                                                                       ancestral-state readers
 //
-// Environment: HYPHY_B200=0 disables the engine (the unmodified CPU path runs); HYPHY_B200_TC=1 selects the tcgen05
+// Environment: HYPHY_B200=0 disables the engine (the unmodified CPU path runs); HYPHY_B200_TC=1 selects the tensor-core
 // pruning path for 33..64-state partitions (error-compensated 3xTF32: every evaluation is within 1e-6*|lnL| of the
-// reference, measured ~1e-9, but that rounding noise is not smooth in the parameters and HyPhy's optimiser differentiates
-// the likelihood numerically -- measured: SimpleOptimizations/SmallCodon.bf stops 0.0035 log units short with it -- so
+// reference, typically ~1e-9, but that rounding noise is not smooth in the parameters and HyPhy's optimiser differentiates
+// the likelihood numerically -- SimpleOptimizations/SmallCodon.bf stops short of the optimum with it -- so
 // the DEFAULT under the optimiser is the fp64 kernels, whose noise is ~1e-13); HYPHY_B200_DEVICE=n selects the CUDA device (default: MPI rank modulo visible devices, or 0);
 // HYPHY_B200_VERBOSE=1 prints one line per partition created / destroyed with evaluation counts.
 #pragma once

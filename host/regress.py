@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""Runs the reference's OWN regression batch files (tests/hbltests, copied to host/_build/hbltests by apply_hooks.py) through
+"""Runs the reference's OWN regression batch files (tests/hbltests, copied to oracle/_ref/host/hbltests by apply_hooks.py) through
 a HyPhy binary and extracts what they report: every `Log Likelihood = x` a fitted likelihood function prints, and the
 test's PASSED / FAILED verdict.
 
-    python host/regress.py expect   # here (container with /root/reference): run the UNMODIFIED reference binary
+    python host/regress.py expect   # where the reference sources were built: run the UNMODIFIED reference binary
                                     # (oracle/_ref/hyphy) and write tests/golden/hbltests_expected.json
-    python host/regress.py check    # GPU box: run the PATCHED binary (host/_build/hyphy, engine on, its default fp64
+    python host/regress.py check    # on the GPU: run the PATCHED binary (oracle/_ref/host/hyphy, engine on, its default fp64
                                     # kernels) and compare;  `tc` = the same with HYPHY_B200_TC=1, `cpu` = engine off
 
 TEST INFRASTRUCTURE (it drives the unmodified reference as the checker); the product is the patched binary it checks.
@@ -15,13 +15,14 @@ from __future__ import annotations
 import json
 import os
 import re
+import shutil
 import subprocess
 import sys
 import tempfile
 import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-BUILD = os.path.join(ROOT, "host", "_build")
+BUILD = os.path.join(ROOT, "oracle", "_ref", "host")
 REF_BIN = os.path.join(ROOT, "oracle", "_ref", "hyphy")
 HOST_BIN = os.path.join(BUILD, "hyphy")
 EXPECTED = os.path.join(ROOT, "tests", "golden", "hbltests_expected.json")
@@ -56,16 +57,35 @@ TESTS = [
 # changes the summation order and with it the optimiser's path): only its first three fits are compared
 STABLE_PREFIX = {"libv3/RELAX.wbf": 3}
 
+_WORK = None
+
+
+def work_tree():
+    """A private, writable copy of the batch-file library and the regression tests: the batch files write their result
+    files (JSON reports, optimisation logs) next to themselves, and the build tree may be read-only for whoever runs them."""
+    global _WORK
+    if _WORK is None:
+        _WORK = tempfile.mkdtemp(prefix="hb2lib_")
+        for sub in ("res", "hbltests"):
+            shutil.copytree(os.path.join(BUILD, sub), os.path.join(_WORK, sub), copy_function=shutil.copyfile)
+        for d, _, files in os.walk(_WORK):           # copytree keeps the directories' modes: make them writable
+            os.chmod(d, 0o755)
+            for f in files:
+                os.chmod(os.path.join(d, f), 0o644)
+    return _WORK
+
+
 LL = re.compile(r"(?:Log Likelihood|Log\(L\))\s*=\s*(-?[0-9]+\.?[0-9]*(?:[eE][-+]?[0-9]+)?)")
 
 
 def run(binary, test, env_extra=None, timeout=900, threads=0):
-    path = os.path.join(BUILD, "hbltests", test)
+    work = work_tree()
+    path = os.path.join(work, "hbltests", test)
     env = dict(os.environ)
     env.update(env_extra or {})
     tmp = tempfile.mkdtemp(prefix="hb2reg_")
     t0 = time.time()
-    args = [binary, f"LIBPATH={os.path.join(BUILD, 'res')}"] + ([f"CPU={threads}"] if threads else []) + [path]
+    args = [binary, f"LIBPATH={os.path.join(work, 'res')}"] + ([f"CPU={threads}"] if threads else []) + [path]
     try:
         pr = subprocess.run(args, cwd=tmp, stdin=subprocess.DEVNULL, stdout=subprocess.PIPE, stderr=subprocess.STDOUT,
                             text=True, env=env, timeout=timeout)

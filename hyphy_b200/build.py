@@ -1,4 +1,4 @@
-"""Builds libhyphy_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Builds libhyphy_b200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import glob
@@ -8,7 +8,8 @@ import subprocess
 PKG = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "libhyphy_b200.so")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC"]
 
 
@@ -32,7 +33,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         subprocess.check_call(cmd)
         objs.append(obj)
     # soname: hosts that link the library (host/Makefile) find it through their rpath, not through the build-time path
-    subprocess.check_call([nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-Xlinker", "-soname,libhyphy_b200.so",
+    subprocess.check_call([nvcc, "-shared"] + ARCH + ["-Xlinker", "-soname,libhyphy_b200.so",
                            "-o", LIB] + objs + ["-ldl"])
     return LIB
 

@@ -231,10 +231,10 @@ struct hb2_partition {
     double *d_cond_side = nullptr;            // fp64 lanes kernel: side products [C][I][Sp][64] (exponents: second half of d_scal)
     int *d_lane_flags = nullptr;              // [C][2I][Sp/64] pass id of the last production
     int lane_pass = 0, lanes_resident[2] = {0, 0}, lanes_force_nw = 0;   // co-resident CTAs of the 4- and 8-warp shapes; HB2_LANES_WARPS
-    int sm_count = 148;
+    int sm_count = 132;
     bool expm_dfma = false;                   // HB2_EXPM_DFMA=1: previous FFMA-style fp64 expm kernel (A/B testing)
     bool use_walk = false;
-    bool walk_v2 = false;                     // HB2_WALK_V2=1: two threads per pattern (prune64_tc_walk2_kernel; correct, measured 20 % slower, DESIGN 4.2)
+    bool walk_v2 = false;                     // HB2_WALK_V2=1: two threads per pattern (prune64_tc_walk2_kernel; correct, opt-in, DESIGN 4.2)
     int walk_max_resident = 0;
     // single-branch shortcut (hb2_branch_cache_*): outside vectors of one branch, all owned classes
     double *d_bc_out = nullptr; int *d_bc_outE = nullptr, *d_bc_sib = nullptr; int64_t bc_node = -1;
@@ -602,8 +602,8 @@ int plan_walk(const std::vector<std::vector<int>> &children, const std::vector<i
             jch[n] = children[n];
         }
     }
-    // Lane assignment = list scheduling of the dirty jobs on K in-order lanes with a rough cost model (cycles measured
-    // with HB2_WALK_TRACE, profiles/): the pass is bound by the busiest lane or by the deepest root path, so the
+    // Lane assignment = list scheduling of the dirty jobs on K in-order lanes with a rough cost model (cycles per step
+    // kind, as HB2_WALK_TRACE reports them): the pass is bound by the busiest lane or by the deepest root path, so the
     // (job, lane) pair that can start first is scheduled next, ties going to the longer remaining path; a job whose
     // contracted internal child was the lane's previous job continues there (register hand-over: the cheapest
     // contraction).  Every lane executes its jobs in the order they were scheduled and a job is scheduled only after
@@ -793,8 +793,8 @@ int run_walk(hb2_partition *p, int cat0, int ncls, const std::vector<std::vector
     return 0;
 }
 
-// 4 states: one or two patterns per thread -- (passes over the resident capacity) x (measured cost of a pass: 0.63 vs 0.98 ms
-// at 256 taxa, profiles/r2x_small*.json)
+// 4 states: one or two patterns per thread -- (passes over the resident capacity) x (relative cost of a pass: a two-pattern
+// pass costs about 1.55 one-pattern passes)
 static bool small_two_patterns(const hb2_partition *p, int ncls) {
     if (p->Dp != 4 || p->small_ilp == 1) return false;
     if (p->small_ilp == 2) return true;
@@ -882,8 +882,7 @@ int run_fp64_lanes(hb2_partition *p, int cat0, int ncls, const std::vector<std::
     for (auto &lv : levels) total += (int)lv.size();
     if (total == 0) return 0;
     // CTA shape: 4 warps x 8 patterns, 4 CTAs per SM.  The 8-warp shape (64 patterns, 3 per SM) gives the north-star shape a
-    // third lane and c5 a single round, and is slower on both (1.28 vs 0.98 ms, 7.6 vs 5.6 ms: profiles/r2s_*): it stays
-    // behind HB2_LANES_WARPS=8 for A/B runs.
+    // third lane and c5 a single round, but was slower on both: it stays behind HB2_LANES_WARPS=8 for A/B runs.
     const int nw = p->lanes_force_nw == 8 ? 8 : 4;
     const int T = (int)(p->Sp / (8 * nw)), CT = ncls * T, resident = p->lanes_resident[nw == 8];
     const int K = std::max(1, std::min(std::min(p->walk_lane_cap, total), resident / std::max(CT, 1)));
@@ -960,8 +959,8 @@ int run_fp64_lanes(hb2_partition *p, int cat0, int ncls, const std::vector<std::
 int run_pruning(hb2_partition *p, int cat0, int ncls, const std::vector<std::vector<int>> &levels) {
     if (p->use_tc && p->use_walk) return run_walk(p, cat0, ncls, levels);
     // one launch per evaluation pays only when (tiles x classes) fills the machine about twice over (c5: 316 CTAs); below
-    // that the per-level launches expose more parallelism (north-star shape: 128 CTAs walk 1.55 ms, 54 level launches take
-    // 1.38 ms; a single class of it -- the patched host's per-class ComputeBlock -- would leave 116 SMs idle)
+    // that the per-level launches expose more parallelism (a single class of the north-star shape -- the patched host's
+    // per-class ComputeBlock -- is 32 CTAs and would leave most SMs idle)
     if (!p->use_tc && p->Dp == 64 && p->fp64_mode == 2) return run_fp64_lanes(p, cat0, ncls, levels);
     if (!p->use_tc && p->Dp == 64 && p->fp64_walk && (int64_t)(p->Sp / hb2::TILE_P) * ncls >= 2 * p->sm_count)
         return run_fp64_walk(p, cat0, ncls, levels);
@@ -1237,7 +1236,7 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
     const int Dp = pad_states(D);
     if (Dp < 0) return fail("state count %lld not supported (max 64)", (long long)D);
     int ndev = hb2_device_count();
-    if (ndev <= 0) return fail("no CUDA device visible: the B200 engine has no CPU fallback");
+    if (ndev <= 0) return fail("no CUDA device visible: the engine has no CPU fallback");
     if (device < 0 || device >= ndev) return fail("device %d out of range (%d visible)", device, ndev);
     CU(cudaSetDevice(device));
 
@@ -1308,11 +1307,10 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
                         per_sm, fa.numRegs, fa.sharedSizeBytes, wk_smem, dp.regsPerMultiprocessor, dp.sharedMemPerMultiprocessor, dp.sharedMemPerBlockOptin, dp.reservedSharedMemPerBlock);
             }
             CUP(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
-            {   // The occupancy API reports 1 CTA/SM for these kernels on B200 although ncu (launch__occupancy_limit_* = 2) and
-                // the measured residence of 256-CTA grids show two are co-resident: the lane count is planned from the
-                // resources.  Correctness does not depend on it: blocks are dispatched in index order and a lane only waits
-                // for lanes of its own (class, tile) slot -- adjacent block indices -- with time-bounded waits, so fewer
-                // resident CTAs than planned only make the pass slower (ADVICE r1).
+            {   // The lane count is planned from the resources (registers, shared memory) as well as from the occupancy API.
+                // Correctness does not depend on it: blocks are dispatched in index order and a lane only waits for lanes of
+                // its own (class, tile) slot -- adjacent block indices -- with time-bounded waits, so fewer resident CTAs
+                // than planned only make the pass slower.
                 cudaFuncAttributes fa;
                 CUP(cudaFuncGetAttributes(&fa, wk));
                 cudaDeviceProp dp; CUP(cudaGetDeviceProperties(&dp, device));
@@ -1323,7 +1321,7 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
             }
             if (const char *ov = getenv("HB2_WALK_CTAS_PER_SM")) per_sm = atoi(ov);      // bring-up override
             if (const char *ov = getenv("HB2_WALK_LANES")) p->walk_lane_cap = std::max(1, std::min(atoi(ov), 15));
-            p->walk_max_resident = std::min(per_sm, 2) * sms;          // TMEM: 256 of 512 columns per CTA -> at most 2 per SM
+            p->walk_max_resident = std::min(per_sm, 2) * sms;
             if (p->walk_max_resident < 1) p->use_walk = false;
             const size_t T = Sp / hb2::TC_TILE_P;
             p->walk_gen.assign((size_t)C * 2 * I, 0);   // matches the zero-filled conditional and exponent buffers

@@ -1,4 +1,4 @@
-// hb2_kernels_fp64.cuh -- fp64 CUDA kernels of the likelihood hot path (sm_100a).
+// hb2_kernels_fp64.cuh -- fp64 CUDA kernels of the likelihood hot path (sm_90a).
 //
 //   expm64_kernel / expm_small_kernel   P = exp(Q t) per (branch, rate class), one CTA per matrix
 //                                       (replaces _Matrix::Exponentiate, reference matrix.cpp:5537-5951)
@@ -1280,7 +1280,7 @@ __global__ void __launch_bounds__(128) prune_small_kernel(PruneArgs a, const int
 // minimum: one coalesced write and (at most) one read of Dp*8+4 bytes per (node, pattern) plus 4 B per leaf state.
 // grid = (Sp/128, classes), block = 128.  jobs = dirty internal indices, ascending (= post-order).
 // ------------------------------------------------------------------------------------------------
-// (Forcing 16 CTAs/SM for 4 states -- 32 registers, spills -- was slower: 1.39 vs 1.18 ms at 256 x 200k, r01s.)
+// (Forcing 16 CTAs/SM for 4 states -- 32 registers, spills -- was slower.)
 template <int DP>
 __global__ void __launch_bounds__(128) prune_small_walk_kernel(PruneArgs a, const int *__restrict__ jobs, int njobs) {
     // 16..32 states: the branch's P^T is staged in shared memory once per child (all threads of the CTA walk the same
@@ -1707,7 +1707,7 @@ __device__ __forceinline__ void bc_renorm(double *v, int D, int &e) {
 // The whole root -> parent(b) path in ONE launch: one CTA of Dp' = 64 (or 32) threads per (class, pattern), thread q owns
 // state q; vectors are exchanged through shared memory and a matrix column / row is read with consecutive threads on
 // consecutive addresses (the transposed table serves messages, its rows serve the outside propagation).  Replaces one
-// launch of bc_step_kernel per path node with a serial thread per pattern (17.7 ms at depth 48 on the north-star shape).
+// launch of bc_step_kernel per path node with a serial thread per pattern.
 //   path[i]      internal index of the i-th path node (root first), npath nodes
 //   sib_off[i]   range of its non-path children in sib[]
 //   down[i]      flat id of the path child below path[i] (the next path node), -1 for the last (whose child is the branch b)

@@ -8,10 +8,8 @@
 // ComputeTreeBlockByBranch (tree_evaluator.cpp:3556-4171) restricted to the nodes DetermineNodesForUpdate marked.
 //   * CTA = 4 warps x 8 patterns; the contraction C[pattern][parent] = sum_j X[pattern][j] * PT[j][parent] runs on the FP64
 //     tensor pipe (mma.sync.m8n8k4.f64): warp tile 8 x 64, 128 DMMA + 144 shared-memory loads per warp and contraction.
-//     History (profiles/r2p_, r2q_, r2r_lanes_trace_cta0.txt): the register-blocked DFMA product took 7.4 k cycles per
-//     contraction, this one 6.0 k (a warp issues one DMMA every ~45 cycles whatever its dependencies); splitting the
-//     parent states over two warps per 8 patterns (8 warps per CTA) brought the product to 4.0 k but cost more than that
-//     in the cross-warp row maximum and in barrier time (1.15 vs 0.99 ms per evaluation): not kept;
+//     A register-blocked DFMA product was slower; splitting the parent states over two warps per 8 patterns (8 warps per
+//     CTA) shortened the product but cost more than that in the cross-warp row maximum and in barrier time: not kept;
 //   * a thread owns ONE pattern (row 8*warp + lane/4) and 16 of its states (8j + 2*(lane%4) + {0,1}): renormalisation and
 //     the root dot product reduce over 4 lanes (two shuffles);
 //   * one P buffer + one X buffer = 53 KB, 128 threads: four CTAs per SM, so that the load / renormalise / publish

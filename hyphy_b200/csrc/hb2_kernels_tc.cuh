@@ -1,29 +1,30 @@
-// hb2_kernels_tc.cuh -- tcgen05 (5th-gen tensor core) pruning path for 33..64-state models (sm_100a only).
+// hb2_kernels_tc.cuh -- tensor-core (Hopper wgmma) pruning path for 33..64-state models (sm_90a).
 //
 // The 61-state codon update  parent[s][n] *= sum_k P[n][k] * child[s][k]  is a dense contraction batched over
-// patterns:  D[128 patterns][64 parent states] = X[128][64 child states] * P^T.  tcgen05 has no fp64 kind, so the
-// contraction runs as an error-compensated split in kind::tf32 with fp32 accumulation in TMEM:
+// patterns:  D[128 patterns][64 parent states] = X[128][64 child states] * P^T.  The tensor core has no fp64 tf32-class
+// kind, so the contraction runs as an error-compensated split in tf32 with fp32 accumulation:
 //        X = Xh + Xl,  P = Ph + Pl   (each part exactly representable in tf32, round-to-nearest splits)
 //        D = Xl*Ph + Xh*Pl + Xh*Ph   (the dropped Xl*Pl term is ~2^-22 relative)
 // All operands are non-negative, so there is no cancellation and the relative error of D is bounded by the
 // representation error of the splits (~2^-22) plus fp32 accumulation.  Conditionals are stored in fp32, renormalised
 // per (node, pattern) to max in [0.5,1) with an int32 binary exponent, so fp32 range is never an issue.
 //
-// Anchors.  The tensor core accumulates in fp32 with truncation (measured on B200: -8e-8 mean relative error per
-// K=64 contraction), which would bias lnL by ~-1.6e-7*|lnL|.  Conditional vectors are sharply peaked (1-3 codons carry
-// almost all the mass), so each thread pulls the entries >= 2^-6 of its row (at most 8, "anchors") out of the tensor
-// operand and multiplies them on the CUDA cores with round-to-nearest fp32 FMAs against fp32 rows of P^T while the
-// MMAs run; the tensor core only contracts the diffuse remainder, whose truncation bias is scaled down by its share.
+// Anchors.  The tensor core accumulates in fp32 without round-to-nearest, which would bias lnL by ~1e-7*|lnL| over a
+// codon tree.  Conditional vectors are sharply peaked (1-3 codons carry almost all the mass), so each thread pulls the
+// entries >= 2^-6 of its row (at most 8, "anchors") out of the tensor operand and multiplies them on the CUDA cores with
+// round-to-nearest fp32 FMAs against fp32 rows of P^T while the MMAs run; the tensor core only contracts the diffuse
+// remainder, whose rounding bias is scaled down by its share.
 //
-// Operand staging:
-//   A (= X, 128 x 64, K-major) comes from TENSOR MEMORY: each of the 128 threads owns one pattern (one TMEM lane),
-//     loads its fp32 row from HBM, splits it in registers and writes Xh / Xl with tcgen05.st (columns 64..191).
-//   B (= P, 64 x 64, K-major) comes from SHARED MEMORY in the canonical no-swizzle UMMA layout (8x16-byte core
-//     matrices; LBO = 1024 B between K chunks, SBO = 128 B between 8-row groups).  The expm stage writes P already
-//     split and tiled that way (pack_tc_kernel), so one 32 KB cp.async.bulk (TMA engine, mbarrier completion) per
-//     child stages Ph and Pl.
-//   D (128 x 64 fp32) lives in TMEM columns 0..63; it is read back with tcgen05.ld, one row per thread, multiplied
-//     into the running product of the parent held in registers.
+// Operand staging (wgmma.mma_async m64n64k8, one warpgroup = 128 threads per 64-pattern half of the tile):
+//   A (= X, 128 x 64, K-major) comes from SHARED MEMORY: each of the 128 threads owns one pattern, loads its fp32 row
+//     from HBM, splits it in registers and writes Xh / Xl into the canonical no-swizzle layout (8x16-byte core
+//     matrices; LBO = 2048 B between K chunks, SBO = 128 B between 8-row groups) -- the same [chunk][pattern][4] order
+//     the conditionals have in HBM, so a thread's stores are 16-byte and conflict-free.
+//   B (= P, 64 x 64, K-major) comes from SHARED MEMORY in the same layout (LBO = 1024 B, SBO = 128 B).  The expm stage
+//     writes P already split and tiled that way (pack_tc_kernel), so one 32 KB cp.async.bulk (TMA engine, mbarrier
+//     completion) per child stages Ph and Pl.
+//   D (128 x 64 fp32) is accumulated in registers (two m64 fragments per warpgroup thread), written to a shared row
+//     buffer and read back one row per thread, multiplied into the running product of the parent held in registers.
 //
 // Replaces (for D in 33..64) reference tree_evaluator.cpp:3875-4008 (_hy_mvp_blocked<61> + _hy_vvmult_sum<61>).
 #pragma once
@@ -33,12 +34,13 @@
 
 namespace hb2 {
 
-constexpr int TC_TILE_P = 128;                 // patterns per CTA (= UMMA M = TMEM lanes)
+constexpr int TC_TILE_P = 128;                 // patterns per CTA (two wgmma M = 64 halves)
 constexpr int TC_PB_FLOATS = 2 * 4096;         // per (class, branch): Ph tile + Pl tile in canonical layout
 constexpr int TC_PTF_ROW = 68;                 // floats per row of the fp32 P^T table (64 + 4 padding: 272-byte rows)
 constexpr int TC_PTF_FLOATS = 64 * TC_PTF_ROW; // per (class, branch)
-constexpr int TC_SMEM_BYTES = 2 * 32768 + 1024; // two B stages (one used for now; also caps residency at 2 CTAs/SM) + barriers
-constexpr uint32_t TC_TMEM_COLS = 256;         // D: 0..63, Xh: 64..127, Xl: 128..191 (allocations are powers of two)
+constexpr int TC_X_BYTES = 2 * 16 * 128 * 16;  // A operand: Xh | Xl, [16 chunks][128 patterns][4] fp32 each
+constexpr int TC_D_ROW = 68;                   // floats per row of the shared accumulator read-back buffer
+constexpr int TC_D_BYTES = 128 * TC_D_ROW * 4;
 constexpr int TC_MAX_ANCHORS = 8;              // per pattern and child (list capacity of the per-level and split-row kernels)
 constexpr int WALK_FAST_ANCHORS = 4;           // anchors handled by the unrolled fast path of the walk kernel; more go to a loop
 constexpr float TC_ANCHOR_THR = 0.015625f;     // 2^-6 (rows are normalised to max in [0.5,1))
@@ -103,24 +105,7 @@ __device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t by
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc], kind::tf32, M=128, N=64, K=8
-__device__ __forceinline__ void tc_mma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, {%5, %5, %5, %5}, p;\n\t"
-        "}" ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate), "r"(0u) : "memory");
-}
-// One lane of a converged warp (the CUTLASS issue idiom).  tcgen05.mma wants its operands in UNIFORM registers: issued
-// from a divergent `if (lane == 0)` ptxas wraps every UTCHMMA in an ELECT / R2UR.BROADCAST waterfall loop (~190 cycles per
-// instruction, profiles/r01j_mma_issue_timing.txt); issued by an elected lane inside a warp-uniform branch, with operands
-// that were broadcast by __shfl_sync, the instructions go out back to back (profiles/r02_mma_issue_uniform.txt).
+// One lane of a converged warp (used to issue the bulk copies from a warp-uniform branch).
 __device__ __forceinline__ uint32_t elect_one() {
     uint32_t pred;
     asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}" : "=r"(pred));
@@ -131,24 +116,60 @@ __device__ __forceinline__ uint32_t elect_one() {
 __device__ __forceinline__ float tf32_rn(float x) {
     return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
 }
-#define HB2_TMEM_ST16(taddr, r, o)                                                                                   \
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" \
-                 ::"r"(taddr), "r"(r[o + 0]), "r"(r[o + 1]), "r"(r[o + 2]), "r"(r[o + 3]), "r"(r[o + 4]), "r"(r[o + 5]),   \
-                 "r"(r[o + 6]), "r"(r[o + 7]), "r"(r[o + 8]), "r"(r[o + 9]), "r"(r[o + 10]), "r"(r[o + 11]),            \
-                 "r"(r[o + 12]), "r"(r[o + 13]), "r"(r[o + 14]), "r"(r[o + 15]) : "memory")
-#define HB2_TMEM_LD16(taddr, r, o)                                                                                   \
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];" \
-                 : "=r"(r[o + 0]), "=r"(r[o + 1]), "=r"(r[o + 2]), "=r"(r[o + 3]), "=r"(r[o + 4]), "=r"(r[o + 5]),      \
-                   "=r"(r[o + 6]), "=r"(r[o + 7]), "=r"(r[o + 8]), "=r"(r[o + 9]), "=r"(r[o + 10]), "=r"(r[o + 11]),    \
-                   "=r"(r[o + 12]), "=r"(r[o + 13]), "=r"(r[o + 14]), "=r"(r[o + 15])                                    \
-                 : "r"(taddr) : "memory")
-
-// UMMA shared-memory descriptor, SWIZZLE_NONE, K-major: start>>4 | (LBO>>4)<<16 | (SBO>>4)<<32 | version 1 @46
-__device__ __forceinline__ uint64_t make_b_desc(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)(1024u >> 4) << 16) | ((uint64_t)(128u >> 4) << 32) | (1ull << 46);
+// ---- warpgroup MMA (sm_90a) ----------------------------------------------------------------------------------------
+// Shared-memory matrix descriptor, no swizzle, K-major: start>>4 @0, LBO>>4 @16 (next 16-byte core-matrix column along
+// K), SBO>>4 @32 (next 8-row group along M or N).
+__device__ __forceinline__ uint64_t wg_desc(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
+    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(sbo >> 4) << 32);
 }
-// instruction descriptor: c=F32 (1<<4), a=b=TF32 (2<<7, 2<<10), K-major both, N=64 (8<<17), M=128 (8<<24)
-constexpr uint32_t TC_IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((64u >> 3) << 17) | ((128u >> 4) << 24);
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// generic-proxy stores to shared memory -> visible to the async proxy (the wgmma operand reads)
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// keeps the compiler from moving accumulator registers across the asynchronous MMA
+__device__ __forceinline__ void wg_pin(float (&d)[32]) {
+#pragma unroll
+    for (int i = 0; i < 32; i++) asm volatile("" : "+f"(d[i])::"memory");
+}
+// D[64 x 64] (+)= A[64 x 8] * B[64 x 8]^T, tf32 operands from shared memory, fp32 accumulator fragment d
+__device__ __forceinline__ void wg_mma_tf32(float (&d)[32], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1;\n\t"
+        "}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate) : "memory");
+}
+// Issues the 24 MMAs of one 64-pattern half m of the tile (small terms first: Xl*Ph, Xh*Pl, then Xh*Ph; 8 K-steps each)
+// into ONE accumulator.  xs: A buffer (TC_X_BYTES, Xh then Xl), pb: Ph then Pl (16 KB each).  The caller brackets the
+// issue with wg_fence() / wg_commit() and waits with wg_wait_all().
+__device__ __forceinline__ void wg_issue_tf32x3(float (&d)[32], uint32_t xs, uint32_t pb, int m) {
+    const uint32_t xh = xs + (uint32_t)m * 1024u, xl = xh + TC_X_BYTES / 2, ph = pb, pl = pb + 16384u;
+#pragma unroll
+    for (int kk = 0; kk < 8; kk++) wg_mma_tf32(d, wg_desc(xl + kk * 4096u, 2048u, 128u), wg_desc(ph + kk * 2048u, 1024u, 128u), kk > 0);
+#pragma unroll
+    for (int kk = 0; kk < 8; kk++) wg_mma_tf32(d, wg_desc(xh + kk * 4096u, 2048u, 128u), wg_desc(pl + kk * 2048u, 1024u, 128u), 1u);
+#pragma unroll
+    for (int kk = 0; kk < 8; kk++) wg_mma_tf32(d, wg_desc(xh + kk * 4096u, 2048u, 128u), wg_desc(ph + kk * 2048u, 1024u, 128u), 1u);
+}
+// Accumulator fragment of warp q (of its warpgroup), lane l -> rows row0 + 16q + l/4 (+8), columns 8j + 2(l%4) (+1) of
+// the shared [128][TC_D_ROW] read-back buffer.
+__device__ __forceinline__ void wg_store_d(float *Ds, const float (&d)[32], int row0, int q, int lane) {
+    float *r0 = Ds + (size_t)(row0 + 16 * q + (lane >> 2)) * TC_D_ROW + 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+        *reinterpret_cast<float2 *>(r0 + 8 * j) = make_float2(d[4 * j], d[4 * j + 1]);
+        *reinterpret_cast<float2 *>(r0 + 8 * TC_D_ROW + 8 * j) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+    }
+}
+// One pattern's split row (16 chunks of hi and lo, chunk q = states 4q..4q+3) into the A buffer.
+__device__ __forceinline__ void store_x_chunk(uint8_t *xs, int q, int pattern, const uint32_t *hi, const uint32_t *lo) {
+    *reinterpret_cast<uint4 *>(xs + (size_t)q * 2048 + pattern * 16) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+    *reinterpret_cast<uint4 *>(xs + TC_X_BYTES / 2 + (size_t)q * 2048 + pattern * 16) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+}
 
 // ------------------------------------------------------------------------------------------------------------------
 // PT (fp64, transposed) -> tensor-path operands: canonical hi/lo tiles of P and an fp32 copy of PT.  One CTA per slot.
@@ -203,7 +224,8 @@ __global__ void __launch_bounds__(256) mix_reduce_kernel(const double *__restric
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// Fused pruning update on tcgen05.  grid = (Sp/128, jobs, classes), block = 128 threads (thread t <-> pattern t).
+// Fused pruning update on the tensor core.  grid = (Sp/128, jobs, classes), block = 128 threads = one warpgroup
+// (thread t <-> pattern t).
 // ------------------------------------------------------------------------------------------------------------------
 // Power-of-two renormalisation of a pattern's 64 conditionals: max -> [0.5,1).  `force` = false only rescales when the
 // maximum has drifted below 2^-32 (cheap guard between the children of one node); true at the end of a node.
@@ -223,15 +245,17 @@ __device__ __forceinline__ void renorm_f32(float (&v)[64], int &ex, bool force =
     }
 }
 
-__global__ void __launch_bounds__(128, 2) prune64_tc_kernel(PruneTcArgs a, const int *__restrict__ jobs) {
+constexpr int TC_SMEM_BYTES = 32768 + TC_X_BYTES + TC_D_BYTES + TC_MAX_ANCHORS * 128 * 8 + 64;  // B, A, D, anchor lists, barrier
+
+__global__ void __launch_bounds__(128, 1) prune64_tc_kernel(PruneTcArgs a, const int *__restrict__ jobs) {
     extern __shared__ __align__(1024) uint8_t smem[];
     float *Bs = reinterpret_cast<float *>(smem);                         // [2][4096] Ph, Pl
-    uint64_t *bar_b = reinterpret_cast<uint64_t *>(smem + 2 * 32768);
-    uint64_t *bar_mma = bar_b + 1;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bar_b + 2);
-    int *s_ak = reinterpret_cast<int *>(smem + 32768);                   // [TC_MAX_ANCHORS][128] anchor state
-    float *s_av = reinterpret_cast<float *>(smem + 32768 + TC_MAX_ANCHORS * 128 * 4);   // [TC_MAX_ANCHORS][128] anchor value
-    const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
+    uint8_t *Xs = smem + 32768;                                          // A operand: Xh | Xl
+    float *Ds = reinterpret_cast<float *>(Xs + TC_X_BYTES);              // [128][TC_D_ROW] accumulator read-back
+    int *s_ak = reinterpret_cast<int *>(Xs + TC_X_BYTES + TC_D_BYTES);   // [TC_MAX_ANCHORS][128] anchor state
+    float *s_av = reinterpret_cast<float *>(s_ak + TC_MAX_ANCHORS * 128); // [TC_MAX_ANCHORS][128] anchor value
+    uint64_t *bar_b = reinterpret_cast<uint64_t *>(s_av + TC_MAX_ANCHORS * 128);
+    const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
     const int par = jobs[blockIdx.y];
     const int cat = a.cat0 + blockIdx.z;
     const size_t Sp = a.Sp;
@@ -239,20 +263,10 @@ __global__ void __launch_bounds__(128, 2) prune64_tc_kernel(PruneTcArgs a, const
 
     if (tid == 0) {
         mbar_init(bar_b, 1);
-        mbar_init(bar_mma, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TC_TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot, 0);
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(warp * 32) << 16);      // this warp's TMEM lane quarter
-    const uint64_t bdesc_hi = make_b_desc(__shfl_sync(0xffffffffu, smem_u32(Bs), 0));
-    const uint64_t bdesc_lo = make_b_desc(__shfl_sync(0xffffffffu, smem_u32(Bs + 4096), 0));
+    const uint32_t xs_addr = smem_u32(Xs), bs_addr = smem_u32(Bs);
 
     float v[64];
 #pragma unroll
@@ -298,15 +312,15 @@ __global__ void __launch_bounds__(128, 2) prune64_tc_kernel(PruneTcArgs a, const
                 mbar_expect_tx(bar_b, 32768u);
                 bulk_g2s(Bs, a.PB + slot * TC_PB_FLOATS, 32768u, bar_b);
             }
-            // (B) this thread's pattern row -> anchors out -> split -> TMEM (Xh at cols 64.., Xl at cols 128..)
+            // (B) this thread's pattern row -> anchors out -> split -> A operand in shared memory
             int na = 0;
             {
                 const float4 *xr = reinterpret_cast<const float4 *>(a.cond) + ((((size_t)cat * a.I + cin) * (Sp / 128) + blockIdx.x) * 16) * 128 + tid;
-                uint32_t hi[64], lo[64];
 #pragma unroll
                 for (int q = 0; q < 16; q++) {
                     const float4 x = xr[(size_t)q * 128];
                     float xs[4] = {x.x, x.y, x.z, x.w};
+                    uint32_t hi[4], lo[4];
 #pragma unroll
                     for (int u = 0; u < 4; u++) {
                         if (xs[u] >= TC_ANCHOR_THR && na < TC_MAX_ANCHORS) {
@@ -316,39 +330,27 @@ __global__ void __launch_bounds__(128, 2) prune64_tc_kernel(PruneTcArgs a, const
                             xs[u] = 0.f;
                         }
                         const float h = tf32_rn(xs[u]);
-                        hi[4 * q + u] = __float_as_uint(h);
-                        lo[4 * q + u] = __float_as_uint(xs[u] - h);
+                        hi[u] = __float_as_uint(h);
+                        lo[u] = __float_as_uint(xs[u] - h);
                     }
+                    store_x_chunk(Xs, q, tid, hi, lo);
                 }
-#pragma unroll
-                for (int o = 0; o < 64; o += 16) {
-                    HB2_TMEM_ST16(lane_addr + 64 + o, hi, o);
-                    HB2_TMEM_ST16(lane_addr + 128 + o, lo, o);
-                }
-                asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
             }
             ex += a.scal[((size_t)cat * a.I + cin) * Sp + s];
-            tc_fence_before();
-            __syncthreads();                 // A operand complete in TMEM; every thread is done reading the previous D
-            if (warp == 0) {
-                tc_fence_after();
-                mbar_wait(bar_b, phase, a.err);
-                if (elect_one()) {
-                    // small terms first: Xl*Ph, Xh*Pl, then Xh*Ph (8 K-steps of 8 each)
-#pragma unroll
-                    for (int kk = 0; kk < 8; kk++)
-                        tc_mma_tf32_ts(tmem_base, tmem_base + 128 + kk * 8, bdesc_hi + (uint64_t)(kk * 2 * 1024 >> 4), TC_IDESC, kk > 0);
-#pragma unroll
-                    for (int kk = 0; kk < 8; kk++)
-                        tc_mma_tf32_ts(tmem_base, tmem_base + 64 + kk * 8, bdesc_lo + (uint64_t)(kk * 2 * 1024 >> 4), TC_IDESC, 1u);
-#pragma unroll
-                    for (int kk = 0; kk < 8; kk++)
-                        tc_mma_tf32_ts(tmem_base, tmem_base + 64 + kk * 8, bdesc_hi + (uint64_t)(kk * 2 * 1024 >> 4), TC_IDESC, 1u);
-                    tc_commit(bar_mma);
-                }
-            }
-            __syncwarp();
-            // anchors on the CUDA cores while the tensor core works: acc[n] = sum_a x[k_a] * P[n][k_a], fp32 RN
+            fence_proxy_async();
+            __syncthreads();                 // A operand complete; every thread is done reading the previous D
+            mbar_wait(bar_b, phase, a.err);
+            float d0[32], d1[32];
+            wg_fence();
+            wg_issue_tf32x3(d0, xs_addr, bs_addr, 0);
+            wg_issue_tf32x3(d1, xs_addr, bs_addr, 1);
+            wg_commit();
+            wg_wait_all();
+            wg_pin(d0);
+            wg_pin(d1);
+            wg_store_d(Ds, d0, 0, warp, lane);
+            wg_store_d(Ds, d1, 64, warp, lane);
+            // anchors on the CUDA cores while the other warps store their fragments: acc[n] = sum_a x[k_a] * P[n][k_a], fp32 RN
             float acc[64];
 #pragma unroll
             for (int k = 0; k < 64; k++) acc[k] = 0.f;
@@ -366,15 +368,15 @@ __global__ void __launch_bounds__(128, 2) prune64_tc_kernel(PruneTcArgs a, const
                     }
                 }
             }
-            mbar_wait(bar_mma, phase, a.err);
-            tc_fence_after();
+            __syncthreads();                 // every row of D is in the read-back buffer
+            {
+                const float4 *drow = reinterpret_cast<const float4 *>(Ds + (size_t)tid * TC_D_ROW);
 #pragma unroll
-            for (int o = 0; o < 64; o += 16) {
-                uint32_t d[16];
-                HB2_TMEM_LD16(lane_addr + o, d, 0);
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                for (int k = 0; k < 16; k++) v[o + k] *= (__uint_as_float(d[k]) + acc[o + k]);
+                for (int q = 0; q < 16; q++) {
+                    const float4 dd = drow[q];
+                    v[4 * q] *= (dd.x + acc[4 * q]); v[4 * q + 1] *= (dd.y + acc[4 * q + 1]);
+                    v[4 * q + 2] *= (dd.z + acc[4 * q + 2]); v[4 * q + 3] *= (dd.w + acc[4 * q + 3]);
+                }
             }
             phase ^= 1u;
         }
@@ -399,11 +401,6 @@ __global__ void __launch_bounds__(128, 2) prune64_tc_kernel(PruneTcArgs a, const
             a.rootE[(size_t)cat * Sp + s] = ex;
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TC_TMEM_COLS) : "memory");
-    }
 }
 
 
@@ -425,11 +422,11 @@ __global__ void __launch_bounds__(128, 2) prune64_tc_kernel(PruneTcArgs a, const
 //
 // The pass is bound by (tree depth x per-step latency), so every operand of step i+1 is staged while step i runs:
 //   * per step, the branch's fp32 P^T table (64 rows x 256 B, padded to 272 B rows) and -- for a contraction -- its
-//     Ph|Pl UMMA tiles are bulk-copied (TMA engine, mbarrier tx completion) into a 2-stage shared-memory ring by thread 0
+//     Ph|Pl operand tiles are bulk-copied (TMA engine, mbarrier tx completion) into a 2-stage shared-memory ring by thread 0
 //     right after the step-begin barrier; leaf column gathers and anchor rows are then shared-memory reads;
 //   * the 32 KB conditional block of the next contraction is prefetched into L2 (cp.async.bulk.prefetch.L2) and the next
 //     leaf's state codes (or the awaited child's generation bit) into a register;
-//   * conditionals are stored tile-wise as [16 chunks][128 patterns][4 floats] (the K-major UMMA core-matrix order), so
+//   * conditionals are stored tile-wise as [16 chunks][128 patterns][4 floats] (the K-major core-matrix order), so
 //     thread t's 16-byte accesses are perfectly coalesced for both the producer and the consumer of a tile.
 // Step encoding: x = child id | WALK_WAIT | WALK_CHAIN | WALK_MUL ; y = job's node slot | STEP_FIRST | STEP_LAST.
 // ------------------------------------------------------------------------------------------------------------------
@@ -441,7 +438,7 @@ constexpr int STEP_FIRST = 1 << 28;
 constexpr int STEP_LAST = 1 << 29;
 constexpr int WALK_PT_ROW = TC_PTF_ROW;        // same padded rows in shared memory: one flat bulk copy stages the table
 constexpr int WALK_STAGE_FLOATS = 64 * WALK_PT_ROW + 8192;     // P^T table + Ph|Pl tiles
-constexpr int WALK_SMEM_BYTES = 2 * WALK_STAGE_FLOATS * 4 + TC_MAX_ANCHORS * 128 * 8 + 64;
+constexpr int WALK_SMEM_BYTES = 2 * WALK_STAGE_FLOATS * 4 + TC_X_BYTES + TC_D_BYTES + 64;   // ring, A, D, barriers
 
 struct WalkArgs {
     PruneTcArgs a;
@@ -476,35 +473,25 @@ __device__ __forceinline__ size_t cond_f4(int cat, int node, int tile, int q, in
     return ((((size_t)cat * I + node) * T + tile) * 16 + q) * 128 + t;
 }
 
-__global__ void __launch_bounds__(128, 2) prune64_tc_walk_kernel(WalkArgs w) {
+__global__ void __launch_bounds__(128, 1) prune64_tc_walk_kernel(WalkArgs w) {
     extern __shared__ __align__(1024) uint8_t smem[];
     const PruneTcArgs &a = w.a;
     float *stage_base = reinterpret_cast<float *>(smem);                           // 2 x [P^T table | Ph | Pl]
-    int *s_ak = reinterpret_cast<int *>(smem + 2 * WALK_STAGE_FLOATS * 4);          // [TC_MAX_ANCHORS][128]
-    float *s_av = reinterpret_cast<float *>(s_ak + TC_MAX_ANCHORS * 128);
-    uint64_t *bar_full = reinterpret_cast<uint64_t *>(s_av + TC_MAX_ANCHORS * 128); // [2]
-    uint64_t *bar_mma = bar_full + 2;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bar_mma + 1);
-    const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
+    uint8_t *Xs = smem + 2 * WALK_STAGE_FLOATS * 4;                                 // A operand: Xh | Xl
+    float *Ds = reinterpret_cast<float *>(Xs + TC_X_BYTES);                         // [128][TC_D_ROW] accumulator read-back
+    uint64_t *bar_full = reinterpret_cast<uint64_t *>(Xs + TC_X_BYTES + TC_D_BYTES); // [2]
+    const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
     const size_t Sp = a.Sp;
     float4 *cond4 = reinterpret_cast<float4 *>(a.cond);
 
     if (tid == 0) {
         mbar_init(bar_full, 1);
         mbar_init(bar_full + 1, 1);
-        mbar_init(bar_mma, 1);               // one tcgen05.commit per contraction (elected lane of warp 0)
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TC_TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot, 0);
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(warp * 32) << 16);
-    uint32_t n_step = 0, n_mma = 0;          // running counters: select ring stage / barrier parities
+    const uint32_t xs_addr = smem_u32(Xs);
+    uint32_t n_step = 0;                     // running counter: selects the ring stage and its barrier parity
     bool bailed = false;                     // a dependency wait timed out: stop waiting, the host reports the error
 
     const int r = blockIdx.x % w.K;
@@ -574,7 +561,7 @@ __global__ void __launch_bounds__(128, 2) prune64_tc_walk_kernel(WalkArgs w) {
         int2 st = __ldg(w.steps + i_begin);
         int2 nx = (i_begin + 1 < i_end) ? __ldg(w.steps + i_begin + 1) : make_int2(0, 0);
         __syncthreads();                      // previous (class, tile): every read of the ring is complete
-        if (warp == 3 && elect_one()) stage_step(cat, tile, st, n_step);     // warp 3 stages: warp 0 issues the MMAs
+        if (warp == 3 && elect_one()) stage_step(cat, tile, st, n_step);     // an elected lane of warp 3 stages
         // fetched one step ahead: a leaf's state code, or (contractions) the generation bit the child's words must carry
         auto step_aux = [&](int2 q) -> int {
             const int ch = q.x & WALK_ID_MASK;
@@ -701,12 +688,9 @@ __global__ void __launch_bounds__(128, 2) prune64_tc_walk_kernel(WalkArgs w) {
                     }
                     if (tr) trp[8] = clock64();
 #pragma unroll
-                    for (int o = 0; o < 64; o += 16) {
-                        HB2_TMEM_ST16(lane_addr + 64 + o, hi, o);
-                        HB2_TMEM_ST16(lane_addr + 128 + o, lo, o);
-                    }
+                    for (int q = 0; q < 16; q++) store_x_chunk(Xs, q, tid, hi + 4 * q, lo + 4 * q);
                     if (tr) trp[9] = clock64();
-                    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
+                    fence_proxy_async();
                     if (tr) trp[10] = clock64();
                 }
                 unsigned long long amask = (unsigned long long)(am0 | (am1 << 16)) | ((unsigned long long)(am2 | (am3 << 16)) << 32);
@@ -724,33 +708,20 @@ __global__ void __launch_bounds__(128, 2) prune64_tc_walk_kernel(WalkArgs w) {
                     }
                 }
                 if (tr) trp[3] = clock64();
-                tc_fence_before();
-                __syncthreads();             // (2) A operand complete in TMEM; every thread is done reading the previous D
+                __syncthreads();             // (2) A operand complete in shared memory; every thread is done reading the previous D
                 if (tr) trp[4] = clock64();
-                if (warp == 0) {
-                    // 24 tcgen05.mma (small terms first: Xl*Ph, Xh*Pl, Xh*Ph; 8 K-steps of 8 each) into ONE accumulator
-                    // (TMEM columns 0..63), issued back to back by the elected lane of warp 0 with uniform operands: the
-                    // chain is bound by the tensor pipe (32 cycles per M128 N64 K8 instruction), not by the issue.
-                    tc_fence_after();
-                    mbar_wait(bar_full + (n_step & 1u), (n_step >> 1) & 1u, a.err);
-                    if (tr) trp[5] = clock64();
-                    const uint32_t baddr = __shfl_sync(0xffffffffu, smem_u32(tab + 64 * WALK_PT_ROW), 0);
-                    const uint64_t bdesc_hi = make_b_desc(baddr);
-                    const uint64_t bdesc_lo = make_b_desc(baddr + 4096 * 4);
-                    if (elect_one()) {
-#pragma unroll
-                        for (int kk = 0; kk < 8; kk++) tc_mma_tf32_ts(tmem_base, tmem_base + 128 + kk * 8, bdesc_hi + (uint64_t)(kk * 2 * 1024 >> 4), TC_IDESC, kk > 0);
-#pragma unroll
-                        for (int kk = 0; kk < 8; kk++) tc_mma_tf32_ts(tmem_base, tmem_base + 64 + kk * 8, bdesc_lo + (uint64_t)(kk * 2 * 1024 >> 4), TC_IDESC, 1u);
-#pragma unroll
-                        for (int kk = 0; kk < 8; kk++) tc_mma_tf32_ts(tmem_base, tmem_base + 64 + kk * 8, bdesc_hi + (uint64_t)(kk * 2 * 1024 >> 4), TC_IDESC, 1u);
-                        tc_commit(bar_mma);
-                    }
-                }
-                __syncwarp();
+                // 48 wgmma (per 64-pattern half: Xl*Ph, Xh*Pl, Xh*Ph; 8 K-steps of 8 each) into one accumulator per half,
+                // issued by the whole warpgroup once the branch's operands have landed
+                mbar_wait(bar_full + (n_step & 1u), (n_step >> 1) & 1u, a.err);
+                if (tr) trp[5] = clock64();
+                const uint32_t baddr = smem_u32(tab + 64 * WALK_PT_ROW);
+                float d0[32], d1[32];
+                wg_fence();
+                wg_issue_tf32x3(d0, xs_addr, baddr, 0);
+                wg_issue_tf32x3(d1, xs_addr, baddr, 1);
+                wg_commit();
                 // anchors on the CUDA cores while the tensor core works (rows of the P^T table in shared memory)
                 float acc[64];
-                mbar_wait(bar_full + (n_step & 1u), (n_step >> 1) & 1u, a.err);
                 {   // first anchor (nearly every row has one: its maximum is >= 0.5): a product, no zero-fill + FMA
                     const float xv = ak[0] >= 0 ? fabsf(av[0]) : 0.f;
                     const float4 *row = reinterpret_cast<const float4 *>(tab + max(ak[0], 0) * WALK_PT_ROW);
@@ -785,18 +756,22 @@ __global__ void __launch_bounds__(128, 2) prune64_tc_walk_kernel(WalkArgs w) {
                         acc[4 * q + 2] = fmaf(xv, rr.z, acc[4 * q + 2]); acc[4 * q + 3] = fmaf(xv, rr.w, acc[4 * q + 3]);
                     }
                 }
-                mbar_wait(bar_mma, n_mma & 1u, a.err);
+                wg_wait_all();
+                wg_pin(d0);
+                wg_pin(d1);
                 if (tr) trp[6] = clock64();
-                tc_fence_after();
+                wg_store_d(Ds, d0, 0, warp, lane);
+                wg_store_d(Ds, d1, 64, warp, lane);
+                __syncthreads();             // (3) every row of D is in the read-back buffer
+                {
+                    const float4 *drow = reinterpret_cast<const float4 *>(Ds + (size_t)tid * TC_D_ROW);
 #pragma unroll
-                for (int o = 0; o < 64; o += 16) {
-                    uint32_t d[16];
-                    HB2_TMEM_LD16(lane_addr + o, d, 0);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                    for (int k = 0; k < 16; k++) v[o + k] *= (__uint_as_float(d[k]) + acc[o + k]);
+                    for (int q = 0; q < 16; q++) {
+                        const float4 dd = drow[q];
+                        v[4 * q] *= (dd.x + acc[4 * q]); v[4 * q + 1] *= (dd.y + acc[4 * q + 1]);
+                        v[4 * q + 2] *= (dd.z + acc[4 * q + 2]); v[4 * q + 3] *= (dd.w + acc[4 * q + 3]);
+                    }
                 }
-                n_mma++;
             }
             if ((flags & STEP_LAST) && a.L + par == a.forced_node) {   // pinned internal node (never a side-product slot)
                 const int f = __ldg(a.forced + s);
@@ -829,23 +804,17 @@ __global__ void __launch_bounds__(128, 2) prune64_tc_walk_kernel(WalkArgs w) {
         }
     }
     if (w.trace_cta_times && tid == 0) w.trace_cta_times[(size_t)blockIdx.x * 4 + 2] = clock64();
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TC_TMEM_COLS) : "memory");
-    }
 }
 
 
 // ------------------------------------------------------------------------------------------------------------------
 // prune64_tc_walk2_kernel: the same pass with TWO threads per pattern (256-thread CTA).
 //
-// The 128-thread kernel above is bound by each warp's own instruction stream (~830 instructions per contraction step at
-// ~6 cycles each, two warps per scheduler: profiles/r2e_prune64_tc_walk_kernel.json) -- every thread carries all 64 states
-// of its pattern through the split, the anchor products and the read-back.  Here warp w (0..7) serves TMEM lane quarter
-// w % 4 (hardware rule for tcgen05.ld/st) and state half h = w / 4: thread (pattern t, half h) owns states 32h..32h+31 of
-// pattern t everywhere (conditional chunks 8h..8h+7, TMEM operand columns 32h.., accumulator columns 32h..), so the serial
-// stream per step halves while the tile, the MMAs, the staging ring and the plan stay exactly the same.
+// The 128-thread kernel above carries all 64 states of a pattern per thread through the split, the anchor products and
+// the read-back.  Here warp w (0..7) belongs to warpgroup h = w / 4, which owns state half h: thread (pattern t, half h)
+// owns states 32h..32h+31 of pattern t everywhere (conditional chunks 8h..8h+7, accumulator read-back columns 32h..), so
+// the serial stream per step halves while the tile, the staging ring and the plan stay exactly the same.  For the MMAs
+// warpgroup h contracts the 64-pattern half h of the tile (patterns 64h..64h+63, all 64 parent states).
 //   * anchors: each thread publishes the anchor mask of ITS half in shared memory before barrier (2); afterwards both threads
 //     of a pattern enumerate the combined 64-bit mask (values re-read from the child's block in L2, as in the first kernel)
 //     and accumulate their own 32 parent states;
@@ -858,7 +827,7 @@ __global__ void __launch_bounds__(128, 2) prune64_tc_walk_kernel(WalkArgs w) {
 // ------------------------------------------------------------------------------------------------------------------
 constexpr int WALK2_XBYTES = 2 * 128 * 4 /* anchor masks */ + 2 * 128 * 4 /* half maxima */ + 2 * 128 * 4 /* half exponents */ +
                              2 * 128 * 8 /* root partials */;
-constexpr int WALK2_SMEM_BYTES = 2 * WALK_STAGE_FLOATS * 4 + WALK2_XBYTES + 64;
+constexpr int WALK2_SMEM_BYTES = 2 * WALK_STAGE_FLOATS * 4 + TC_X_BYTES + TC_D_BYTES + WALK2_XBYTES + 64;
 
 __device__ __forceinline__ void renorm_half(float (&v)[32], int &ex) {     // guard inside a job: own half only, rarely taken
     float m0 = v[0], m1 = v[1], m2 = v[2], m3 = v[3];
@@ -874,38 +843,30 @@ __device__ __forceinline__ void renorm_half(float (&v)[32], int &ex) {     // gu
     }
 }
 
-__global__ void __launch_bounds__(256, 2) prune64_tc_walk2_kernel(WalkArgs w) {
+__global__ void __launch_bounds__(256, 1) prune64_tc_walk2_kernel(WalkArgs w) {
     extern __shared__ __align__(1024) uint8_t smem[];
     const PruneTcArgs &a = w.a;
     float *stage_base = reinterpret_cast<float *>(smem);                           // 2 x [P^T table | Ph | Pl]
-    uint32_t *s_am = reinterpret_cast<uint32_t *>(smem + 2 * WALK_STAGE_FLOATS * 4);   // [2][128] anchor masks of the two halves
+    uint8_t *Xs = smem + 2 * WALK_STAGE_FLOATS * 4;                                 // A operand: Xh | Xl
+    float *Ds = reinterpret_cast<float *>(Xs + TC_X_BYTES);                         // [128][TC_D_ROW] accumulator read-back
+    uint32_t *s_am = reinterpret_cast<uint32_t *>(Xs + TC_X_BYTES + TC_D_BYTES);   // [2][128] anchor masks of the two halves
     float *s_mx = reinterpret_cast<float *>(s_am + 2 * 128);                        // [2][128]
     int *s_ex = reinterpret_cast<int *>(s_mx + 2 * 128);                            // [2][128]
     double *s_rt = reinterpret_cast<double *>(s_ex + 2 * 128);                      // [2][128]
     uint64_t *bar_full = reinterpret_cast<uint64_t *>(s_rt + 2 * 128);              // [2]
-    uint64_t *bar_mma = bar_full + 2;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bar_mma + 1);
-    const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
-    const int lq = warp & 3, h = warp >> 2, t = 32 * lq + (tid & 31);              // TMEM lane quarter, state half, pattern in tile
+    const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
+    const int lq = warp & 3, h = warp >> 2, t = 32 * lq + lane;                     // warp in warpgroup, state half, pattern in tile
     const size_t Sp = a.Sp;
     float4 *cond4 = reinterpret_cast<float4 *>(a.cond);
 
     if (tid == 0) {
         mbar_init(bar_full, 1);
         mbar_init(bar_full + 1, 1);
-        mbar_init(bar_mma, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TC_TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot, 0);
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(lq * 32) << 16);
-    uint32_t n_step = 0, n_mma = 0;
+    const uint32_t xs_addr = smem_u32(Xs);
+    uint32_t n_step = 0;
     bool bailed = false;
 
     const int r = blockIdx.x % w.K;
@@ -1065,49 +1026,36 @@ __global__ void __launch_bounds__(256, 2) prune64_tc_walk2_kernel(WalkArgs w) {
                     }
                     ex += (int)sc >> 1;
                 }
-                // split in two 16-column pieces (registers): anchors out, tf32 hi / lo -> TMEM columns 64 + 32h.. / 128 + 32h..
+                // split in 4-state chunks (registers): anchors out, tf32 hi / lo -> A operand chunks 8h..8h+7 of pattern t
 #pragma unroll
-                for (int o = 0; o < 32; o += 16) {
-                    uint32_t hi[16], lo[16];
+                for (int q = 0; q < 8; q++) {
+                    uint32_t hi[4], lo[4];
 #pragma unroll
-                    for (int k = 0; k < 16; k++) {
-                        const float xv = xa[o + k];
+                    for (int u = 0; u < 4; u++) {
+                        const float xv = xa[4 * q + u];
                         const bool big = xv >= w.anchor_thr;
-                        if (big) am |= 1u << (o + k);
+                        if (big) am |= 1u << (4 * q + u);
                         const float x = big ? 0.f : xv;
                         const float hh = tf32_rn(x);
-                        hi[k] = __float_as_uint(hh);
-                        lo[k] = __float_as_uint(x - hh);
+                        hi[u] = __float_as_uint(hh);
+                        lo[u] = __float_as_uint(x - hh);
                     }
-                    HB2_TMEM_ST16(lane_addr + 64 + 32 * h + o, hi, 0);
-                    HB2_TMEM_ST16(lane_addr + 128 + 32 * h + o, lo, 0);
+                    store_x_chunk(Xs, 8 * h + q, t, hi, lo);
                 }
                 if (tr) trp[8] = clock64();
                 s_am[h * 128 + t] = am;                                              // for both threads of the pattern
                 if (tr) trp[9] = clock64();
-                asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
+                fence_proxy_async();
                 if (tr) { trp[10] = clock64(); trp[3] = trp[10]; }
-                tc_fence_before();
-                __syncthreads();             // (2) A operand complete in TMEM, anchor lists published; previous D consumed
+                __syncthreads();             // (2) A operand complete in shared memory, anchor lists published; previous D consumed
                 if (tr) trp[4] = clock64();
-                if (warp == 0) {
-                    tc_fence_after();
-                    mbar_wait(bar_full + (n_step & 1u), (n_step >> 1) & 1u, a.err);
-                    if (tr) trp[5] = clock64();
-                    const uint32_t baddr = __shfl_sync(0xffffffffu, smem_u32(tab + 64 * WALK_PT_ROW), 0);
-                    const uint64_t bdesc_hi = make_b_desc(baddr);
-                    const uint64_t bdesc_lo = make_b_desc(baddr + 4096 * 4);
-                    if (elect_one()) {
-#pragma unroll
-                        for (int kk = 0; kk < 8; kk++) tc_mma_tf32_ts(tmem_base, tmem_base + 128 + kk * 8, bdesc_hi + (uint64_t)(kk * 2 * 1024 >> 4), TC_IDESC, kk > 0);
-#pragma unroll
-                        for (int kk = 0; kk < 8; kk++) tc_mma_tf32_ts(tmem_base, tmem_base + 64 + kk * 8, bdesc_lo + (uint64_t)(kk * 2 * 1024 >> 4), TC_IDESC, 1u);
-#pragma unroll
-                        for (int kk = 0; kk < 8; kk++) tc_mma_tf32_ts(tmem_base, tmem_base + 64 + kk * 8, bdesc_hi + (uint64_t)(kk * 2 * 1024 >> 4), TC_IDESC, 1u);
-                        tc_commit(bar_mma);
-                    }
-                }
-                __syncwarp();
+                // warpgroup h: the 24 wgmma of pattern half h, issued once the branch's operands have landed
+                mbar_wait(bar_full + (n_step & 1u), (n_step >> 1) & 1u, a.err);
+                if (tr) trp[5] = clock64();
+                float d[32];
+                wg_fence();
+                wg_issue_tf32x3(d, xs_addr, smem_u32(tab + 64 * WALK_PT_ROW), h);
+                wg_commit();
                 // anchors of BOTH halves on the CUDA cores while the tensor core works: this thread's 32 parent states.  Values
                 // are re-read from the child's block in L2 (loaded, or stored by the two threads of this pattern a moment ago --
                 // barrier (2) made those stores visible), a handful of loads in flight under the MMAs.
@@ -1126,7 +1074,6 @@ __global__ void __launch_bounds__(256, 2) prune64_tc_walk2_kernel(WalkArgs w) {
                     }
                 }
                 float acc[32];
-                mbar_wait(bar_full + (n_step & 1u), (n_step >> 1) & 1u, a.err);
                 const float *tabh = tab + 32 * h;
                 {
                     const float xv = ak[0] >= 0 ? fabsf(av[0]) : 0.f;
@@ -1162,18 +1109,20 @@ __global__ void __launch_bounds__(256, 2) prune64_tc_walk2_kernel(WalkArgs w) {
                         acc[4 * q + 2] = fmaf(xv, rr.z, acc[4 * q + 2]); acc[4 * q + 3] = fmaf(xv, rr.w, acc[4 * q + 3]);
                     }
                 }
-                mbar_wait(bar_mma, n_mma & 1u, a.err);
+                wg_wait_all();
+                wg_pin(d);
                 if (tr) trp[6] = clock64();
-                tc_fence_after();
+                wg_store_d(Ds, d, 64 * h, lq, lane);
+                __syncthreads();             // (3) every row of D is in the read-back buffer
+                {
+                    const float4 *drow = reinterpret_cast<const float4 *>(Ds + (size_t)t * TC_D_ROW + 32 * h);
 #pragma unroll
-                for (int o = 0; o < 32; o += 16) {
-                    uint32_t d[16];
-                    HB2_TMEM_LD16(lane_addr + 32 * h + o, d, 0);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                    for (int k = 0; k < 16; k++) v[o + k] *= (__uint_as_float(d[k]) + acc[o + k]);
+                    for (int q = 0; q < 8; q++) {
+                        const float4 dd = drow[q];
+                        v[4 * q] *= (dd.x + acc[4 * q]); v[4 * q + 1] *= (dd.y + acc[4 * q + 1]);
+                        v[4 * q + 2] *= (dd.z + acc[4 * q + 2]); v[4 * q + 3] *= (dd.w + acc[4 * q + 3]);
+                    }
                 }
-                n_mma++;
             }
             n_step++;
             if (!(flags & STEP_LAST)) {
@@ -1233,11 +1182,6 @@ __global__ void __launch_bounds__(256, 2) prune64_tc_walk2_kernel(WalkArgs w) {
         }
     }
     if (w.trace_cta_times && tid == 0) w.trace_cta_times[(size_t)blockIdx.x * 4 + 2] = clock64();
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TC_TMEM_COLS) : "memory");
-    }
 }
 
 }  // namespace hb2

@@ -1,5 +1,5 @@
 /*
- * hyphy_b200.h -- C ABI of the B200-native phylogenetic-likelihood engine (libhyphy_b200.so).
+ * hyphy_b200.h -- C ABI of the GPU-native (H100, sm_90a) phylogenetic-likelihood engine (libhyphy_b200.so).
  *
  * This is the drop-in boundary behind the reference's `_LikelihoodFunction::ComputeBlock`
  * (veg/hyphy src/core/likefunc.cpp:10783-11289).  The reference has no plugin interface for its evaluator; the
@@ -191,7 +191,7 @@ int hb2_comm_gather_sites(hb2_partition *p, const double *siteL, const int64_t *
 /* Pair of SetupLFCaches in DeleteCaches (likefunc.cpp:10556-10601). */
 void hb2_destroy(hb2_partition *p);
 
-/* Host-side planner of the tcgen05 pruning pass, callable WITHOUT a GPU (tests/test_planner.py): for a tree (same
+/* Host-side planner of the tensor-core pruning pass, callable WITHOUT a GPU (tests/test_planner.py): for a tree (same
  * flatParents as hb2_create), a dirty set given as hb2_evaluate's updateNodes (NULL or nUpdate < 0 = whole tree) and a
  * number of lanes (1..15), returns the lanes' step lists exactly as the kernel receives them: laneStart[lanes+1] and
  * 2 ints per step -- child id | HB2_STEP_WAIT (1<<30: produced by another lane) | HB2_STEP_CHAIN (1<<29: produced by
@@ -205,7 +205,7 @@ int hb2_plan_walk(int64_t L, int64_t I, const int64_t *flatParents, int64_t nUpd
 /* Introspection for tests/bench: kernel launches issued so far by this partition, and device pointers/timing. */
 int64_t hb2_launch_count(const hb2_partition *p);
 /* 0: fp64 pruning kernels (4/20-state register kernels, or HB2_FLAG_FORCE_FP64);
- * 1: tcgen05 tensor-core pruning, error-compensated 3xTF32 split with fp32 conditionals (33..64 states). */
+ * 1: tensor-core (wgmma) pruning, error-compensated 3xTF32 split with fp32 conditionals (33..64 states). */
 int hb2_precision_mode(const hb2_partition *p);
 /* Name of the pruning kernel this partition launches, and the kernel launches per evaluation of the three stages
  * {expm, pruning, root reduction} as counted during the last hb2_time_resident (bench.py's roofline object). */

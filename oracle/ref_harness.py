@@ -159,7 +159,7 @@ def run_reference(w: synth.Workload, n_evals: int = 0, threads: int = 0, per_sit
                   env_extra: dict | None = None, ancestors: bool = False) -> dict:
     """Run the reference binary on `w`.  Returns {"lnL", "site_lnL" (np array, alignment order) or None,
     "loop_seconds" (wall time between LOOP_BEGIN and LOOP_END, measured on this side of the pipe), "wall"}.
-    binary: another HyPhy executable fed the same script -- the PATCHED host (host/_build/hyphy) in tests/test_host_binding.py."""
+    binary: another HyPhy executable fed the same script -- the PATCHED host (oracle/_ref/host/hyphy) in tests/test_host_binding.py."""
     if binary is None and not have_reference():
         raise RuntimeError(f"reference binary missing: {REF_BIN} (build with make -f oracle/Makefile.ref)")
     tmp = workdir or tempfile.mkdtemp(prefix="hb2ref_")

@@ -1,7 +1,7 @@
 """GPU suite (pytest -m gpu): the CUDA path, called through the C ABI, against the oracle and the reference's
 golden vectors.  north_star's contract is |dlnL| < 1e-6*|lnL|.  Two precisions are exercised:
   fp64 : HB2_FLAG_FORCE_FP64 -- fp64 kernels everywhere, held to 1e-10 (parity reference on the device)
-  tc   : default flags -- 33..64-state models run on tcgen05 (error-compensated 3xTF32 + anchors, fp32 conditionals),
+  tc   : default flags -- 33..64-state models run on the tensor cores (wgmma, error-compensated 3xTF32 + anchors, fp32 conditionals),
          held to 1e-7 (10x inside the contract); other state counts use the fp64 register kernels in both modes.
 Measured errors are appended to gpurun_out/parity_errors.jsonl for DESIGN.md."""
 import json
@@ -701,7 +701,7 @@ def test_more_class_tile_pairs_than_resident_ctas(mode):
 
 
 def test_tensor_path_against_fp64_path_deep_and_wide():
-    """The tcgen05 path against the fp64 kernels on the same device, on shapes chosen to stress error accumulation
+    """The tensor-core path against the fp64 kernels on the same device, on shapes chosen to stress error accumulation
     (500 taxa: ~1000 contractions per pattern) and short/long branch mixes.  Contract: 1e-6; required here: 1e-7."""
     for (taxa, codons, C, mean_t) in [(500, 96, 4, 0.05), (200, 128, 1, 0.005), (64, 256, 4, 0.3)]:
         w = synth.codon_workload(taxa, codons, C, seed=77, mean_t=mean_t)

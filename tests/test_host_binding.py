@@ -1,6 +1,6 @@
-"""GPU suite, part 2: the REAL boundary.  host/_build/hyphy is a build copy of the reference with the hook calls of
-host/apply_hooks.py inserted and host/hb2_hyphy_hooks.cpp linked against libhyphy_b200.so (built here by
-__graft_entry__.build(); the binary travels to the GPU box).  The same HBL scripts that produced the golden fixtures with
+"""GPU suite, part 2: the REAL boundary.  oracle/_ref/host/hyphy is a build copy of the reference with the hook calls of
+host/apply_hooks.py inserted and host/hb2_hyphy_hooks.cpp linked against libhyphy_b200.so (built by
+__graft_entry__.build() where the reference sources exist; oracle/_ref/ is carried to the GPU machine with the tree).  The same HBL scripts that produced the golden fixtures with
 the UNMODIFIED reference binary are fed to the patched binary: `LFCompute`, `ConstructCategoryMatrix`, `Optimize` now run
 on the engine, behind `_LikelihoodFunction::ComputeBlock`, with no change to the batch files."""
 import json
@@ -17,13 +17,18 @@ from tests import golden_cases as gc
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HOST_BIN = os.path.join(ROOT, "host", "_build", "hyphy")
+HOST_DIR = os.path.join(ROOT, "oracle", "_ref", "host")
+HOST_BIN = os.path.join(HOST_DIR, "hyphy")
+# what the UNMODIFIED reference binary printed for the evaluation stream and the ancestral reconstructions below
+# (tools/make_golden.py --runs)
+with open(os.path.join(ROOT, "tests", "golden", "reference_runs.json")) as _f:
+    REFERENCE_RUNS = json.load(_f)
 MODES = {"fp64": ({}, 1e-10, 1e-8), "tc": ({"HYPHY_B200_TC": "1"}, 1e-7, 1e-5)}     # the host's default is fp64 (see hb2_hyphy_hooks.h)
 
 
 @pytest.fixture(scope="module", autouse=True)
 def _need_host():
-    assert os.path.isfile(HOST_BIN), f"{HOST_BIN} is missing: run __graft_entry__.build() where /root/reference exists"
+    assert os.path.isfile(HOST_BIN), f"{HOST_BIN} is missing: run __graft_entry__.build() where the reference sources exist"
 
 
 def _tol(w, mode):
@@ -50,9 +55,10 @@ def test_patched_host_reproduces_reference_fixture(name, mode):
 def test_patched_host_evaluation_stream_and_partial_updates():
     """The bench's evaluation stream (one global parameter perturbed per evaluation -> every matrix re-exponentiated on the
     device) through the patched binary: final lnL of the loop equals the unmodified binary's to 1e-7 relative."""
-    w, g = gc.load("mg94_30x100_c4_ambig")
-    a = rh.run_reference(w, n_evals=5, n_warm=1, per_site=False)
-    b = rh.run_reference(w, n_evals=5, n_warm=1, per_site=False, binary=HOST_BIN, env_extra={"HYPHY_B200_VERBOSE": "1", "HYPHY_B200_TC": "1"})
+    a = REFERENCE_RUNS["evaluation_stream"]
+    w, g = gc.load(a["case"])
+    b = rh.run_reference(w, n_evals=a["n_evals"], n_warm=a["n_warm"], per_site=False, binary=HOST_BIN,
+                         env_extra={"HYPHY_B200_VERBOSE": "1", "HYPHY_B200_TC": "1"})
     assert abs(b["loop_lnL"] - a["loop_lnL"]) <= 1e-7 * abs(a["loop_lnL"])
     assert abs(b["lnL"] - g["lnL"]) <= 1e-7 * abs(g["lnL"])
 
@@ -63,7 +69,7 @@ def test_patched_host_ancestral_reconstruction_matches_reference(name):
     rate variation, the class assignments -- on the HOST; with the engine they are copied back from the device first
     (hb2_hooks::materialize).  Same ancestral sequences as the unmodified binary, in both precisions."""
     w, g = gc.load(name)
-    ref = rh.run_reference(w, ancestors=True, per_site=False)
+    ref = {"ancestors": REFERENCE_RUNS["ancestors"][name]}
     assert ref["ancestors"] and all(len(a) == len(ref["ancestors"][0]) for a in ref["ancestors"])
     for mode in MODES:
         r = rh.run_reference(w, ancestors=True, per_site=False, binary=HOST_BIN, env_extra=dict(MODES[mode][0], HYPHY_B200_VERBOSE="1"))
@@ -80,9 +86,11 @@ def test_patched_host_reference_ancestor_batch_file():
     """The reference's own Ancestors/NucAncestors.bf compares the joint ML reconstruction with sequences stored in the file
     ([OK: ML SEQUENCE RECONSTRUCTION]); its later sections fail with the unmodified binary as well and are not judged."""
     import tempfile
-    test = os.path.join(ROOT, "host", "_build", "hbltests", "Ancestors", "NucAncestors.bf")
+    from host import regress
+    work = regress.work_tree()
+    test = os.path.join(work, "hbltests", "Ancestors", "NucAncestors.bf")
     tmp = tempfile.mkdtemp(prefix="hb2anc_")
-    pr = subprocess.run([HOST_BIN, f"LIBPATH={os.path.join(ROOT, 'host', '_build', 'res')}", test], cwd=tmp, stdin=subprocess.DEVNULL,
+    pr = subprocess.run([HOST_BIN, f"LIBPATH={os.path.join(work, 'res')}", test], cwd=tmp, stdin=subprocess.DEVNULL,
                         stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=dict(os.environ, HYPHY_B200_VERBOSE="1"), timeout=600)
     assert "partition 0 on device" in pr.stdout
     assert "[OK: ML SEQUENCE RECONSTRUCTION]" in pr.stdout and "MISMATCHED" not in pr.stdout, pr.stdout[-1500:]
@@ -94,10 +102,6 @@ def test_patched_host_runs_reference_regression_batch_files():
     same fitted log-likelihoods as the unmodified reference binary recorded in tests/golden/hbltests_expected.json."""
     pr = subprocess.run([sys.executable, os.path.join(ROOT, "host", "regress.py"), "check"], stdout=subprocess.PIPE, text=True)
     rows = [json.loads(l) for l in pr.stdout.splitlines() if l.startswith("{")]
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    with open(os.path.join(ROOT, "gpurun_out", "host_regression.jsonl"), "w") as f:
-        for r in rows:
-            f.write(json.dumps(r) + "\n")
     assert rows, pr.stdout[-2000:]
-    bad = [r["test"] for r in rows if not r["ok"]]
-    assert not bad, bad
+    bad = [r for r in rows if not r["ok"]]
+    assert not bad, [(r["test"], r["got"]["verdict"], r["got"]["lnL"], r["got"]["tail"][-300:]) for r in bad]

@@ -1,4 +1,4 @@
-"""CPU suite: the patched host binary (host/_build/hyphy, built by __graft_entry__.build() where /root/reference exists)
+"""CPU suite: the patched host binary (oracle/_ref/host/hyphy, built by __graft_entry__.build() where the reference sources exist)
 without a GPU -- what must keep working, and what must fail loudly.  Skipped when the binary is not there."""
 import os
 import subprocess
@@ -11,10 +11,10 @@ from oracle import ref_harness as rh
 from tests import golden_cases as gc
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HOST_BIN = os.path.join(ROOT, "host", "_build", "hyphy")
-BUILD = os.path.join(ROOT, "host", "_build")
+BUILD = os.path.join(ROOT, "oracle", "_ref", "host")
+HOST_BIN = os.path.join(BUILD, "hyphy")
 
-pytestmark = pytest.mark.skipif(not os.path.isfile(HOST_BIN), reason="patched host binary not built (needs /root/reference)")
+pytestmark = pytest.mark.skipif(not os.path.isfile(HOST_BIN), reason="patched host binary not built (needs the reference sources)")
 
 
 def _no_gpu_env(**extra):
@@ -45,7 +45,10 @@ def test_two_sequence_analysis_stays_on_the_host_path():
     test = os.path.join(BUILD, "hbltests", "SimpleOptimizations", "TwoSequenceTest.bf")
     if not os.path.isfile(test):
         pytest.skip("hbltests not copied")
+    from host import regress
+    work = regress.work_tree()
+    test = os.path.join(work, "hbltests", "SimpleOptimizations", "TwoSequenceTest.bf")
     tmp = tempfile.mkdtemp(prefix="hb2two_")
-    pr = subprocess.run([HOST_BIN, f"LIBPATH={os.path.join(BUILD, 'res')}", test], cwd=tmp, stdin=subprocess.DEVNULL,
+    pr = subprocess.run([HOST_BIN, f"LIBPATH={os.path.join(work, 'res')}", test], cwd=tmp, stdin=subprocess.DEVNULL,
                         stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=_no_gpu_env(), timeout=300)
     assert pr.returncode == 0 and "[TEST PASSED]" in pr.stdout, pr.stdout[-800:]

@@ -1,4 +1,4 @@
-"""CPU suite: the host-side planner of the tcgen05 pruning pass (hb2_plan_walk, the very code hb2_evaluate runs before
+"""CPU suite: the host-side planner of the tensor-core pruning pass (hb2_plan_walk, the very code hb2_evaluate runs before
 it launches prune64_tc_walk_kernel).  The kernel trusts the plan blindly -- a lane waits for another lane's tile only
 where the plan says WAIT, takes registers where it says CHAIN -- so the plan's invariants are checked here for many
 trees, lane counts and dirty sets, and each plan is executed by a small in-order-lane simulator to prove that its

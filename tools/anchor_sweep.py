@@ -1,4 +1,4 @@
-"""Sweep of the anchor threshold of the tcgen05 pruning kernel (HB2_ANCHOR_THR): pruning time against lnL error on the
+"""Sweep of the anchor threshold of the tensor-core pruning kernel (HB2_ANCHOR_THR): pruning time against lnL error on the
 north-star workload and on the deep-tree fixtures.  One process per setting (the threshold is read once per process)."""
 import json
 import os

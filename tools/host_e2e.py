@@ -1,4 +1,4 @@
-"""Evaluation stream of the north-star workload through the PATCHED HyPhy binary (host/_build/hyphy): evaluations/s of HBL
+"""Evaluation stream of the north-star workload through the PATCHED HyPhy binary (oracle/_ref/host/hyphy): evaluations/s of HBL
 `LFCompute` for both hand-over routes (compiled formula values / dense Q*t) and both precisions, next to the engine's own
 account of where the time went (HYPHY_B200_VERBOSE)."""
 import json
@@ -10,7 +10,7 @@ sys.path.insert(0, ROOT)
 from hyphy_b200 import synth          # noqa: E402
 from oracle import ref_harness as rh  # noqa: E402
 
-HOST = os.path.join(ROOT, "host", "_build", "hyphy")
+HOST = os.path.join(ROOT, "oracle", "_ref", "host", "hyphy")
 n = int(sys.argv[1]) if len(sys.argv) > 1 else 20
 w = synth.codon_workload(200, 2000, 4)
 out = []

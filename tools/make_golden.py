@@ -1,11 +1,14 @@
-"""Regenerates tests/golden/*.npz by running the UNMODIFIED reference binary (oracle/_ref/hyphy, built from
-/root/reference by oracle/Makefile.ref) on seeded synthetic workloads (hyphy_b200/synth.py).
+"""Regenerates tests/golden/*.npz by running the UNMODIFIED reference binary (oracle/_ref/hyphy, built from the
+reference sources by oracle/Makefile.ref) on seeded synthetic workloads (hyphy_b200/synth.py).
 
 Each fixture holds the reference's lnL and per-site log-likelihoods (ConstructCategoryMatrix SITE_LOG_LIKELIHOODS,
 alignment order) plus a checksum of the generated leaf states, so tests can prove they regenerated the same input.
-Run here (the container that has /root/reference):  python tools/make_golden.py
+`--runs` writes tests/golden/reference_runs.json instead: what tests/test_host_binding.py compares the patched host
+with (the final lnL of an evaluation stream, joint ML ancestral sequences).
+Run where the reference binary was built:  python tools/make_golden.py [--runs | name ...]
 """
 import hashlib
+import json
 import os
 import sys
 
@@ -15,6 +18,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from hyphy_b200 import synth            # noqa: E402
 from oracle import ref_harness as rh    # noqa: E402
+
+STREAM_CASE, STREAM_EVALS, STREAM_WARM = "mg94_30x100_c4_ambig", 5, 1
+ANCESTOR_CASES = ["mg94_8x60_c1", "mg94_8x60_c4_ambig", "c1_hky85_8x500", "mg94_30x100_c4_ambig"]
 
 # name -> constructor.  tests/golden_cases.py imports this table so both sides build identical inputs.
 CASES = {
@@ -42,10 +48,22 @@ def checksum(w) -> str:
     return h.hexdigest()
 
 
+def reference_runs(out):
+    s = rh.run_reference(CASES[STREAM_CASE](), n_evals=STREAM_EVALS, n_warm=STREAM_WARM, per_site=False)
+    runs = {"evaluation_stream": {"case": STREAM_CASE, "n_evals": STREAM_EVALS, "n_warm": STREAM_WARM, "loop_lnL": s["loop_lnL"]},
+            "ancestors": {name: rh.run_reference(CASES[name](), ancestors=True, per_site=False)["ancestors"] for name in ANCESTOR_CASES}}
+    with open(os.path.join(out, "reference_runs.json"), "w") as f:
+        json.dump(runs, f, indent=1, sort_keys=True)
+        f.write("\n")
+
+
 def main():
     out = os.path.join(ROOT, "tests", "golden")
     os.makedirs(out, exist_ok=True)
     only = sys.argv[1:]
+    if only == ["--runs"]:
+        reference_runs(out)
+        return
     for name, make in CASES.items():
         if only and name not in only:
             continue

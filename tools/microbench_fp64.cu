@@ -1,5 +1,5 @@
 // Microbenchmark: peak FP64 FMA and FP64 tensor (mma.sync.m8n8k4.f64) throughput on this GPU.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o gpurun_out/mb_fp64 tools/microbench_fp64.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o /tmp/mb_fp64 tools/microbench_fp64.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 
