@@ -223,18 +223,11 @@ struct hb2_partition {
     int *d_forced = nullptr, *h_forced = nullptr;   // forced states of the current evaluation (hb2_evaluate_forced)
     int forced_node = -1;
     // persistent walk kernel (one launch per evaluation): plan buffers, generation bits of the tagged hand-over, residency
-    bool small_walk = true;                   // HB2_SMALL_WALK=0: per-level launches of prune_small_kernel (A/B testing)
     int small_ilp = 0, small_resident[2] = {1, 1};   // HB2_SMALL_ILP=1/2 forces one / two patterns per thread (4 states); co-resident CTAs of both
-    bool small_dmma = true;                   // HB2_SMALL_DMMA=0: one thread per pattern (prune_small_walk_kernel) also for 16..32 states
-    int fp64_mode = 2;                        // HB2_FP64_WALK: 2 (default) prune64_lanes_kernel, 1 prune64_walk_kernel when it fills the machine, 0 per-level launches
-    bool fp64_walk = true;                    // fp64_mode >= 1
     double *d_cond_side = nullptr;            // fp64 lanes kernel: side products [C][I][Sp][64] (exponents: second half of d_scal)
     int *d_lane_flags = nullptr;              // [C][2I][Sp/64] pass id of the last production
-    int lane_pass = 0, lanes_resident[2] = {0, 0}, lanes_force_nw = 0;   // co-resident CTAs of the 4- and 8-warp shapes; HB2_LANES_WARPS
+    int lane_pass = 0, lanes_resident = 0;    // co-resident CTAs of prune64_lanes_kernel
     int sm_count = 132;
-    bool expm_dfma = false;                   // HB2_EXPM_DFMA=1: previous FFMA-style fp64 expm kernel (A/B testing)
-    bool use_walk = false;
-    bool walk_v2 = false;                     // HB2_WALK_V2=1: two threads per pattern (prune64_tc_walk2_kernel; correct, opt-in, DESIGN 4.2)
     int walk_max_resident = 0;
     // single-branch shortcut (hb2_branch_cache_*): outside vectors of one branch, all owned classes
     double *d_bc_out = nullptr; int *d_bc_outE = nullptr, *d_bc_sib = nullptr; int64_t bc_node = -1;
@@ -297,7 +290,7 @@ int plan_shared(hb2_partition *p, const int *h_dst, int64_t n, int kind, const i
     sp = SharedPlan();
     hb2_partition::ExBuf &x = bx ? *bx : p->ex;
     sp.x = &x;
-    if (p->Dp != 64 || p->expm_dfma || !p->ex_enabled || !x.d_int || n <= 0 || n > x.cap) return 0;
+    if (p->Dp != 64 || !p->ex_enabled || !x.d_int || n <= 0 || n > x.cap) return 0;
     if (kind == 1 && !p->tmpls[tmpl].d_Vres) return 0;
     if (wait_staging(p)) return 1;            // an earlier plan's upload may still be reading the pinned arrays
     int *grp = x.h_int, *ref = x.h_int + x.cap, *refs = x.h_int + 2 * x.cap;
@@ -338,93 +331,49 @@ int launch_expm(hb2_partition *p, const double *dQ, const int *d_dst, int n, int
         a.is_trans = 0; a.Q = nullptr; a.V = dQ; a.tmpl_index = t.d_index; a.tmpl_formula = t.d_formula;
         a.tmpl_colfreq = t.has_colfreq ? t.d_colfreq : nullptr; a.tmpl_nnz = (int)t.nnz; a.nF = (int)t.nF;
     }
-    bool packed = false;
     pack_tc = pack_tc && p->use_tc && !pt_override;
     switch (p->Dp) {
-        case 64:
-            if (p->expm_dfma) {
-                hb2::expm64_kernel<<<n, 256, 5 * 64 * hb2::LD64 * sizeof(double), p->stream>>>(a);
-            } else {
-                const size_t smem = 3 * 64 * hb2::LD64 * sizeof(double);
-                if (sp && sp->use && is_trans != 1) {
-                    hb2_partition::ExBuf &x = *sp->x;
-                    const int nV = sp->kind == 1 ? (int)p->tmpls[tmpl].nF : (int)(p->D * p->D);
-                    const hb2::ExpmGroup *groups = static_cast<const hb2::ExpmGroup *>(x.d_groups);
-                    hb2::ExpmClassifyArgs ca{};
-                    ca.V = dQ; ca.nV = nV; ca.kind = sp->kind; ca.dst = d_dst; ca.group = x.d_int + off;
-                    ca.ref = x.d_int + x.cap + off; ca.groups = groups; ca.refvec = x.d_refvec; ca.refvec_stride = x.stride;
-                    ca.weight = x.d_weight + off; ca.flag = x.d_flag + off;
-                    ca.res = pt_override ? nullptr : (sp->kind == 1 ? p->tmpls[tmpl].d_Vres : qres);   // scratch targets keep no resident copy
-                    // references index the whole batch: classification has to see it in one piece (off == 0 for compiled batches
-                    // and for dense batches that consist of a single run; mixed dense batches fall back below)
-                    static const bool warp_classify = !(getenv("HB2_CLASSIFY_WARP") && getenv("HB2_CLASSIFY_WARP")[0] == '0');
-                    if (nV <= 256 && warp_classify) hb2::expm_classify_warp_kernel<<<(n + 7) / 8, 256, 0, p->stream>>>(ca, n);
-                    else hb2::expm_classify_kernel<<<n, 128, 0, p->stream>>>(ca);
-                    a.group = ca.group; a.flag = ca.flag; a.weight = ca.weight; a.groups = groups; a.pow = x.d_pow;
-                    a.Qres = nullptr;                    // the classification stage keeps the resident copy
-                    if (sp->n_refs > 0) {
-                        hb2::ExpmPowersArgs pa{};
-                        pa.a = a; pa.refs = x.d_int + 2 * x.cap; pa.groups = static_cast<hb2::ExpmGroup *>(x.d_groups);
-                        pa.pow = x.d_pow; pa.refvec = x.d_refvec; pa.refvec_stride = x.stride; pa.nV = nV; pa.kind = sp->kind; pa.Vin = dQ;
-                        pa.flags = x.d_flags; pa.gen = ++x.gen; pa.err = p->d_err;
-                        hb2::expm_powers_kernel<<<dim3(hb2::EXPM_POW_TERMS - 1, (unsigned)sp->n_refs), 256, smem, p->stream>>>(pa);
-                        p->launches++;
-                    }
-                    hb2::ExpmTcOut tcs{nullptr, nullptr};
-                    if (pack_tc) { tcs.PB = p->d_PB; tcs.PTf = p->d_PTf; }
-                    double *colsum = x.d_colsum + (size_t)off * 16 * 64;
-                    hb2::expm_poly_kernel<<<dim3(16, (unsigned)((n + hb2::EXPM_POLY_CHUNK - 1) / hb2::EXPM_POLY_CHUNK)), 256, 0, p->stream>>>(a, tcs, colsum, n);
-                    // the row repair of the entries the polynomial kernel finished rides in the finishing kernel below (same
-                    // arithmetic as expm_diag_kernel, one launch less); needs the tensor-path outputs to be the same set
-                    static const bool fuse_diag = !(getenv("HB2_EXPM_FUSE_DIAG") && getenv("HB2_EXPM_FUSE_DIAG")[0] == '0');
-                    if (fuse_diag) { a.colsum = colsum; p->launches += 2; }
-                    else { hb2::expm_diag_kernel<<<n, 64, 0, p->stream>>>(a, tcs, colsum); p->launches += 3; }
+        case 64: {
+            const size_t smem = 3 * 64 * hb2::LD64 * sizeof(double);
+            hb2::ExpmTcOut tc{nullptr, nullptr};
+            if (pack_tc) { tc.PB = p->d_PB; tc.PTf = p->d_PTf; }
+            if (sp && sp->use && is_trans != 1) {
+                hb2_partition::ExBuf &x = *sp->x;
+                const int nV = sp->kind == 1 ? (int)p->tmpls[tmpl].nF : (int)(p->D * p->D);
+                const hb2::ExpmGroup *groups = static_cast<const hb2::ExpmGroup *>(x.d_groups);
+                hb2::ExpmClassifyArgs ca{};
+                ca.V = dQ; ca.nV = nV; ca.kind = sp->kind; ca.dst = d_dst; ca.group = x.d_int + off;
+                ca.ref = x.d_int + x.cap + off; ca.groups = groups; ca.refvec = x.d_refvec; ca.refvec_stride = x.stride;
+                ca.weight = x.d_weight + off; ca.flag = x.d_flag + off;
+                ca.res = pt_override ? nullptr : (sp->kind == 1 ? p->tmpls[tmpl].d_Vres : qres);   // scratch targets keep no resident copy
+                // references index the whole batch: classification has to see it in one piece (off == 0 for compiled batches
+                // and for dense batches that consist of a single run; mixed dense batches fall back below)
+                if (nV <= 256) hb2::expm_classify_warp_kernel<<<(n + 7) / 8, 256, 0, p->stream>>>(ca, n);
+                else hb2::expm_classify_kernel<<<n, 128, 0, p->stream>>>(ca);
+                a.group = ca.group; a.flag = ca.flag; a.weight = ca.weight; a.groups = groups; a.pow = x.d_pow;
+                a.Qres = nullptr;                    // the classification stage keeps the resident copy
+                if (sp->n_refs > 0) {
+                    hb2::ExpmPowersArgs pa{};
+                    pa.a = a; pa.refs = x.d_int + 2 * x.cap; pa.groups = static_cast<hb2::ExpmGroup *>(x.d_groups);
+                    pa.pow = x.d_pow; pa.refvec = x.d_refvec; pa.refvec_stride = x.stride; pa.nV = nV; pa.kind = sp->kind; pa.Vin = dQ;
+                    pa.flags = x.d_flags; pa.gen = ++x.gen; pa.err = p->d_err;
+                    hb2::expm_powers_kernel<<<dim3(hb2::EXPM_POW_TERMS - 1, (unsigned)sp->n_refs), 256, smem, p->stream>>>(pa);
+                    p->launches++;
                 }
-                hb2::ExpmTcOut tco{nullptr, nullptr};
-                if (pack_tc) { tco.PB = p->d_PB; tco.PTf = p->d_PTf; packed = true; }
-                hb2::expm64_dmma_kernel<<<n, 256, smem, p->stream>>>(a, tco);
+                double *colsum = x.d_colsum + (size_t)off * 16 * 64;
+                hb2::expm_poly_kernel<<<dim3(16, (unsigned)((n + hb2::EXPM_POLY_CHUNK - 1) / hb2::EXPM_POLY_CHUNK)), 256, 0, p->stream>>>(a, tc, colsum, n);
+                a.colsum = colsum;                   // the finishing kernel below repairs the rows of the entries finished here
+                p->launches += 2;
             }
+            hb2::expm64_dmma_kernel<<<n, 256, smem, p->stream>>>(a, tc);
             break;
+        }
         case 4: hb2::expm_small_kernel<4><<<n, 128, hb2::expm_small_smem_bytes(4), p->stream>>>(a); break;
         case 8: hb2::expm_small_kernel<8><<<n, 128, hb2::expm_small_smem_bytes(8), p->stream>>>(a); break;
         case 16: hb2::expm_small_kernel<16><<<n, 128, hb2::expm_small_smem_bytes(16), p->stream>>>(a); break;
         case 24: hb2::expm_small_kernel<24><<<n, 128, hb2::expm_small_smem_bytes(24), p->stream>>>(a); break;
         case 32: hb2::expm_small_kernel<32><<<n, 128, hb2::expm_small_smem_bytes(32), p->stream>>>(a); break;
         default: return fail("unsupported padded state count %d", p->Dp);
-    }
-    p->launches++;
-    CU(cudaGetLastError());
-    if (pack_tc && !packed) {
-        hb2::pack_tc_kernel<<<n, 256, 0, p->stream>>>(p->d_PT, d_dst, p->d_PB, p->d_PTf);
-        p->launches++;
-        CU(cudaGetLastError());
-    }
-    return 0;
-}
-
-int launch_prune(hb2_partition *p, const hb2::PruneArgs &a, const int *d_jobs, int njobs, int ncls) {
-    if (njobs <= 0) return 0;
-    if (p->use_tc) {
-        hb2::PruneTcArgs t;
-        t.PB = p->d_PB; t.PTf = p->d_PTf; t.cond = p->d_condf; t.scal = a.scal; t.leaf = a.leaf; t.ambig = a.ambig; t.pi = a.pi;
-        t.rootL = a.rootL; t.rootE = a.rootE; t.tree = a.tree; t.err = p->d_err;
-        t.L = a.L; t.I = a.I; t.B = a.B; t.D = a.D; t.Sp = a.Sp; t.cat0 = a.cat0;
-        t.forced = a.forced; t.forced_node = a.forced_node;
-        dim3 grid((unsigned)(p->Sp / hb2::TC_TILE_P), (unsigned)njobs, (unsigned)ncls);
-        hb2::prune64_tc_kernel<<<grid, 128, hb2::TC_SMEM_BYTES, p->stream>>>(t, d_jobs);
-    } else if (p->Dp == 64) {
-        dim3 grid((unsigned)(p->Sp / hb2::TILE_P), (unsigned)njobs, (unsigned)ncls);
-        hb2::prune64_kernel<<<grid, 256, 2 * 64 * hb2::LD64 * sizeof(double), p->stream>>>(a, d_jobs);
-    } else {
-        dim3 grid((unsigned)(p->Sp / 128), (unsigned)njobs, (unsigned)ncls);
-        switch (p->Dp) {
-            case 4: hb2::prune_small_kernel<4><<<grid, 128, 0, p->stream>>>(a, d_jobs); break;
-            case 8: hb2::prune_small_kernel<8><<<grid, 128, 0, p->stream>>>(a, d_jobs); break;
-            case 16: hb2::prune_small_kernel<16><<<grid, 128, 0, p->stream>>>(a, d_jobs); break;
-            case 24: hb2::prune_small_kernel<24><<<grid, 128, 0, p->stream>>>(a, d_jobs); break;
-            case 32: hb2::prune_small_kernel<32><<<grid, 128, 0, p->stream>>>(a, d_jobs); break;
-            default: return fail("unsupported padded state count %d", p->Dp);
-        }
     }
     p->launches++;
     CU(cudaGetLastError());
@@ -577,7 +526,7 @@ int plan_walk(const std::vector<std::vector<int>> &children, const std::vector<i
     // canonical_multi (fp64 lanes kernel): a node with more than two children is neither split nor chained and its children
     // are multiplied in tree order, so its product is associated the same way in every plan; with two children the product
     // is exact-commutative and power-of-two rescalings are exact, hence conditionals do not depend on the plan at all (a
-    // partial re-evaluation reproduces the full one bit for bit, like the per-level kernel).
+    // partial re-evaluation reproduces the full one bit for bit).
     // Jobs.  Job j < I is node j; job I + n is the SIDE PRODUCT of node n: a node with two or more internal children is
     // split into "contract the child with the deepest subtree" (+ multiply the side product in: no matrix, the cheapest
     // step after a leaf) and a side job that contracts all OTHER children.  Side jobs sit off the root path, so other
@@ -761,8 +710,7 @@ int run_walk(hb2_partition *p, int cat0, int ncls, const std::vector<std::vector
         w.trace = d_trace;
         w.trace_cta_times = d_trace + (size_t)(ns + 1) * 12;
     }
-    if (p->walk_v2) hb2::prune64_tc_walk2_kernel<<<nslots * K, 256, hb2::WALK2_SMEM_BYTES, p->stream>>>(w);
-    else hb2::prune64_tc_walk_kernel<<<nslots * K, 128, hb2::WALK_SMEM_BYTES, p->stream>>>(w);
+    hb2::prune64_tc_walk_kernel<<<nslots * K, 128, hb2::WALK_SMEM_BYTES, p->stream>>>(w);
     if (d_trace) {
         std::vector<long long> ht((size_t)(ns + 1) * 12 + (size_t)nslots * K * 4);
         CU(cudaStreamSynchronize(p->stream));
@@ -802,7 +750,7 @@ static bool small_two_patterns(const hb2_partition *p, int ncls) {
     return 1.55 * std::ceil((double)ct2 / p->small_resident[1]) < std::ceil((double)ct1 / p->small_resident[0]);
 }
 
-// Small state spaces: one launch, one thread per pattern walking the dirty nodes in post-order.
+// Small state spaces: one launch, every CTA walking the dirty nodes in post-order.
 int run_small_walk(hb2_partition *p, int cat0, int ncls, const std::vector<std::vector<int>> &levels) {
     std::vector<int> jobs;
     for (auto &lv : levels) jobs.insert(jobs.end(), lv.begin(), lv.end());
@@ -811,9 +759,8 @@ int run_small_walk(hb2_partition *p, int cat0, int ncls, const std::vector<std::
     std::copy(jobs.begin(), jobs.end(), p->h_jobs);
     CU(cudaMemcpyAsync(p->d_jobs, p->h_jobs, jobs.size() * sizeof(int), cudaMemcpyHostToDevice, p->stream));
     hb2::PruneArgs a = prune_args(p, cat0);
-    dim3 grid((unsigned)(p->Sp / 128), (unsigned)ncls);
     const int n = (int)jobs.size();
-    if (p->Dp >= 16 && p->small_dmma) {          // 16 / 24 / 32 padded states: FP64 tensor pipe, 8 patterns per warp
+    if (p->Dp >= 16) {                           // 16 / 24 / 32 padded states: FP64 tensor pipe, 8 patterns per warp
         // every CTA walks the whole tree: the launch is a few long waves.  Shape with the smaller last-wave loss: 8 warps
         // (4 CTAs per SM; 3 at 32 states) or, up to 24 states, 4 warps (9 per SM).
         const double warps = (double)(p->Sp / 8) * ncls;
@@ -845,12 +792,10 @@ int run_small_walk(hb2_partition *p, int cat0, int ncls, const std::vector<std::
         CU(cudaGetLastError());
         return 0;
     }
+    dim3 grid((unsigned)(p->Sp / 128), (unsigned)ncls);   // 4 / 8 padded states: one thread per pattern
     switch (p->Dp) {
         case 4: hb2::prune_small_walk_kernel<4><<<grid, 128, 0, p->stream>>>(a, p->d_jobs, n); break;
         case 8: hb2::prune_small_walk_kernel<8><<<grid, 128, 0, p->stream>>>(a, p->d_jobs, n); break;
-        case 16: hb2::prune_small_walk_kernel<16><<<grid, 128, 0, p->stream>>>(a, p->d_jobs, n); break;
-        case 24: hb2::prune_small_walk_kernel<24><<<grid, 128, 0, p->stream>>>(a, p->d_jobs, n); break;
-        case 32: hb2::prune_small_walk_kernel<32><<<grid, 128, 0, p->stream>>>(a, p->d_jobs, n); break;
         default: return fail("unsupported padded state count %d", p->Dp);
     }
     p->launches++;
@@ -858,33 +803,14 @@ int run_small_walk(hb2_partition *p, int cat0, int ncls, const std::vector<std::
     return 0;
 }
 
-// 33..64 states in fp64: one launch, CTA (tile, class) walks the dirty nodes in post-order (prune64_walk_kernel).
-int run_fp64_walk(hb2_partition *p, int cat0, int ncls, const std::vector<std::vector<int>> &levels) {
-    std::vector<int> jobs;
-    for (auto &lv : levels) jobs.insert(jobs.end(), lv.begin(), lv.end());
-    if (jobs.empty()) return 0;
-    std::sort(jobs.begin(), jobs.end());                 // internal indices ascending == post-order
-    std::copy(jobs.begin(), jobs.end(), p->h_jobs);      // (every evaluation ends with a stream synchronisation: the buffer is free)
-    CU(cudaMemcpyAsync(p->d_jobs, p->h_jobs, jobs.size() * sizeof(int), cudaMemcpyHostToDevice, p->stream));
-    hb2::PruneArgs a = prune_args(p, cat0);
-    dim3 grid((unsigned)(p->Sp / hb2::TILE_P), (unsigned)ncls);
-    hb2::prune64_walk_kernel<<<grid, 256, 2 * 64 * hb2::LD64 * sizeof(double), p->stream>>>(a, p->d_jobs, (int)jobs.size());
-    p->launches++;
-    CU(cudaGetLastError());
-    return 0;
-}
-
-// 33..64 states in fp64, default: one launch, K in-order lanes per (class, 64-pattern tile) (prune64_lanes_kernel).  Same
+// 33..64 states in fp64: one launch, K in-order lanes per (class, 32-pattern tile) (prune64_lanes_kernel).  Same
 // planner and plan cache as the tensor walk; the step list travels without a generation table (hand-over by pass id).
 int run_fp64_lanes(hb2_partition *p, int cat0, int ncls, const std::vector<std::vector<int>> &levels) {
     const int I = (int)p->I, L = (int)p->L;
     int total = 0;
     for (auto &lv : levels) total += (int)lv.size();
     if (total == 0) return 0;
-    // CTA shape: 4 warps x 8 patterns, 4 CTAs per SM.  The 8-warp shape (64 patterns, 3 per SM) gives the north-star shape a
-    // third lane and c5 a single round, but was slower on both: it stays behind HB2_LANES_WARPS=8 for A/B runs.
-    const int nw = p->lanes_force_nw == 8 ? 8 : 4;
-    const int T = (int)(p->Sp / (8 * nw)), CT = ncls * T, resident = p->lanes_resident[nw == 8];
+    const int T = (int)(p->Sp / hb2::LANES_TILE_P), CT = ncls * T, resident = p->lanes_resident;
     const int K = std::max(1, std::min(std::min(p->walk_lane_cap, total), resident / std::max(CT, 1)));
     const int nslots = (K == 1) ? std::min(CT, resident) : CT;
     std::vector<char> dirty(I, 0);
@@ -920,7 +846,7 @@ int run_fp64_lanes(hb2_partition *p, int cat0, int ncls, const std::vector<std::
     w.lane_start = p->d_walk; w.steps = reinterpret_cast<const int4 *>(p->d_walk + o4);
     w.flags = p->d_lane_flags; w.err = p->d_err;
     w.K = K; w.T = T; w.ncls = ncls; w.nslots = nslots; w.pass = ++p->lane_pass;
-    if (getenv("HB2_DEBUG")) fprintf(stderr, "[hb2] fp64 lanes: jobs=%d steps=%d K=%d T=%d ncls=%d nslots=%d grid=%d warps=%d resident=%d\n", total, ns, K, T, ncls, nslots, nslots * K, nw, resident);
+    if (getenv("HB2_DEBUG")) fprintf(stderr, "[hb2] fp64 lanes: jobs=%d steps=%d K=%d T=%d ncls=%d nslots=%d grid=%d resident=%d\n", total, ns, K, T, ncls, nslots, nslots * K, resident);
     w.trace = nullptr; w.trace_cta = 0;
     const char *trace_path = getenv("HB2_WALK_TRACE");
     long long *d_trace = nullptr;
@@ -931,8 +857,7 @@ int run_fp64_lanes(hb2_partition *p, int cat0, int ncls, const std::vector<std::
         CU(cudaMemsetAsync(d_trace, 0, (size_t)(ns + 1) * 12 * sizeof(long long), p->stream));
         w.trace = d_trace;
     }
-    if (nw == 4) hb2::prune64_lanes_kernel<4><<<nslots * K, 128, hb2::lanes_smem_bytes(4), p->stream>>>(w);
-    else hb2::prune64_lanes_kernel<8><<<nslots * K, 256, hb2::lanes_smem_bytes(8), p->stream>>>(w);
+    hb2::prune64_lanes_kernel<<<nslots * K, hb2::LANES_THREADS, hb2::LANES_SMEM_BYTES, p->stream>>>(w);
     if (d_trace) {
         std::vector<long long> ht((size_t)(ns + 1) * 12);
         CU(cudaStreamSynchronize(p->stream));
@@ -956,29 +881,12 @@ int run_fp64_lanes(hb2_partition *p, int cat0, int ncls, const std::vector<std::
     return 0;
 }
 
+// One launch per evaluation: the tensor walk (33..64 states), the fp64 lanes kernel (33..64 states with
+// HB2_FLAG_FORCE_FP64) or the small-state walk (<= 32 padded states).
 int run_pruning(hb2_partition *p, int cat0, int ncls, const std::vector<std::vector<int>> &levels) {
-    if (p->use_tc && p->use_walk) return run_walk(p, cat0, ncls, levels);
-    // one launch per evaluation pays only when (tiles x classes) fills the machine about twice over (c5: 316 CTAs); below
-    // that the per-level launches expose more parallelism (a single class of the north-star shape -- the patched host's
-    // per-class ComputeBlock -- is 32 CTAs and would leave most SMs idle)
-    if (!p->use_tc && p->Dp == 64 && p->fp64_mode == 2) return run_fp64_lanes(p, cat0, ncls, levels);
-    if (!p->use_tc && p->Dp == 64 && p->fp64_walk && (int64_t)(p->Sp / hb2::TILE_P) * ncls >= 2 * p->sm_count)
-        return run_fp64_walk(p, cat0, ncls, levels);
-    if (p->Dp <= 32 && p->small_walk) return run_small_walk(p, cat0, ncls, levels);
-    // upload all job lists in one copy
-    int total = 0;
-    for (auto &lv : levels) total += (int)lv.size();
-    if (total == 0) return 0;
-    int off = 0;
-    for (auto &lv : levels) { std::copy(lv.begin(), lv.end(), p->h_jobs + off); off += (int)lv.size(); }
-    CU(cudaMemcpyAsync(p->d_jobs, p->h_jobs, total * sizeof(int), cudaMemcpyHostToDevice, p->stream));
-    hb2::PruneArgs a = prune_args(p, cat0);
-    off = 0;
-    for (auto &lv : levels) {
-        if (launch_prune(p, a, p->d_jobs + off, (int)lv.size(), ncls)) return 1;
-        off += (int)lv.size();
-    }
-    return 0;
+    if (p->use_tc) return run_walk(p, cat0, ncls, levels);
+    if (p->Dp == 64) return run_fp64_lanes(p, cat0, ncls, levels);
+    return run_small_walk(p, cat0, ncls, levels);
 }
 
 // (Re)creates the peer-exchange buffers with room for `payload` doubles per rank and maps every other rank's buffer through
@@ -1066,9 +974,7 @@ hb2::PeerBuf peer_buf(hb2_partition *p) {
 }
 
 int run_root(hb2_partition *p, int c0, int nc, bool use_weights, bool want_sites) {
-    static const bool fuse_root = !(getenv("HB2_ROOT_FUSED") && getenv("HB2_ROOT_FUSED")[0] == '0');
-    const bool plain = p->cg_G <= 1;           // single GPU or pattern shards: combine + sum in one kernel (its last block)
-    if (!(plain && fuse_root)) CU(cudaMemsetAsync(p->d_flag, 0, sizeof(int), p->stream));
+    if (p->cg_G > 1) CU(cudaMemsetAsync(p->d_flag, 0, sizeof(int), p->stream));
     hb2::CombineArgs c;
     c.counter = nullptr; c.out = nullptr;
     c.rootL = p->d_rootL; c.rootE = p->d_rootE; c.weights = use_weights ? p->d_weights : nullptr; c.freq = p->d_freq;
@@ -1104,15 +1010,10 @@ int run_root(hb2_partition *p, int c0, int nc, bool use_weights, bool want_sites
         CU(cudaGetLastError());
         return 0;
     }
-    if (fuse_root) {
-        c.counter = p->d_root_counter; c.out = p->d_lnL;
-        hb2::combine_kernel<<<p->n_partial_blocks, 256, 0, p->stream>>>(c);
-        p->launches += 1;
-    } else {
-        hb2::combine_kernel<<<p->n_partial_blocks, 256, 0, p->stream>>>(c);
-        hb2::final_sum_kernel<<<1, 256, 0, p->stream>>>(p->d_partial, p->n_partial_blocks, p->d_flag, p->d_lnL);
-        p->launches += 2;
-    }
+    // single GPU or pattern shards: combine + sum in one kernel (its last block)
+    c.counter = p->d_root_counter; c.out = p->d_lnL;
+    hb2::combine_kernel<<<p->n_partial_blocks, 256, 0, p->stream>>>(c);
+    p->launches += 1;
     CU(cudaGetLastError());
     if (p->comm && p->px_ok) {                // pattern shards: R partial lnL over peer memory, summed in rank order
         hb2::peer_sum_kernel<<<1, 64, 0, p->stream>>>(peer_buf(p), p->d_lnL);
@@ -1198,7 +1099,7 @@ int evaluate_impl(hb2_partition *p, int c0, int nc, const double *weights, int64
     if (siteScale) CU(cudaMemcpyAsync(siteScale, p->d_siteScale, p->S * sizeof(long long), cudaMemcpyDeviceToHost, p->stream));
     CU(cudaStreamSynchronize(p->stream));
     if (const int code = *reinterpret_cast<int *>(hs + p->Dp + p->C + 1)) {
-        p->walk_reset = p->use_tc && p->use_walk;          // tags are inconsistent: the next pass starts from scratch
+        p->walk_reset = p->use_tc;          // tags are inconsistent: the next pass starts from scratch
         cudaMemsetAsync(p->d_err, 0, sizeof(int), p->stream);   // on every path, or each later evaluation would fail too
         std::fill(p->evaluated_cat.begin(), p->evaluated_cat.end(), 0);
         return fail("a device-side wait timed out (code %d: 1 = operand staging / tensor pipe, 2 = another lane's conditionals, 3 = a peer "
@@ -1245,7 +1146,8 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
     p->device = device; p->flags = flags; p->S = S; p->D = D; p->L = L; p->I = I; p->C = C; p->B = L + I - 1; p->nAmb = nAmb;
     p->Dp = Dp;
     p->use_tc = (Dp == 64) && !(flags & HB2_FLAG_FORCE_FP64);
-    const int64_t tile = (Dp == 64 && !p->use_tc) ? hb2::TILE_P : 128;
+    // pattern padding: fp64 codon partitions to 64 (a multiple of the 32-pattern lanes-kernel tile), all others to 128
+    const int64_t tile = (Dp == 64 && !p->use_tc) ? 64 : 128;
     p->Sp = (S + tile - 1) / tile * tile;
     p->parents.assign(flatParents, flatParents + L + I);
     p->children.assign(I, {});
@@ -1280,25 +1182,19 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
     CUP(cudaMalloc(&p->d_ambig, std::max<int64_t>(nAmb, 1) * Dp * sizeof(double)));
     CUP(cudaMalloc(&p->d_freq, Sp * sizeof(double)));
     if (p->use_tc) {
-        // 2I node slots per class: I nodes + I side products of the walk kernel (the per-level kernel uses the first I)
+        // 2I node slots per class: I nodes + I side products of the walk kernel
         CUP(cudaMalloc(&p->d_condf, (size_t)C * 2 * I * Sp * 64 * sizeof(float)));
         CUP(cudaMalloc(&p->d_PB, (size_t)C * p->B * hb2::TC_PB_FLOATS * sizeof(float)));
         CUP(cudaMalloc(&p->d_PTf, (size_t)C * p->B * hb2::TC_PTF_FLOATS * sizeof(float)));
         CUP(cudaMemsetAsync(p->d_condf, 0, (size_t)C * 2 * I * Sp * 64 * sizeof(float), p->stream));
         CUP(cudaMemsetAsync(p->d_PB, 0, (size_t)C * p->B * hb2::TC_PB_FLOATS * sizeof(float), p->stream));
         CUP(cudaMemsetAsync(p->d_PTf, 0, (size_t)C * p->B * hb2::TC_PTF_FLOATS * sizeof(float), p->stream));
-        CUP(cudaFuncSetAttribute(hb2::prune64_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, hb2::TC_SMEM_BYTES));
         CUP(cudaFuncSetAttribute(hb2::prune64_tc_walk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, hb2::WALK_SMEM_BYTES));
-        CUP(cudaFuncSetAttribute(hb2::prune64_tc_walk2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, hb2::WALK2_SMEM_BYTES));
-        CUP(cudaFuncSetAttribute(hb2::prune64_tc_walk2_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-        { const char *env = getenv("HB2_WALK_V2"); p->walk_v2 = env && env[0] == '1'; }
         {
-            const char *env = getenv("HB2_TC_WALK");
-            p->use_walk = !(env && env[0] == '0');
             int per_sm = 0, sms = 0;
             CUP(cudaFuncSetAttribute(hb2::prune64_tc_walk_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-            const void *wk = p->walk_v2 ? (const void *)hb2::prune64_tc_walk2_kernel : (const void *)hb2::prune64_tc_walk_kernel;
-            const int wk_threads = p->walk_v2 ? 256 : 128, wk_smem = p->walk_v2 ? hb2::WALK2_SMEM_BYTES : hb2::WALK_SMEM_BYTES;
+            const void *wk = (const void *)hb2::prune64_tc_walk_kernel;
+            const int wk_threads = 128, wk_smem = hb2::WALK_SMEM_BYTES;
             CUP(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, wk, wk_threads, wk_smem));
             if (getenv("HB2_DEBUG")) {
                 cudaFuncAttributes fa; cudaFuncGetAttributes(&fa, wk);
@@ -1322,7 +1218,11 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
             if (const char *ov = getenv("HB2_WALK_CTAS_PER_SM")) per_sm = atoi(ov);      // bring-up override
             if (const char *ov = getenv("HB2_WALK_LANES")) p->walk_lane_cap = std::max(1, std::min(atoi(ov), 15));
             p->walk_max_resident = std::min(per_sm, 2) * sms;
-            if (p->walk_max_resident < 1) p->use_walk = false;
+            if (p->walk_max_resident < 1) {
+                fail("prune64_tc_walk_kernel (%d B of shared memory) cannot be resident on device %d", wk_smem, device);
+                hb2_destroy(p);
+                return 1;
+            }
             const size_t T = Sp / hb2::TC_TILE_P;
             p->walk_gen.assign((size_t)C * 2 * I, 0);   // matches the zero-filled conditional and exponent buffers
             const size_t walk_ints = 16 + 2 * (size_t)(L + 2 * I) + (size_t)C * 2 * I;
@@ -1333,10 +1233,9 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
     } else {
         CUP(cudaMalloc(&p->d_cond, (size_t)C * I * Sp * Dp * sizeof(double)));
         CUP(cudaMemsetAsync(p->d_cond, 0, (size_t)C * I * Sp * Dp * sizeof(double), p->stream));
-        { const char *env = getenv("HB2_FP64_WALK"); p->fp64_mode = (env && env[0] >= '0' && env[0] <= '2') ? env[0] - '0' : 2; }
-        if (Dp == 64 && p->fp64_mode == 2) {
+        if (Dp == 64) {
             // lanes kernel: side products, hand-over flags, the step list, and how many CTAs can be co-resident
-            const size_t T = Sp / 32;                                        // flags are sized for the smaller tile
+            const size_t T = Sp / hb2::LANES_TILE_P;
             CUP(cudaMalloc(&p->d_cond_side, (size_t)C * I * Sp * 64 * sizeof(double)));
             CUP(cudaMemsetAsync(p->d_cond_side, 0, (size_t)C * I * Sp * 64 * sizeof(double), p->stream));
             CUP(cudaMalloc(&p->d_lane_flags, (size_t)C * 2 * I * T * sizeof(int)));
@@ -1346,28 +1245,25 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
             CUP(cudaMallocHost(&p->h_walk, walk_ints * sizeof(int)));
             { const char *ev = getenv("HB2_WALK_SPLIT_NODES"); p->walk_split_nodes = !(ev && ev[0] == '0'); }
             if (const char *ov = getenv("HB2_WALK_LANES")) p->walk_lane_cap = std::max(1, std::min(atoi(ov), 15));
-            if (const char *ov = getenv("HB2_LANES_WARPS")) p->lanes_force_nw = atoi(ov) == 8 ? 8 : atoi(ov) == 4 ? 4 : 0;
             int sms = 0;
             CUP(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
             cudaDeviceProp dp; CUP(cudaGetDeviceProperties(&dp, device));
-            for (int v = 0; v < 2; v++) {
-                const void *fn = v ? (const void *)hb2::prune64_lanes_kernel<8> : (const void *)hb2::prune64_lanes_kernel<4>;
-                const int threads = v ? 256 : 128, smem = hb2::lanes_smem_bytes(v ? 8 : 4), cap = v ? 3 : 4;
-                CUP(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-                CUP(cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-                int per_sm = 0;
-                CUP(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, threads, smem));
-                // same resource arithmetic as for the tensor walk kernel (the occupancy API under-reports there)
-                cudaFuncAttributes fa;
-                CUP(cudaFuncGetAttributes(&fa, fn));
-                const int regs_per_cta = ((fa.numRegs + 7) / 8 * 8) * threads;
-                const size_t smem_per_cta = (size_t)smem + fa.sharedSizeBytes + dp.reservedSharedMemPerBlock;
-                const int by_res = std::min(dp.regsPerMultiprocessor / std::max(regs_per_cta, 1), (int)(dp.sharedMemPerMultiprocessor / smem_per_cta));
-                if (getenv("HB2_DEBUG")) fprintf(stderr, "[hb2] fp64 lanes kernel <%d warps>: occupancy API %d, by resources %d (regs %d)\n", v ? 8 : 4, per_sm, by_res, fa.numRegs);
-                per_sm = std::max(per_sm, std::min(by_res, cap));
-                if (const char *ov = getenv("HB2_WALK_CTAS_PER_SM")) per_sm = atoi(ov);
-                p->lanes_resident[v] = std::max(per_sm, 1) * sms;
-            }
+            const void *fn = (const void *)hb2::prune64_lanes_kernel;
+            const int threads = hb2::LANES_THREADS, smem = hb2::LANES_SMEM_BYTES;
+            CUP(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+            CUP(cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+            int per_sm = 0;
+            CUP(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, threads, smem));
+            // same resource arithmetic as for the tensor walk kernel (the occupancy API under-reports there)
+            cudaFuncAttributes fa;
+            CUP(cudaFuncGetAttributes(&fa, fn));
+            const int regs_per_cta = ((fa.numRegs + 7) / 8 * 8) * threads;
+            const size_t smem_per_cta = (size_t)smem + fa.sharedSizeBytes + dp.reservedSharedMemPerBlock;
+            const int by_res = std::min(dp.regsPerMultiprocessor / std::max(regs_per_cta, 1), (int)(dp.sharedMemPerMultiprocessor / smem_per_cta));
+            if (getenv("HB2_DEBUG")) fprintf(stderr, "[hb2] fp64 lanes kernel: occupancy API %d, by resources %d (regs %d)\n", per_sm, by_res, fa.numRegs);
+            per_sm = std::max(per_sm, std::min(by_res, hb2::LANES_CTAS_PER_SM));
+            if (const char *ov = getenv("HB2_WALK_CTAS_PER_SM")) per_sm = atoi(ov);
+            p->lanes_resident = std::max(per_sm, 1) * sms;
         }
     }
     CUP(cudaMalloc(&p->d_err, sizeof(int)));
@@ -1438,18 +1334,10 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
         CUP(cudaMemsetAsync(p->ex.d_flags, 0, (size_t)p->ex.G * hb2::EXPM_POW_TERMS * sizeof(unsigned long long), p->stream));
         CUP(cudaMalloc(&p->ex.d_refvec, (size_t)p->ex.G * p->ex.stride * sizeof(double)));
         CUP(cudaFuncSetAttribute(hb2::expm_powers_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(3 * 64 * hb2::LD64 * sizeof(double))));
-        CUP(cudaFuncSetAttribute(hb2::expm64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(5 * 64 * hb2::LD64 * sizeof(double))));
         CUP(cudaFuncSetAttribute(hb2::expm64_dmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(3 * 64 * hb2::LD64 * sizeof(double))));
         CUP(cudaFuncSetAttribute(hb2::expm64_dmma_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-        { const char *env = getenv("HB2_EXPM_DFMA"); p->expm_dfma = env && env[0] == '1'; }
-    }
-    {
-        CUP(cudaFuncSetAttribute(hb2::prune64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(2 * 64 * hb2::LD64 * sizeof(double))));
-        CUP(cudaFuncSetAttribute(hb2::prune64_walk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(2 * 64 * hb2::LD64 * sizeof(double))));
     }
 #undef CUP
-    { const char *env = getenv("HB2_SMALL_WALK"); p->small_walk = !(env && env[0] == '0'); }
-    { const char *env = getenv("HB2_SMALL_DMMA"); p->small_dmma = !(env && env[0] == '0'); }
     if (Dp == 4) {
         if (const char *env = getenv("HB2_SMALL_ILP")) p->small_ilp = atoi(env);
         int b1 = 0, b2 = 0;
@@ -1458,7 +1346,6 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
         p->small_resident[0] = std::max(b1, 1) * p->sm_count;
         p->small_resident[1] = std::max(b2, 1) * p->sm_count;
     }
-    p->fp64_walk = p->fp64_mode >= 1;
     p->have_matrix.assign(C * p->B, 0);
     p->is_rate.assign(C * p->B, 0);
     p->pend_pos.assign(C * p->B, -1);
@@ -1784,7 +1671,7 @@ int hb2_read_conditionals(hb2_partition *p, int64_t cat, int64_t inode, double *
     CU(cudaSetDevice(p->device));
     std::vector<double> tmp((size_t)p->Sp * p->Dp);
     std::vector<int> te(p->Sp);
-    const int64_t nstride = (p->use_tc && p->use_walk) ? 2 * p->I : p->I;     // node slots per class (walk: + side products)
+    const int64_t nstride = p->use_tc ? 2 * p->I : p->I;     // node slots per class (tensor walk: + side products)
     CU(cudaStreamSynchronize(p->stream));
     if (p->use_tc) {
         std::vector<float> tf(tmp.size());
@@ -1798,7 +1685,7 @@ int hb2_read_conditionals(hb2_partition *p, int64_t cat, int64_t inode, double *
     CU(cudaMemcpy(te.data(), p->d_scal + ((size_t)cat * nstride + inode) * p->Sp, te.size() * sizeof(int), cudaMemcpyDeviceToHost));
     for (int64_t s = 0; s < p->S; s++) {
         for (int64_t k = 0; k < p->D; k++) cond[s * p->D + k] = tmp[s * p->Dp + k];
-        exp2[s] = (p->use_tc && p->use_walk) ? (te[s] >> 1) : te[s];      // walk path: bit 0 is the generation tag
+        exp2[s] = p->use_tc ? (te[s] >> 1) : te[s];      // tensor walk: bit 0 is the generation tag
     }
     return 0;
 }
@@ -1821,7 +1708,7 @@ static hb2::BranchCacheArgs bc_args(hb2_partition *p, int c0, int nc) {
     hb2::BranchCacheArgs a{};
     a.cv.c64 = p->use_tc ? nullptr : p->d_cond;
     a.cv.c32 = p->use_tc ? p->d_condf : nullptr;
-    a.cv.scal = p->d_scal; a.cv.I = (int)((p->use_tc && p->use_walk) ? 2 * p->I : p->I); a.cv.Sp = (int)p->Sp; a.cv.Dp = p->Dp; a.cv.tagged = (p->use_tc && p->use_walk) ? 1 : 0;
+    a.cv.scal = p->d_scal; a.cv.I = (int)(p->use_tc ? 2 * p->I : p->I); a.cv.Sp = (int)p->Sp; a.cv.Dp = p->Dp; a.cv.tagged = p->use_tc ? 1 : 0;
     a.PT = p->d_PT; a.leaf = p->d_leaf; a.ambig = p->d_ambig; a.pi = p->d_pi; a.out = p->d_bc_out; a.outE = p->d_bc_outE;
     a.L = (int)p->L; a.B = (int)p->B; a.D = (int)p->D; a.Dp = p->Dp; a.Sp = (int)p->Sp; a.S = (int)p->S; a.cat0 = c0; a.ncls = nc;
     return a;
@@ -2094,12 +1981,11 @@ int hb2_stage_launches(const hb2_partition *p, int64_t *out3) {
 }
 const char *hb2_pruning_kernel(const hb2_partition *p) {
     if (!p) return "";
-    if (p->use_tc) return p->use_walk ? (p->walk_v2 ? "prune64_tc_walk2_kernel" : "prune64_tc_walk_kernel") : "prune64_tc_kernel";
-    if (p->Dp == 64 && p->fp64_mode == 2) return "prune64_lanes_kernel";
-    if (p->Dp == 64) return (p->fp64_walk && (int64_t)(p->Sp / hb2::TILE_P) * p->ownN >= 2 * p->sm_count) ? "prune64_walk_kernel" : "prune64_kernel";
-    if (p->small_walk && p->small_dmma && p->Dp >= 16) return "prune_small_dmma_kernel";
-    if (p->small_walk && small_two_patterns(p, p->ownN)) return "prune_small_walk_ilp_kernel";
-    return p->small_walk ? "prune_small_walk_kernel" : "prune_small_kernel";
+    if (p->use_tc) return "prune64_tc_walk_kernel";
+    if (p->Dp == 64) return "prune64_lanes_kernel";
+    if (p->Dp >= 16) return "prune_small_dmma_kernel";
+    if (small_two_patterns(p, p->ownN)) return "prune_small_walk_ilp_kernel";
+    return "prune_small_walk_kernel";
 }
 
 int hb2_time_resident(hb2_partition *p, const double *weights, const double *rootFreqs, int iters, double *msPerEval,

@@ -1,13 +1,13 @@
 // hb2_kernels_fp64.cuh -- fp64 CUDA kernels of the likelihood hot path (sm_90a).
 //
-//   expm64_kernel / expm_small_kernel   P = exp(Q t) per (branch, rate class), one CTA per matrix
-//                                       (replaces _Matrix::Exponentiate, reference matrix.cpp:5537-5951)
-//   prune64_kernel / prune_small_kernel fused Felsenstein update of one internal node for a tile of patterns:
-//                                       all children folded (leaf column gather, ambiguity mat-vec, internal
-//                                       contraction), per-pattern renormalisation, root pi-dot
-//                                       (replaces ComputeTreeBlockByBranch, reference tree_evaluator.cpp:3556-4171)
-//   combine_kernel / final_sum_kernel   rate-class mixture, log, pattern-frequency weighting, deterministic sum
-//                                       (replaces likefunc2.cpp:828-859,1446-1506 and tree_evaluator.cpp:4093-4149)
+//   expm64_dmma_kernel / expm_small_kernel  P = exp(Q t) per (branch, rate class), one CTA per matrix
+//                                           (replaces _Matrix::Exponentiate, reference matrix.cpp:5537-5951)
+//   prune_small_walk_kernel                 Felsenstein pruning pass for 4 / 8 padded states, one thread per pattern:
+//                                           all children folded (leaf column gather, ambiguity mat-vec, internal
+//                                           contraction), per-pattern renormalisation, root pi-dot
+//                                           (replaces ComputeTreeBlockByBranch, reference tree_evaluator.cpp:3556-4171)
+//   combine_kernel / final_sum_kernel       rate-class mixture, log, pattern-frequency weighting, deterministic sum
+//                                           (replaces likefunc2.cpp:828-859,1446-1506 and tree_evaluator.cpp:4093-4149)
 //
 // Device data layout (Dp = padded state count, Sp = pattern count padded to 64):
 //   PT    [C][B][Dp][Dp]   TRANSPOSED transition matrices: PT[j][k] = P(parent k -> child j); padding = 0
@@ -24,7 +24,6 @@
 
 namespace hb2 {
 
-constexpr int TILE_P = 64;          // patterns per CTA in the 64-state kernel
 constexpr int LD64 = 66;            // smem leading dimension (doubles) for 64x64 operands: conflict-free row pairs
 
 struct TreeDev {
@@ -55,54 +54,18 @@ __device__ __forceinline__ double exp2i(int e) {   // exact 2^e for |e| < 1022
 }
 
 // ------------------------------------------------------------------------------------------------
-// 64x64x64 fp64 tile product, 256 threads; thread (tx,ty) owns rows 4ty..4ty+3 and columns
-// {2tx, 2tx+1, 32+2tx, 33+2tx} of C (col_of):  acc[i][j] += sum_k A[(4*ty+i)*LD64 + k] * B[k*LD64 + col_of(tx,j)]
-// A rows are read as broadcasts (two distinct rows per warp, 16 banks apart thanks to LD64); each B read is one
-// 16-byte vector per thread, 256 contiguous bytes per half-warp: conflict-free.
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ int col_of(int tx, int j) { return (j < 2) ? 2 * tx + j : 32 + 2 * tx + (j - 2); }
-
-__device__ __forceinline__ void tile_mm64(const double *__restrict__ A, const double *__restrict__ Bm,
-                                          int tx, int ty, double (&acc)[4][4]) {
-    const double *a0 = A + (4 * ty) * LD64;
-    const double *b0 = Bm + 2 * tx;
-#pragma unroll 4
-    for (int k = 0; k < 64; k += 2) {
-        double2 a[4];
-#pragma unroll
-        for (int i = 0; i < 4; i++) a[i] = *reinterpret_cast<const double2 *>(a0 + i * LD64 + k);
-        double2 b00 = *reinterpret_cast<const double2 *>(b0 + k * LD64);
-        double2 b01 = *reinterpret_cast<const double2 *>(b0 + k * LD64 + 32);
-        double2 b10 = *reinterpret_cast<const double2 *>(b0 + (k + 1) * LD64);
-        double2 b11 = *reinterpret_cast<const double2 *>(b0 + (k + 1) * LD64 + 32);
-#pragma unroll
-        for (int i = 0; i < 4; i++) {
-            acc[i][0] = fma(a[i].x, b00.x, acc[i][0]);
-            acc[i][1] = fma(a[i].x, b00.y, acc[i][1]);
-            acc[i][2] = fma(a[i].x, b01.x, acc[i][2]);
-            acc[i][3] = fma(a[i].x, b01.y, acc[i][3]);
-            acc[i][0] = fma(a[i].y, b10.x, acc[i][0]);
-            acc[i][1] = fma(a[i].y, b10.y, acc[i][1]);
-            acc[i][2] = fma(a[i].y, b11.x, acc[i][2]);
-            acc[i][3] = fma(a[i].y, b11.y, acc[i][3]);
-        }
-    }
-}
-
-// ------------------------------------------------------------------------------------------------
-// Matrix exponential, 64-padded states.  One CTA (256 threads) per matrix.
+// Matrix exponential.  One CTA per matrix (expm64_dmma_kernel, expm_small_kernel), or the shared-powers path below.
 //   in : Q [n][D*D] row-major rate matrices (Q*t, diagonal = -rowsum), dst[n] = slot index into PT
 //   out: PT[slot] = exp(Q)^T with padding rows/cols zeroed, negatives clamped, columns repaired to sum to 1
-// Algorithm (engine's own, same result as the reference's Taylor+squaring to ~1e-15): scale by 2^-s so that
-// ||A||_inf <= 1, degree-15 Taylor polynomial by Paterson-Stockmeyer with A^2,A^3,A^4 (6 products), s squarings.
-// mix_w != nullptr: PT[slot] (+)= w * result, used for explicit-form mixtures (sum_k w_k Exp(Q_k)).
+// Algorithm (engine's own, same result as the reference's Taylor+squaring to ~1e-15): scale by 2^-s, Taylor polynomial
+// by Paterson-Stockmeyer, s squarings.
 // ------------------------------------------------------------------------------------------------
 struct ExpmArgs {
     const double *Q;        // [n][D*D]
     const int *dst;         // [n] destination slot; < 0: retired entry (the slot was handed over again), skipped
     double *PT;
     const double *colsum;   // nullable [n][16][64]: column-sum partials of expm_poly_kernel; non-null = expm64_dmma_kernel also
-                            // does the row repair of the entries that kernel finished (no separate expm_diag_kernel launch)
+                            // does the row repair of the entries that kernel finished
     double *Qres;           // nullable [slots][D*D]: resident copy of the rate matrices, written while loading
     int D;
     int is_trans;           // 1: input already a transition matrix -> just transpose/pad
@@ -183,119 +146,8 @@ __constant__ double c_taylor[16] = {1.0, 1.0, 0.5, 1.0 / 6, 1.0 / 24, 1.0 / 120,
                                     1.0 / 87178291200.0, 1.0 / 1307674368000.0};
 __device__ __forceinline__ double taylor_c(int k) { return c_taylor[k]; }
 
-__global__ void __launch_bounds__(256, 1) expm64_kernel(ExpmArgs a) {
-    extern __shared__ __align__(16) double sm[];
-    double *A1 = sm, *A2 = A1 + 64 * LD64, *A3 = A2 + 64 * LD64, *A4 = A3 + 64 * LD64, *R = A4 + 64 * LD64;
-    __shared__ double red[64];
-    __shared__ int s_shift;
-    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-    const int D = a.D;
-    if (a.dst[blockIdx.x] < 0) return;
-    double *out = a.PT + (size_t)a.dst[blockIdx.x] * 4096;
-
-    load_rate_matrix<64, LD64, 256>(a, A1, tid);
-    if (a.is_trans) {
-        for (int idx = tid; idx < 4096; idx += 256) out[idx] = A1[(idx >> 6) * LD64 + (idx & 63)];
-        return;
-    }
-    // ||A||_1 of A^T == ||Q||_inf: max over columns i of sum_j |A1[j][i]|
-    if (tid < 64) {
-        double s = 0.0;
-        for (int j = 0; j < 64; j++) s += fabs(A1[j * LD64 + tid]);
-        red[tid] = s;
-    }
-    __syncthreads();
-    if (tid == 0) {
-        double m = 0.0;
-        bool bad = false;
-        for (int i = 0; i < 64; i++) { if (!(red[i] == red[i]) || isinf(red[i])) bad = true; m = fmax(m, red[i]); }
-        int e = 0;
-        if (m > 0.0) frexp(m, &e);
-        s_shift = bad ? -1 : max(e, 0);
-    }
-    __syncthreads();
-    const int shift = s_shift;
-    if (shift < 0 || shift > 900) {           // NaN/inf or absurd rates: propagate NaN (host sees NaN lnL)
-        for (int idx = tid; idx < 4096; idx += 256) out[idx] = __longlong_as_double(0x7ff8000000000000LL);
-        return;
-    }
-    if (shift > 0) {
-        const double sc = exp2i(-shift);
-        for (int idx = tid; idx < 64 * 64; idx += 256) A1[(idx >> 6) * LD64 + (idx & 63)] *= sc;
-        __syncthreads();
-    }
-    double acc[4][4];
-    auto zero = [&]() {
-#pragma unroll
-        for (int i = 0; i < 4; i++)
-#pragma unroll
-            for (int j = 0; j < 4; j++) acc[i][j] = 0.0;
-    };
-    auto store = [&](double *M) {
-#pragma unroll
-        for (int i = 0; i < 4; i++)
-#pragma unroll
-            for (int j = 0; j < 4; j += 2)
-                *reinterpret_cast<double2 *>(M + (4 * ty + i) * LD64 + col_of(tx, j)) = make_double2(acc[i][j], acc[i][j + 1]);
-    };
-    zero(); tile_mm64(A1, A1, tx, ty, acc); store(A2);
-    __syncthreads();
-    zero(); tile_mm64(A2, A1, tx, ty, acc); store(A3);
-    zero(); tile_mm64(A2, A2, tx, ty, acc); store(A4);
-    // R = B3 = c12 I + c13 A + c14 A2 + c15 A3
-    auto poly_block = [&](int q, int i, int j) -> double {
-        int r = 4 * ty + i, c = col_of(tx, j), o = r * LD64 + c;
-        double v = taylor_c(4 * q + 1) * A1[o] + taylor_c(4 * q + 2) * A2[o];
-        if (r == c) v += taylor_c(4 * q);
-        return v;   // the A3 term is added by the caller after the barrier that publishes A3
-    };
-    __syncthreads();
-#pragma unroll
-    for (int i = 0; i < 4; i++)
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-            int o = (4 * ty + i) * LD64 + col_of(tx, j);
-            R[o] = poly_block(3, i, j) + taylor_c(15) * A3[o];
-        }
-    __syncthreads();
-    for (int q = 2; q >= 0; q--) {               // R = R*A4 + B_q   (all matrices are polynomials in A: they commute)
-        zero(); tile_mm64(R, A4, tx, ty, acc);
-        __syncthreads();
-#pragma unroll
-        for (int i = 0; i < 4; i++)
-#pragma unroll
-            for (int j = 0; j < 4; j++) {
-                int o = (4 * ty + i) * LD64 + col_of(tx, j);
-                R[o] = acc[i][j] + poly_block(q, i, j) + taylor_c(4 * q + 3) * A3[o];
-            }
-        __syncthreads();
-    }
-    for (int s = 0; s < shift; s++) {            // squarings
-        zero(); tile_mm64(R, R, tx, ty, acc);
-        __syncthreads();
-        store(R);
-        __syncthreads();
-    }
-    // clamp negatives, zero the padding, repair: column k of PT (= row k of P) must sum to 1
-    for (int idx = tid; idx < 64 * 64; idx += 256) {
-        int j = idx >> 6, k = idx & 63;
-        double v = R[j * LD64 + k];
-        if (j >= D || k >= D) v = 0.0; else if (v < 0.0) v = 0.0;
-        R[j * LD64 + k] = v;
-    }
-    __syncthreads();
-    if (tid < 64) {
-        double s = 0.0;
-        for (int j = 0; j < 64; j++) if (j != tid) s += R[j * LD64 + tid];
-        if (tid < D) R[tid * LD64 + tid] = fmax(1.0 - s, 0.0);
-    }
-    __syncthreads();
-    for (int idx = tid; idx < 4096; idx += 256) out[idx] = R[(idx >> 6) * LD64 + (idx & 63)];
-}
-
-
 // ------------------------------------------------------------------------------------------------
-// expm64_dmma_kernel: same contract as expm64_kernel, products on the FP64 tensor pipe (mma.sync.m8n8k4.f64, DMMA)
+// expm64_dmma_kernel: 64 padded states, products on the FP64 tensor pipe (mma.sync.m8n8k4.f64, DMMA)
 // and a Paterson-Stockmeyer polynomial whose degree follows the norm:
 //   p(A) = sum_{q=0..Q} A3^q * (c_{3q} I + c_{3q+1} A + c_{3q+2} A2),   A3 = A^3,   degree 3Q+2,   2+Q products,
 //   Q chosen so that theta^(3Q+3)/(3Q+3)! <= 1e-16 with theta = ||A||/2^s <= 0.975; s squarings follow.
@@ -469,7 +321,7 @@ __global__ void __launch_bounds__(256, 2) expm64_dmma_kernel(ExpmArgs a, ExpmTcO
         const double rho = gi.nu * (a.weight[blockIdx.x] / gi.weight);
         int shift = 0;
         if (rho > EXPM_POLY_THETA) { int e = 0; frexp(rho / EXPM_POLY_THETA, &e); shift = max(e, 0); }
-        if (shift == 0 && rho == rho) {          // finished by expm_poly_kernel up to the row repair (expm_diag_kernel's arithmetic)
+        if (shift == 0 && rho == rho) {          // finished by expm_poly_kernel up to the row repair
             if (a.colsum && tid < 64) {
                 const int col = tid;
                 double s = 0.0;
@@ -759,7 +611,7 @@ __global__ void __launch_bounds__(256, 1) expm_powers_kernel(ExpmPowersArgs pa) 
 //   shift == 0: the value is final up to the row repair.  It is clamped at 0, padding is zeroed, and PT (fp64), PTf (fp32
 //               table) and PB (tf32 hi/lo tiles; chunk sl of the canonical layout is exactly this slice, offset t) are
 //               written directly; the partial column sums of the slice (4 rows, diagonal excluded; 4 adjacent lanes) go to
-//               colsum[entry][sl][column] for expm_diag_kernel, which sets the diagonal to 1 - (sum of the rest of P's row).
+//               colsum[entry][sl][column] for expm64_dmma_kernel, which sets the diagonal to 1 - (sum of the rest of P's row).
 //   shift  > 0: the raw polynomial value goes to PT; expm64_dmma_kernel squares and finishes the entry.
 // ------------------------------------------------------------------------------------------------
 constexpr int EXPM_POLY_CHUNK = 8;
@@ -824,7 +676,7 @@ __global__ void __launch_bounds__(256, 3) expm_poly_kernel(ExpmArgs a, ExpmTcOut
         part += __shfl_xor_sync(0xffffffffu, part, 1);
         part += __shfl_xor_sync(0xffffffffu, part, 2);
         if ((tid & 3) == 0) colsum[((size_t)(k0 + i) * 16 + sl) * 64 + col] = part;
-        if (row != col) {                                             // expm_diag_kernel owns the diagonal
+        if (row != col) {                                             // expm64_dmma_kernel owns the diagonal
             __stcg(a.PT + sidx * 4096 + out_pt, v);
             if (tc.PB) {
                 const float vf = (float)v;
@@ -835,30 +687,6 @@ __global__ void __launch_bounds__(256, 3) expm_poly_kernel(ExpmArgs a, ExpmTcOut
                 pb[4096] = tf32_rn_dev((float)(v - (double)hi));
             }
         }
-    }
-}
-
-// Row repair of the entries expm_poly_kernel finished (flagged, no squaring): P[k][k] = max(1 - sum_{j != k} P[k][j], 0),
-// i.e. PT[k][k] from the column sums of PT, added up in slice order (deterministic).  One CTA of 64 threads per entry.
-__global__ void __launch_bounds__(64) expm_diag_kernel(ExpmArgs a, ExpmTcOut tc, const double *__restrict__ colsum) {
-    const int k = blockIdx.x, col = threadIdx.x;
-    const int slot = a.dst[k];
-    if (slot < 0 || !a.flag[k]) return;
-    const ExpmGroup gi = a.groups[a.group[k]];
-    const double rho = gi.nu * (a.weight[k] / gi.weight);
-    if (!(rho <= EXPM_POLY_THETA)) return;                            // squared and finished by expm64_dmma_kernel
-    double s = 0.0;
-#pragma unroll
-    for (int sl = 0; sl < 16; sl++) s += colsum[((size_t)k * 16 + sl) * 64 + col];
-    const double d = col < a.D ? fmax(1.0 - s, 0.0) : 0.0;
-    const size_t sidx = (size_t)slot;
-    a.PT[sidx * 4096 + col * 64 + col] = d;
-    if (tc.PB) {
-        tc.PTf[sidx * 4352 + col * 68 + col] = (float)d;
-        const float hi = tf32_rn_dev((float)d);
-        float *pb = tc.PB + sidx * 8192 + (col >> 2) * 256 + col * 4 + (col & 3);
-        pb[0] = hi;
-        pb[4096] = tf32_rn_dev((float)(d - (double)hi));
     }
 }
 
@@ -948,332 +776,9 @@ __global__ void __launch_bounds__(128) expm_small_kernel(ExpmArgs a) {
     for (int idx = tid; idx < DP * DP; idx += 128) out[idx] = R[(idx / DP) * LD + idx % DP];
 }
 
-// ------------------------------------------------------------------------------------------------
-// Fused pruning update, 33..64 states (codon models), fp64.
-// grid = (Sp/64, jobs, classes); block = 256 threads as a 16x16 grid, thread (tx,ty) owns patterns 4ty..4ty+3
-// and parent states 4tx..4tx+3 of the tile.  jobs[blockIdx.y] = internal index of the parent to (re)compute.
-// ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256, 2) prune64_kernel(PruneArgs a, const int *__restrict__ jobs) {
-    extern __shared__ __align__(16) double sm[];
-    double *Xs = sm;                    // [64][LD64] child conditionals (pattern-major)
-    double *Ps = sm + 64 * LD64;        // [64][LD64] PT of the child's branch
-    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-    const int par = jobs[blockIdx.y];
-    const int cat = a.cat0 + blockIdx.z;
-    const int s0 = blockIdx.x * TILE_P;
-    const size_t Sp = a.Sp;
-    double v[4][4];
-    int ex[4];
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-        ex[i] = 0;
-#pragma unroll
-        for (int j = 0; j < 4; j++) v[i][j] = 1.0;
-    }
-    const int c_begin = a.tree.child_start[par], c_end = a.tree.child_start[par + 1];
-    for (int ci = c_begin; ci < c_end; ci++) {
-        const int child = a.tree.child_ids[ci];
-        const double *PT = a.PT + ((size_t)cat * a.B + child) * 4096;
-        if (child < a.L) {
-            // leaf: column gather PT[state][k]; ambiguous: sum_j amb[j] PT[j][k]
-#pragma unroll
-            for (int i = 0; i < 4; i++) {
-                const int code = (child == a.forced_node) ? a.forced[s0 + 4 * ty + i] : a.leaf[(size_t)child * Sp + s0 + 4 * ty + i];
-                double m0, m1, m2, m3;
-                if (code >= 0) {
-                    const double2 *p = reinterpret_cast<const double2 *>(PT + (size_t)code * 64 + 2 * tx);
-                    double2 q0 = __ldg(p), q1 = __ldg(p + 16);
-                    m0 = q0.x; m1 = q0.y; m2 = q1.x; m3 = q1.y;
-                } else {
-                    const double *amb = a.ambig + (size_t)(-code - 1) * 64;
-                    m0 = m1 = m2 = m3 = 0.0;
-                    for (int j = 0; j < a.D; j++) {
-                        const double w = __ldg(amb + j);
-                        if (w != 0.0) {
-                            const double2 *p = reinterpret_cast<const double2 *>(PT + (size_t)j * 64 + 2 * tx);
-                            double2 q0 = __ldg(p), q1 = __ldg(p + 16);
-                            m0 = fma(w, q0.x, m0); m1 = fma(w, q0.y, m1); m2 = fma(w, q1.x, m2); m3 = fma(w, q1.y, m3);
-                        }
-                    }
-                }
-                v[i][0] *= m0; v[i][1] *= m1; v[i][2] *= m2; v[i][3] *= m3;
-            }
-        } else {
-            const int cin = child - a.L;
-            const double *X = a.cond + (((size_t)cat * a.I + cin) * Sp + s0) * 64;
-            __syncthreads();            // previous child's tiles fully consumed
-            for (int idx = tid; idx < 2048; idx += 256) {       // 4096 doubles as double2, coalesced
-                const int r = idx >> 5, c2 = (idx & 31) * 2;
-                *reinterpret_cast<double2 *>(Xs + r * LD64 + c2) = *reinterpret_cast<const double2 *>(X + r * 64 + c2);
-                *reinterpret_cast<double2 *>(Ps + r * LD64 + c2) = __ldg(reinterpret_cast<const double2 *>(PT + r * 64 + c2));
-            }
-            __syncthreads();
-            double acc[4][4];
-#pragma unroll
-            for (int i = 0; i < 4; i++)
-#pragma unroll
-                for (int j = 0; j < 4; j++) acc[i][j] = 0.0;
-            tile_mm64(Xs, Ps, tx, ty, acc);
-            const int *sc = a.scal + ((size_t)cat * a.I + cin) * Sp + s0 + 4 * ty;
-#pragma unroll
-            for (int i = 0; i < 4; i++) {
-                ex[i] += sc[i];
-#pragma unroll
-                for (int j = 0; j < 4; j++) v[i][j] *= acc[i][j];
-            }
-        }
-    }
-    if (a.L + par == a.forced_node) {            // pinned internal node: only the forced state survives
-#pragma unroll
-        for (int i = 0; i < 4; i++) {
-            const int f = a.forced[s0 + 4 * ty + i];
-#pragma unroll
-            for (int j = 0; j < 4; j++) if (col_of(tx, j) != f) v[i][j] = 0.0;
-        }
-    }
-    // per-pattern renormalisation: exact power of two so that max_k lands in [0.5, 1)
-    const bool is_root = (par == a.I - 1);
-    double *outp = a.cond + (((size_t)cat * a.I + par) * Sp + s0) * 64;
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-        double m = fmax(fmax(v[i][0], v[i][1]), fmax(v[i][2], v[i][3]));
-#pragma unroll
-        for (int o = 1; o < 16; o <<= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
-        int e = 0;
-        if (m > 0.0 && m < INFINITY) {
-            e = ilogb(m) + 1;
-            const double s1 = exp2i(-(e / 2)), s2 = exp2i(-(e - e / 2));   // two steps: |e| may exceed 1022
-#pragma unroll
-            for (int j = 0; j < 4; j++) v[i][j] = v[i][j] * s1 * s2;
-        }
-        ex[i] += e;
-        const int row = 4 * ty + i;
-        *reinterpret_cast<double2 *>(outp + (size_t)row * 64 + 2 * tx) = make_double2(v[i][0], v[i][1]);
-        *reinterpret_cast<double2 *>(outp + (size_t)row * 64 + 32 + 2 * tx) = make_double2(v[i][2], v[i][3]);
-        if (tx == 0) a.scal[((size_t)cat * a.I + par) * Sp + s0 + row] = ex[i];
-        if (is_root) {
-            double r = v[i][0] * a.pi[2 * tx] + v[i][1] * a.pi[2 * tx + 1] + v[i][2] * a.pi[32 + 2 * tx] + v[i][3] * a.pi[33 + 2 * tx];
-#pragma unroll
-            for (int o = 1; o < 16; o <<= 1) r += __shfl_xor_sync(0xffffffffu, r, o);
-            if (tx == 0) {
-                a.rootL[(size_t)cat * Sp + s0 + row] = r;
-                a.rootE[(size_t)cat * Sp + s0 + row] = ex[i];
-            }
-        }
-    }
-}
 
 // ------------------------------------------------------------------------------------------------
-// 33..64 states, fp64, WHOLE pruning pass in one launch: patterns are independent, so tile t of a node needs tile t of its
-// children only -- CTA (tile, class) walks the dirty internal nodes in post-order (jobs ascending) and every dependency is
-// CTA-local (a child's tile was written by this CTA earlier in the launch, or is resident from an earlier evaluation).  No
-// grid-wide synchronisation, no launch per tree level (the north-star tree has 48 levels: 54 launches per evaluation
-// before).  Same tile body as prune64_kernel.  grid = (Sp/64, classes).
-// ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256, 2) prune64_walk_kernel(PruneArgs a, const int *__restrict__ jobs, int njobs) {
-    extern __shared__ __align__(16) double sm[];
-    double *Xs = sm;                    // [64][LD64] child conditionals (pattern-major)
-    double *Ps = sm + 64 * LD64;        // [64][LD64] PT of the child's branch
-    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-    const int cat = a.cat0 + blockIdx.y;
-    const int s0 = blockIdx.x * TILE_P;
-    const size_t Sp = a.Sp;
-  for (int jb = 0; jb < njobs; jb++) {
-    const int par = __ldg(jobs + jb);
-    double v[4][4];
-    int ex[4];
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-        ex[i] = 0;
-#pragma unroll
-        for (int j = 0; j < 4; j++) v[i][j] = 1.0;
-    }
-    const int c_begin = a.tree.child_start[par], c_end = a.tree.child_start[par + 1];
-    for (int ci = c_begin; ci < c_end; ci++) {
-        const int child = a.tree.child_ids[ci];
-        const double *PT = a.PT + ((size_t)cat * a.B + child) * 4096;
-        if (child < a.L) {
-            // leaf: column gather PT[state][k]; ambiguous: sum_j amb[j] PT[j][k]
-#pragma unroll
-            for (int i = 0; i < 4; i++) {
-                const int code = (child == a.forced_node) ? a.forced[s0 + 4 * ty + i] : a.leaf[(size_t)child * Sp + s0 + 4 * ty + i];
-                double m0, m1, m2, m3;
-                if (code >= 0) {
-                    const double2 *p = reinterpret_cast<const double2 *>(PT + (size_t)code * 64 + 2 * tx);
-                    double2 q0 = __ldg(p), q1 = __ldg(p + 16);
-                    m0 = q0.x; m1 = q0.y; m2 = q1.x; m3 = q1.y;
-                } else {
-                    const double *amb = a.ambig + (size_t)(-code - 1) * 64;
-                    m0 = m1 = m2 = m3 = 0.0;
-                    for (int j = 0; j < a.D; j++) {
-                        const double w = __ldg(amb + j);
-                        if (w != 0.0) {
-                            const double2 *p = reinterpret_cast<const double2 *>(PT + (size_t)j * 64 + 2 * tx);
-                            double2 q0 = __ldg(p), q1 = __ldg(p + 16);
-                            m0 = fma(w, q0.x, m0); m1 = fma(w, q0.y, m1); m2 = fma(w, q1.x, m2); m3 = fma(w, q1.y, m3);
-                        }
-                    }
-                }
-                v[i][0] *= m0; v[i][1] *= m1; v[i][2] *= m2; v[i][3] *= m3;
-            }
-        } else {
-            const int cin = child - a.L;
-            const double *X = a.cond + (((size_t)cat * a.I + cin) * Sp + s0) * 64;
-            __syncthreads();            // previous child's tiles fully consumed
-            for (int idx = tid; idx < 2048; idx += 256) {       // 4096 doubles as double2, coalesced
-                const int r = idx >> 5, c2 = (idx & 31) * 2;
-                *reinterpret_cast<double2 *>(Xs + r * LD64 + c2) = *reinterpret_cast<const double2 *>(X + r * 64 + c2);
-                *reinterpret_cast<double2 *>(Ps + r * LD64 + c2) = __ldg(reinterpret_cast<const double2 *>(PT + r * 64 + c2));
-            }
-            __syncthreads();
-            double acc[4][4];
-#pragma unroll
-            for (int i = 0; i < 4; i++)
-#pragma unroll
-                for (int j = 0; j < 4; j++) acc[i][j] = 0.0;
-            tile_mm64(Xs, Ps, tx, ty, acc);
-            const int *sc = a.scal + ((size_t)cat * a.I + cin) * Sp + s0 + 4 * ty;
-#pragma unroll
-            for (int i = 0; i < 4; i++) {
-                ex[i] += sc[i];
-#pragma unroll
-                for (int j = 0; j < 4; j++) v[i][j] *= acc[i][j];
-            }
-        }
-    }
-    if (a.L + par == a.forced_node) {            // pinned internal node: only the forced state survives
-#pragma unroll
-        for (int i = 0; i < 4; i++) {
-            const int f = a.forced[s0 + 4 * ty + i];
-#pragma unroll
-            for (int j = 0; j < 4; j++) if (col_of(tx, j) != f) v[i][j] = 0.0;
-        }
-    }
-    // per-pattern renormalisation: exact power of two so that max_k lands in [0.5, 1)
-    const bool is_root = (par == a.I - 1);
-    double *outp = a.cond + (((size_t)cat * a.I + par) * Sp + s0) * 64;
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-        double m = fmax(fmax(v[i][0], v[i][1]), fmax(v[i][2], v[i][3]));
-#pragma unroll
-        for (int o = 1; o < 16; o <<= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
-        int e = 0;
-        if (m > 0.0 && m < INFINITY) {
-            e = ilogb(m) + 1;
-            const double s1 = exp2i(-(e / 2)), s2 = exp2i(-(e - e / 2));   // two steps: |e| may exceed 1022
-#pragma unroll
-            for (int j = 0; j < 4; j++) v[i][j] = v[i][j] * s1 * s2;
-        }
-        ex[i] += e;
-        const int row = 4 * ty + i;
-        *reinterpret_cast<double2 *>(outp + (size_t)row * 64 + 2 * tx) = make_double2(v[i][0], v[i][1]);
-        *reinterpret_cast<double2 *>(outp + (size_t)row * 64 + 32 + 2 * tx) = make_double2(v[i][2], v[i][3]);
-        if (tx == 0) a.scal[((size_t)cat * a.I + par) * Sp + s0 + row] = ex[i];
-        if (is_root) {
-            double r = v[i][0] * a.pi[2 * tx] + v[i][1] * a.pi[2 * tx + 1] + v[i][2] * a.pi[32 + 2 * tx] + v[i][3] * a.pi[33 + 2 * tx];
-#pragma unroll
-            for (int o = 1; o < 16; o <<= 1) r += __shfl_xor_sync(0xffffffffu, r, o);
-            if (tx == 0) {
-                a.rootL[(size_t)cat * Sp + s0 + row] = r;
-                a.rootE[(size_t)cat * Sp + s0 + row] = ex[i];
-            }
-        }
-    }
-    __syncthreads();                 // this node's tile (global) is visible to the whole CTA before a parent reads it
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// Fused pruning update for small state spaces (Dp in {4,8,16,24,32}): one thread per pattern.
-// grid = (Sp/128, jobs, classes), block = 128.  PT of each child is staged in shared memory (broadcast reads).
-// ------------------------------------------------------------------------------------------------
-template <int DP>
-__global__ void __launch_bounds__(128) prune_small_kernel(PruneArgs a, const int *__restrict__ jobs) {
-    __shared__ double Ps[DP * DP];
-    const int tid = threadIdx.x;
-    const int par = jobs[blockIdx.y];
-    const int cat = a.cat0 + blockIdx.z;
-    const size_t Sp = a.Sp;
-    const size_t s = (size_t)blockIdx.x * 128 + tid;       // Sp is a multiple of 128 for the small kernels
-    double v[DP];
-#pragma unroll
-    for (int k = 0; k < DP; k++) v[k] = 1.0;
-    int ex = 0;
-    const int c_begin = a.tree.child_start[par], c_end = a.tree.child_start[par + 1];
-    for (int ci = c_begin; ci < c_end; ci++) {
-        const int child = a.tree.child_ids[ci];
-        const double *PT = a.PT + ((size_t)cat * a.B + child) * DP * DP;
-        __syncthreads();
-        for (int idx = tid; idx < DP * DP; idx += 128) Ps[idx] = __ldg(PT + idx);
-        __syncthreads();
-        if (child < a.L) {
-            const int code = (child == a.forced_node) ? a.forced[s] : a.leaf[(size_t)child * Sp + s];
-            if (code >= 0) {
-#pragma unroll
-                for (int k = 0; k < DP; k++) v[k] *= Ps[code * DP + k];
-            } else {
-                const double *amb = a.ambig + (size_t)(-code - 1) * DP;
-                double acc[DP];
-#pragma unroll
-                for (int k = 0; k < DP; k++) acc[k] = 0.0;
-                for (int j = 0; j < a.D; j++) {
-                    const double w = __ldg(amb + j);
-#pragma unroll
-                    for (int k = 0; k < DP; k++) acc[k] = fma(w, Ps[j * DP + k], acc[k]);
-                }
-#pragma unroll
-                for (int k = 0; k < DP; k++) v[k] *= acc[k];
-            }
-        } else {
-            const int cin = child - a.L;
-            const double *X = a.cond + (((size_t)cat * a.I + cin) * Sp + s) * DP;
-            double acc[DP];
-#pragma unroll
-            for (int k = 0; k < DP; k++) acc[k] = 0.0;
-#pragma unroll
-            for (int j = 0; j < DP; j += 2) {
-                const double2 x = *reinterpret_cast<const double2 *>(X + j);
-#pragma unroll
-                for (int k = 0; k < DP; k++) acc[k] = fma(x.x, Ps[j * DP + k], acc[k]);
-#pragma unroll
-                for (int k = 0; k < DP; k++) acc[k] = fma(x.y, Ps[(j + 1) * DP + k], acc[k]);
-            }
-#pragma unroll
-            for (int k = 0; k < DP; k++) v[k] *= acc[k];
-            ex += a.scal[((size_t)cat * a.I + cin) * Sp + s];
-        }
-    }
-    if (a.L + par == a.forced_node) {
-        const int f = a.forced[s];
-#pragma unroll
-        for (int k = 0; k < DP; k++) if (k != f) v[k] = 0.0;
-    }
-    double m = 0.0;
-#pragma unroll
-    for (int k = 0; k < DP; k++) m = fmax(m, v[k]);
-    if (m > 0.0 && m < INFINITY) {
-        const int e = ilogb(m) + 1;
-        const double s1 = exp2i(-(e / 2)), s2 = exp2i(-(e - e / 2));
-#pragma unroll
-        for (int k = 0; k < DP; k++) v[k] = v[k] * s1 * s2;
-        ex += e;
-    }
-    double *outp = a.cond + (((size_t)cat * a.I + par) * Sp + s) * DP;
-#pragma unroll
-    for (int k = 0; k < DP; k += 2) *reinterpret_cast<double2 *>(outp + k) = make_double2(v[k], v[k + 1]);
-    a.scal[((size_t)cat * a.I + par) * Sp + s] = ex;
-    if (par == a.I - 1) {
-        double r = 0.0;
-#pragma unroll
-        for (int k = 0; k < DP; k++) r = fma(v[k], a.pi[k], r);
-        a.rootL[(size_t)cat * Sp + s] = r;
-        a.rootE[(size_t)cat * Sp + s] = ex;
-    }
-}
-
-
-// ------------------------------------------------------------------------------------------------
-// Small state spaces, whole pruning pass in ONE launch: thread s owns pattern s and walks the dirty internal nodes in
+// 4 / 8 padded states, whole pruning pass in ONE launch: thread s owns pattern s and walks the dirty internal nodes in
 // post-order.  Every dependency is thread-local (a child's conditionals were written by the same thread earlier in the
 // same launch, or are a valid cache from an earlier evaluation), so there is no synchronisation of any kind; P^T of a
 // branch is read by all threads at the same address (L1 broadcast).  HBM traffic per evaluation is the algorithmic
@@ -1283,19 +788,16 @@ __global__ void __launch_bounds__(128) prune_small_kernel(PruneArgs a, const int
 // (Forcing 16 CTAs/SM for 4 states -- 32 registers, spills -- was slower.)
 template <int DP>
 __global__ void __launch_bounds__(128) prune_small_walk_kernel(PruneArgs a, const int *__restrict__ jobs, int njobs) {
-    // 16..32 states: the branch's P^T is staged in shared memory once per child (all threads of the CTA walk the same
-    // job list in lockstep) and read as broadcasts; 4/8 states read the 16/64 doubles straight through L1.
-    constexpr bool kStage = DP > 8;
+    // P^T of a branch (16 / 64 doubles) is read straight through L1; 16..32 states run prune_small_dmma_kernel.
+    static_assert(DP <= 8, "one thread per pattern is used for 4 and 8 padded states only");
     // The node computed by the previous job is, in post-order, very often a child of the current one (every node follows
     // its last child): its vector is handed over in registers instead of being re-read from L2 (the thread would wait a
-    // full L2 round trip for data it wrote a moment ago).  Register budget allows it up to 24 padded states.
-    constexpr bool kChain = DP <= 24;
-    __shared__ double Ps[kStage ? DP * DP : 1];
+    // full L2 round trip for data it wrote a moment ago).
     const int tid = threadIdx.x;
     const int cat = a.cat0 + blockIdx.y;
     const size_t Sp = a.Sp;
     const size_t s = (size_t)blockIdx.x * 128 + tid;
-    double pv[kChain ? DP : 1];
+    double pv[DP];
     int prev = -1, pex = 0;
     for (int jb = 0; jb < njobs; jb++) {
         const int par = __ldg(jobs + jb);
@@ -1306,21 +808,13 @@ __global__ void __launch_bounds__(128) prune_small_walk_kernel(PruneArgs a, cons
         const int c_begin = __ldg(a.tree.child_start + par), c_end = __ldg(a.tree.child_start + par + 1);
         for (int ci = c_begin; ci < c_end; ci++) {
             const int child = __ldg(a.tree.child_ids + ci);
-            const double *PTg = a.PT + ((size_t)cat * a.B + child) * DP * DP;
-            const double *PT = PTg;
-            if (kStage) {
-                __syncthreads();
-                for (int idx = tid; idx < DP * DP / 2; idx += 128)
-                    reinterpret_cast<double2 *>(Ps)[idx] = __ldg(reinterpret_cast<const double2 *>(PTg) + idx);
-                __syncthreads();
-                PT = Ps;
-            }
+            const double *PT = a.PT + ((size_t)cat * a.B + child) * DP * DP;
             if (child < a.L) {
                 const int code = (child == a.forced_node) ? __ldg(a.forced + s) : __ldg(a.leaf + (size_t)child * Sp + s);
                 if (code >= 0) {
                     const double2 *row = reinterpret_cast<const double2 *>(PT + (size_t)code * DP);
 #pragma unroll
-                    for (int k = 0; k < DP; k += 2) { const double2 r = kStage ? row[k / 2] : __ldg(row + k / 2); v[k] *= r.x; v[k + 1] *= r.y; }
+                    for (int k = 0; k < DP; k += 2) { const double2 r = __ldg(row + k / 2); v[k] *= r.x; v[k + 1] *= r.y; }
                 } else {
                     const double *amb = a.ambig + (size_t)(-code - 1) * DP;
                     double acc[DP];
@@ -1330,7 +824,7 @@ __global__ void __launch_bounds__(128) prune_small_walk_kernel(PruneArgs a, cons
                         const double wgt = __ldg(amb + j);
                         const double2 *row = reinterpret_cast<const double2 *>(PT + (size_t)j * DP);
 #pragma unroll
-                        for (int k = 0; k < DP; k += 2) { const double2 r = kStage ? row[k / 2] : __ldg(row + k / 2); acc[k] = fma(wgt, r.x, acc[k]); acc[k + 1] = fma(wgt, r.y, acc[k + 1]); }
+                        for (int k = 0; k < DP; k += 2) { const double2 r = __ldg(row + k / 2); acc[k] = fma(wgt, r.x, acc[k]); acc[k + 1] = fma(wgt, r.y, acc[k + 1]); }
                     }
 #pragma unroll
                     for (int k = 0; k < DP; k++) v[k] *= acc[k];
@@ -1338,7 +832,7 @@ __global__ void __launch_bounds__(128) prune_small_walk_kernel(PruneArgs a, cons
             } else {
                 const int cin = child - a.L;
                 double x[DP];
-                if (kChain && cin == prev) {
+                if (cin == prev) {
 #pragma unroll
                     for (int j = 0; j < DP; j++) x[j] = pv[j];
                     ex += pex;
@@ -1355,7 +849,7 @@ __global__ void __launch_bounds__(128) prune_small_walk_kernel(PruneArgs a, cons
                 for (int j = 0; j < DP; j++) {
                     const double2 *row = reinterpret_cast<const double2 *>(PT + (size_t)j * DP);
 #pragma unroll
-                    for (int k = 0; k < DP; k += 2) { const double2 r = kStage ? row[k / 2] : __ldg(row + k / 2); acc[k] = fma(x[j], r.x, acc[k]); acc[k + 1] = fma(x[j], r.y, acc[k + 1]); }
+                    for (int k = 0; k < DP; k += 2) { const double2 r = __ldg(row + k / 2); acc[k] = fma(x[j], r.x, acc[k]); acc[k + 1] = fma(x[j], r.y, acc[k + 1]); }
                 }
 #pragma unroll
                 for (int k = 0; k < DP; k++) v[k] *= acc[k];
@@ -1380,11 +874,9 @@ __global__ void __launch_bounds__(128) prune_small_walk_kernel(PruneArgs a, cons
 #pragma unroll
         for (int k = 0; k < DP; k += 2) outp[k / 2] = make_double2(v[k], v[k + 1]);
         a.scal[((size_t)cat * a.I + par) * Sp + s] = ex;
-        if (kChain) {
 #pragma unroll
-            for (int k = 0; k < DP; k++) pv[k] = v[k];
-            prev = par; pex = ex;
-        }
+        for (int k = 0; k < DP; k++) pv[k] = v[k];
+        prev = par; pex = ex;
         if (par == a.I - 1) {
             double r = 0.0;
 #pragma unroll

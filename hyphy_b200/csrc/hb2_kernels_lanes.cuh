@@ -1,8 +1,6 @@
 // hb2_kernels_lanes.cuh -- fp64 pruning pass for 33..64 states in ONE launch with K in-order lanes per (class, tile).
 //
-// Replaces, for the double-precision path, both the per-level launches of prune64_kernel (54 launches on the north-star
-// tree, each bound by launch + load latency) and prune64_walk_kernel (one CTA per (class, tile) walking ALL dirty nodes
-// serially).  Same decomposition as the tensor walk kernel (hb2_kernels_tc.cuh): the host planner (hb2_engine.cu
+// Same decomposition as the tensor walk kernel (hb2_kernels_tc.cuh): the host planner (hb2_engine.cu
 // plan_walk) list-schedules the dirty jobs -- nodes and side products of nodes with two internal children -- on K lanes;
 // CTA (class c, 32-pattern tile t, lane r) executes its lane's steps back to back.  Reference semantics:
 // ComputeTreeBlockByBranch (tree_evaluator.cpp:3556-4171) restricted to the nodes DetermineNodesForUpdate marked.
@@ -23,7 +21,7 @@
 // The children of a node are multiplied in plan order; with two children the product is exact-commutative and
 // power-of-two rescalings are exact, and nodes with more children are planned in tree order (plan_walk,
 // canonical_multi), so conditionals do not depend on the plan: a partial re-evaluation reproduces the full one bit for
-// bit.  Against prune64_kernel results agree to rounding (different summation tree inside a product).
+// bit.
 #pragma once
 #include "hb2_kernels_fp64.cuh"
 #include "hb2_kernels_tc.cuh"      // step encoding (WALK_*, STEP_*), globaltimer_ns, HB2_WAIT_LIMIT_NS
@@ -44,11 +42,11 @@ struct LaneArgs {
     int trace_cta;
 };
 
-// Two CTA shapes, NW warps x 8 patterns: NW = 4 (32 patterns, 128 threads, four CTAs per SM; the default) and NW = 8 (64
-// patterns, 256 threads, three CTAs per SM; HB2_LANES_WARPS=8, measured slower).
+// CTA shape: 4 warps x 8 patterns (32 patterns, 128 threads, four CTAs per SM).
+constexpr int LANES_WARPS = 4, LANES_TILE_P = 8 * LANES_WARPS, LANES_THREADS = 32 * LANES_WARPS, LANES_CTAS_PER_SM = 4;
 constexpr int LANES_LDX = 68;                    // leading dimensions (doubles): both fragment loads are 2 wavefronts, the
 constexpr int LANES_LDP = 72;                    // minimum for 256 bytes per warp
-constexpr int lanes_smem_bytes(int nw) { return (8 * nw * LANES_LDX + 64 * LANES_LDP) * (int)sizeof(double); }
+constexpr int LANES_SMEM_BYTES = (LANES_TILE_P * LANES_LDX + 64 * LANES_LDP) * (int)sizeof(double);
 
 __device__ __forceinline__ void cp_async16(void *smem_dst, const void *gsrc) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
@@ -69,11 +67,9 @@ __device__ __forceinline__ void lanes_mm(const double *__restrict__ Xs, const do
     }
 }
 
-template <int NW>
-__global__ void __launch_bounds__(32 * NW, NW == 4 ? 4 : 3) prune64_lanes_kernel(LaneArgs w) {
-    constexpr int LANES_TILE_P = 8 * NW, LANES_THREADS = 32 * NW;
+__global__ void __launch_bounds__(LANES_THREADS, LANES_CTAS_PER_SM) prune64_lanes_kernel(LaneArgs w) {
     extern __shared__ __align__(16) double sm[];
-    double *Xs = sm;                              // [8 NW][LDX] child conditionals (pattern-major)
+    double *Xs = sm;                              // [LANES_TILE_P][LDX] child conditionals (pattern-major)
     double *Ps = sm + LANES_TILE_P * LANES_LDX;   // [64][LDP] transition matrix (transposed) of the current / next contraction
     const PruneArgs &a = w.a;
     const int tid = threadIdx.x, warp = tid >> 5, g = (tid & 31) >> 2, q4 = tid & 3;
@@ -268,7 +264,7 @@ __global__ void __launch_bounds__(32 * NW, NW == 4 ? 4 : 3) prune64_lanes_kernel
 #pragma unroll
                         for (int j = 0; j < 8; j++) { v[j][0] = v[j][0] * s1 * s2; v[j][1] = v[j][1] * s1 * s2; }
                     }
-                }                                                     // inf / NaN: left alone, like prune64_kernel
+                }                                                     // inf / NaN: left alone
                 ex += e;
                 const bool is_root = !side && node == a.I - 1;
                 double2 *outp = reinterpret_cast<double2 *>((side ? w.cond_side : a.cond) + (((size_t)cat * a.I + node) * Sp + s) * 64 + c0s);

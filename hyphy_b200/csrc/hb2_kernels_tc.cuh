@@ -11,7 +11,7 @@
 //
 // Anchors.  The tensor core accumulates in fp32 without round-to-nearest, which would bias lnL by ~1e-7*|lnL| over a
 // codon tree.  Conditional vectors are sharply peaked (1-3 codons carry almost all the mass), so each thread pulls the
-// entries >= 2^-6 of its row (at most 8, "anchors") out of the tensor operand and multiplies them on the CUDA cores with
+// entries >= 2^-6 of its row ("anchors") out of the tensor operand and multiplies them on the CUDA cores with
 // round-to-nearest fp32 FMAs against fp32 rows of P^T while the MMAs run; the tensor core only contracts the diffuse
 // remainder, whose rounding bias is scaled down by its share.
 //
@@ -21,8 +21,8 @@
 //     matrices; LBO = 2048 B between K chunks, SBO = 128 B between 8-row groups) -- the same [chunk][pattern][4] order
 //     the conditionals have in HBM, so a thread's stores are 16-byte and conflict-free.
 //   B (= P, 64 x 64, K-major) comes from SHARED MEMORY in the same layout (LBO = 1024 B, SBO = 128 B).  The expm stage
-//     writes P already split and tiled that way (pack_tc_kernel), so one 32 KB cp.async.bulk (TMA engine, mbarrier
-//     completion) per child stages Ph and Pl.
+//     writes P already split and tiled that way (the ExpmTcOut epilogues of hb2_kernels_fp64.cuh, mix_reduce_kernel),
+//     so one 32 KB cp.async.bulk (TMA engine, mbarrier completion) per child stages Ph and Pl.
 //   D (128 x 64 fp32) is accumulated in registers (two m64 fragments per warpgroup thread), written to a shared row
 //     buffer and read back one row per thread, multiplied into the running product of the parent held in registers.
 //
@@ -41,7 +41,6 @@ constexpr int TC_PTF_FLOATS = 64 * TC_PTF_ROW; // per (class, branch)
 constexpr int TC_X_BYTES = 2 * 16 * 128 * 16;  // A operand: Xh | Xl, [16 chunks][128 patterns][4] fp32 each
 constexpr int TC_D_ROW = 68;                   // floats per row of the shared accumulator read-back buffer
 constexpr int TC_D_BYTES = 128 * TC_D_ROW * 4;
-constexpr int TC_MAX_ANCHORS = 8;              // per pattern and child (list capacity of the per-level and split-row kernels)
 constexpr int WALK_FAST_ANCHORS = 4;           // anchors handled by the unrolled fast path of the walk kernel; more go to a loop
 constexpr float TC_ANCHOR_THR = 0.015625f;     // 2^-6 (rows are normalised to max in [0.5,1))
 
@@ -171,27 +170,6 @@ __device__ __forceinline__ void store_x_chunk(uint8_t *xs, int q, int pattern, c
     *reinterpret_cast<uint4 *>(xs + TC_X_BYTES / 2 + (size_t)q * 2048 + pattern * 16) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
 }
 
-// ------------------------------------------------------------------------------------------------------------------
-// PT (fp64, transposed) -> tensor-path operands: canonical hi/lo tiles of P and an fp32 copy of PT.  One CTA per slot.
-// ------------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) pack_tc_kernel(const double *__restrict__ PT, const int *__restrict__ slots,
-                                                       float *__restrict__ PB, float *__restrict__ PTf) {
-    if (slots[blockIdx.x] < 0) return;
-    const size_t slot = slots[blockIdx.x];
-    const double *src = PT + slot * 4096;
-    float *pb = PB + slot * TC_PB_FLOATS;
-    float *pf = PTf + slot * TC_PTF_FLOATS;
-    for (int o = threadIdx.x; o < 4096; o += 256) {
-        const int chunk = o >> 8, n = (o >> 2) & 63, kk = chunk * 4 + (o & 3);
-        const double p = src[kk * 64 + n];              // P[n][kk] = PT[kk][n]
-        const float hi = tf32_rn((float)p);
-        const float lo = tf32_rn((float)(p - (double)hi));
-        pb[o] = hi;
-        pb[4096 + o] = lo;
-        pf[(o >> 6) * TC_PTF_ROW + (o & 63)] = (float)src[o];
-    }
-}
-
 // Explicit-form mixtures (BS-REL, reference tree.cpp:3047-3089): PT[slot_i] = sum_k w[i][k] * comp[i*K + k], components
 // added in order k = 0..K-1 (deterministic); 64-state tensor partitions also get the split tiles and the fp32 table.
 // One CTA per node; comp = scratch matrices [n*K][Dp*Dp] in the PT layout (transposed).
@@ -223,13 +201,9 @@ __global__ void __launch_bounds__(256) mix_reduce_kernel(const double *__restric
     }
 }
 
-// ------------------------------------------------------------------------------------------------------------------
-// Fused pruning update on the tensor core.  grid = (Sp/128, jobs, classes), block = 128 threads = one warpgroup
-// (thread t <-> pattern t).
-// ------------------------------------------------------------------------------------------------------------------
 // Power-of-two renormalisation of a pattern's 64 conditionals: max -> [0.5,1).  `force` = false only rescales when the
 // maximum has drifted below 2^-32 (cheap guard between the children of one node); true at the end of a node.
-__device__ __forceinline__ void renorm_f32(float (&v)[64], int &ex, bool force = true) {
+__device__ __forceinline__ void renorm_f32(float (&v)[64], int &ex, bool force) {
     float m0 = v[0], m1 = v[1], m2 = v[2], m3 = v[3];          // four independent chains instead of one of length 64
 #pragma unroll
     for (int k = 4; k < 64; k += 4) { m0 = fmaxf(m0, v[k]); m1 = fmaxf(m1, v[k + 1]); m2 = fmaxf(m2, v[k + 2]); m3 = fmaxf(m3, v[k + 3]); }
@@ -244,165 +218,6 @@ __device__ __forceinline__ void renorm_f32(float (&v)[64], int &ex, bool force =
         }
     }
 }
-
-constexpr int TC_SMEM_BYTES = 32768 + TC_X_BYTES + TC_D_BYTES + TC_MAX_ANCHORS * 128 * 8 + 64;  // B, A, D, anchor lists, barrier
-
-__global__ void __launch_bounds__(128, 1) prune64_tc_kernel(PruneTcArgs a, const int *__restrict__ jobs) {
-    extern __shared__ __align__(1024) uint8_t smem[];
-    float *Bs = reinterpret_cast<float *>(smem);                         // [2][4096] Ph, Pl
-    uint8_t *Xs = smem + 32768;                                          // A operand: Xh | Xl
-    float *Ds = reinterpret_cast<float *>(Xs + TC_X_BYTES);              // [128][TC_D_ROW] accumulator read-back
-    int *s_ak = reinterpret_cast<int *>(Xs + TC_X_BYTES + TC_D_BYTES);   // [TC_MAX_ANCHORS][128] anchor state
-    float *s_av = reinterpret_cast<float *>(s_ak + TC_MAX_ANCHORS * 128); // [TC_MAX_ANCHORS][128] anchor value
-    uint64_t *bar_b = reinterpret_cast<uint64_t *>(s_av + TC_MAX_ANCHORS * 128);
-    const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
-    const int par = jobs[blockIdx.y];
-    const int cat = a.cat0 + blockIdx.z;
-    const size_t Sp = a.Sp;
-    const size_t s = (size_t)blockIdx.x * TC_TILE_P + tid;
-
-    if (tid == 0) {
-        mbar_init(bar_b, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    const uint32_t xs_addr = smem_u32(Xs), bs_addr = smem_u32(Bs);
-
-    float v[64];
-#pragma unroll
-    for (int k = 0; k < 64; k++) v[k] = 1.f;
-    int ex = 0;
-    uint32_t phase = 0;
-    const int c_begin = a.tree.child_start[par], c_end = a.tree.child_start[par + 1];
-    for (int ci = c_begin; ci < c_end; ci++) {
-        const int child = a.tree.child_ids[ci];
-        const size_t slot = (size_t)cat * a.B + child;
-        if (child < a.L) {
-            const int code = (child == a.forced_node) ? a.forced[s] : a.leaf[(size_t)child * Sp + s];
-            const float *PTf = a.PTf + slot * TC_PTF_FLOATS;
-            if (code >= 0) {
-                const float4 *row = reinterpret_cast<const float4 *>(PTf + (size_t)code * TC_PTF_ROW);
-#pragma unroll
-                for (int q = 0; q < 16; q++) {
-                    const float4 r = __ldg(row + q);
-                    v[4 * q] *= r.x; v[4 * q + 1] *= r.y; v[4 * q + 2] *= r.z; v[4 * q + 3] *= r.w;
-                }
-            } else {
-                float acc[64];
-#pragma unroll
-                for (int k = 0; k < 64; k++) acc[k] = 0.f;
-                const double *amb = a.ambig + (size_t)(-code - 1) * 64;
-                for (int j = 0; j < a.D; j++) {
-                    if (__ldg(amb + j) != 0.0) {
-                        const float4 *row = reinterpret_cast<const float4 *>(PTf + (size_t)j * TC_PTF_ROW);
-#pragma unroll
-                        for (int q = 0; q < 16; q++) {
-                            const float4 r = __ldg(row + q);
-                            acc[4 * q] += r.x; acc[4 * q + 1] += r.y; acc[4 * q + 2] += r.z; acc[4 * q + 3] += r.w;
-                        }
-                    }
-                }
-#pragma unroll
-                for (int k = 0; k < 64; k++) v[k] *= acc[k];
-            }
-        } else {
-            const int cin = child - a.L;
-            // (A) stage Ph|Pl of this branch: one 32 KB bulk copy (TMA engine), completion on bar_b
-            if (tid == 0) {
-                mbar_expect_tx(bar_b, 32768u);
-                bulk_g2s(Bs, a.PB + slot * TC_PB_FLOATS, 32768u, bar_b);
-            }
-            // (B) this thread's pattern row -> anchors out -> split -> A operand in shared memory
-            int na = 0;
-            {
-                const float4 *xr = reinterpret_cast<const float4 *>(a.cond) + ((((size_t)cat * a.I + cin) * (Sp / 128) + blockIdx.x) * 16) * 128 + tid;
-#pragma unroll
-                for (int q = 0; q < 16; q++) {
-                    const float4 x = xr[(size_t)q * 128];
-                    float xs[4] = {x.x, x.y, x.z, x.w};
-                    uint32_t hi[4], lo[4];
-#pragma unroll
-                    for (int u = 0; u < 4; u++) {
-                        if (xs[u] >= TC_ANCHOR_THR && na < TC_MAX_ANCHORS) {
-                            s_ak[na * 128 + tid] = 4 * q + u;
-                            s_av[na * 128 + tid] = xs[u];
-                            na++;
-                            xs[u] = 0.f;
-                        }
-                        const float h = tf32_rn(xs[u]);
-                        hi[u] = __float_as_uint(h);
-                        lo[u] = __float_as_uint(xs[u] - h);
-                    }
-                    store_x_chunk(Xs, q, tid, hi, lo);
-                }
-            }
-            ex += a.scal[((size_t)cat * a.I + cin) * Sp + s];
-            fence_proxy_async();
-            __syncthreads();                 // A operand complete; every thread is done reading the previous D
-            mbar_wait(bar_b, phase, a.err);
-            float d0[32], d1[32];
-            wg_fence();
-            wg_issue_tf32x3(d0, xs_addr, bs_addr, 0);
-            wg_issue_tf32x3(d1, xs_addr, bs_addr, 1);
-            wg_commit();
-            wg_wait_all();
-            wg_pin(d0);
-            wg_pin(d1);
-            wg_store_d(Ds, d0, 0, warp, lane);
-            wg_store_d(Ds, d1, 64, warp, lane);
-            // anchors on the CUDA cores while the other warps store their fragments: acc[n] = sum_a x[k_a] * P[n][k_a], fp32 RN
-            float acc[64];
-#pragma unroll
-            for (int k = 0; k < 64; k++) acc[k] = 0.f;
-            {
-                const float *PTf = a.PTf + slot * TC_PTF_FLOATS;
-                for (int ai = 0; ai < na; ai++) {
-                    const int ka = s_ak[ai * 128 + tid];
-                    const float xv = s_av[ai * 128 + tid];
-                    const float4 *row = reinterpret_cast<const float4 *>(PTf + (size_t)ka * TC_PTF_ROW);
-#pragma unroll
-                    for (int q = 0; q < 16; q++) {
-                        const float4 r = __ldg(row + q);
-                        acc[4 * q] = fmaf(xv, r.x, acc[4 * q]); acc[4 * q + 1] = fmaf(xv, r.y, acc[4 * q + 1]);
-                        acc[4 * q + 2] = fmaf(xv, r.z, acc[4 * q + 2]); acc[4 * q + 3] = fmaf(xv, r.w, acc[4 * q + 3]);
-                    }
-                }
-            }
-            __syncthreads();                 // every row of D is in the read-back buffer
-            {
-                const float4 *drow = reinterpret_cast<const float4 *>(Ds + (size_t)tid * TC_D_ROW);
-#pragma unroll
-                for (int q = 0; q < 16; q++) {
-                    const float4 dd = drow[q];
-                    v[4 * q] *= (dd.x + acc[4 * q]); v[4 * q + 1] *= (dd.y + acc[4 * q + 1]);
-                    v[4 * q + 2] *= (dd.z + acc[4 * q + 2]); v[4 * q + 3] *= (dd.w + acc[4 * q + 3]);
-                }
-            }
-            phase ^= 1u;
-        }
-        if (ci == c_end - 1 && a.L + par == a.forced_node) {     // pinned internal node: only the forced state survives
-            const int f = a.forced[s];
-#pragma unroll
-            for (int k = 0; k < 64; k++) if (k != f) v[k] = 0.f;
-        }
-        renorm_f32(v, ex);
-    }
-    // write the parent's conditionals (already renormalised after the last child) and the root reduction
-    {
-        float4 *outp = reinterpret_cast<float4 *>(a.cond) + ((((size_t)cat * a.I + par) * (Sp / 128) + blockIdx.x) * 16) * 128 + tid;
-#pragma unroll
-        for (int q = 0; q < 16; q++) outp[(size_t)q * 128] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-        a.scal[((size_t)cat * a.I + par) * Sp + s] = ex;
-        if (par == a.I - 1) {
-            double r = 0.0;
-#pragma unroll
-            for (int k = 0; k < 64; k++) r = fma((double)v[k], a.pi[k], r);
-            a.rootL[(size_t)cat * Sp + s] = r;
-            a.rootE[(size_t)cat * Sp + s] = ex;
-        }
-    }
-}
-
 
 // ------------------------------------------------------------------------------------------------------------------
 // Persistent "walk" kernel: the whole pruning pass of one evaluation in ONE launch.
@@ -744,7 +559,7 @@ __global__ void __launch_bounds__(128, 1) prune64_tc_walk_kernel(WalkArgs w) {
                         }
                     }
                 }
-                while (amask) {                  // more than TC_MAX_ANCHORS entries above the threshold (diffuse vectors): rare
+                while (amask) {                  // more than WALK_FAST_ANCHORS entries above the threshold (diffuse vectors): rare
                     const int kk = __ffsll((long long)amask) - 1;
                     amask &= amask - 1;
                     const float xv = fabsf(__ldcg(xrow_f + ((size_t)(kk >> 2) * 128) * 4 + (kk & 3)));
@@ -796,384 +611,6 @@ __global__ void __launch_bounds__(128, 1) prune64_tc_walk_kernel(WalkArgs w) {
                     for (int k = 0; k < 64; k++) rr = fma((double)v[k], a.pi[k], rr);
                     a.rootL[(size_t)cat * Sp + s] = rr;
                     a.rootE[(size_t)cat * Sp + s] = ex;
-                }
-            }
-            if (tr) trp[7] = clock64();
-            st = nx;
-            nx = nx2;
-        }
-    }
-    if (w.trace_cta_times && tid == 0) w.trace_cta_times[(size_t)blockIdx.x * 4 + 2] = clock64();
-}
-
-
-// ------------------------------------------------------------------------------------------------------------------
-// prune64_tc_walk2_kernel: the same pass with TWO threads per pattern (256-thread CTA).
-//
-// The 128-thread kernel above carries all 64 states of a pattern per thread through the split, the anchor products and
-// the read-back.  Here warp w (0..7) belongs to warpgroup h = w / 4, which owns state half h: thread (pattern t, half h)
-// owns states 32h..32h+31 of pattern t everywhere (conditional chunks 8h..8h+7, accumulator read-back columns 32h..), so
-// the serial stream per step halves while the tile, the staging ring and the plan stay exactly the same.  For the MMAs
-// warpgroup h contracts the 64-pattern half h of the tile (patterns 64h..64h+63, all 64 parent states).
-//   * anchors: each thread publishes the anchor mask of ITS half in shared memory before barrier (2); afterwards both threads
-//     of a pattern enumerate the combined 64-bit mask (values re-read from the child's block in L2, as in the first kernel)
-//     and accumulate their own 32 parent states;
-//   * exponents: inside a job the two halves rescale independently (own guard, own exponent); when the job is complete
-//     (STEP_LAST) the halves exchange (maximum, exponent) through shared memory and bring the node to ONE power-of-two scale
-//     with max in [0.5,1), which is what is stored (tagged) and handed over in registers on a chain;
-//   * the root dot product is combined the same way.
-// Everything observable (layouts, tags, plan, results' meaning) is identical to prune64_tc_walk_kernel; the summation order
-// inside a row differs, so results agree to rounding, not bitwise (both are deterministic).
-// ------------------------------------------------------------------------------------------------------------------
-constexpr int WALK2_XBYTES = 2 * 128 * 4 /* anchor masks */ + 2 * 128 * 4 /* half maxima */ + 2 * 128 * 4 /* half exponents */ +
-                             2 * 128 * 8 /* root partials */;
-constexpr int WALK2_SMEM_BYTES = 2 * WALK_STAGE_FLOATS * 4 + TC_X_BYTES + TC_D_BYTES + WALK2_XBYTES + 64;
-
-__device__ __forceinline__ void renorm_half(float (&v)[32], int &ex) {     // guard inside a job: own half only, rarely taken
-    float m0 = v[0], m1 = v[1], m2 = v[2], m3 = v[3];
-#pragma unroll
-    for (int k = 4; k < 32; k += 4) { m0 = fmaxf(m0, v[k]); m1 = fmaxf(m1, v[k + 1]); m2 = fmaxf(m2, v[k + 2]); m3 = fmaxf(m3, v[k + 3]); }
-    const float m = fmaxf(fmaxf(m0, m1), fmaxf(m2, m3));
-    if (m > 0.f && m < 2.3283064e-10f) {
-        const int e = max((int)((__float_as_uint(m) >> 23) & 0xffu) - 126, -125);
-        const float sc = __uint_as_float((uint32_t)(127 - e) << 23);
-#pragma unroll
-        for (int k = 0; k < 32; k++) v[k] *= sc;
-        ex += e;
-    }
-}
-
-__global__ void __launch_bounds__(256, 1) prune64_tc_walk2_kernel(WalkArgs w) {
-    extern __shared__ __align__(1024) uint8_t smem[];
-    const PruneTcArgs &a = w.a;
-    float *stage_base = reinterpret_cast<float *>(smem);                           // 2 x [P^T table | Ph | Pl]
-    uint8_t *Xs = smem + 2 * WALK_STAGE_FLOATS * 4;                                 // A operand: Xh | Xl
-    float *Ds = reinterpret_cast<float *>(Xs + TC_X_BYTES);                         // [128][TC_D_ROW] accumulator read-back
-    uint32_t *s_am = reinterpret_cast<uint32_t *>(Xs + TC_X_BYTES + TC_D_BYTES);   // [2][128] anchor masks of the two halves
-    float *s_mx = reinterpret_cast<float *>(s_am + 2 * 128);                        // [2][128]
-    int *s_ex = reinterpret_cast<int *>(s_mx + 2 * 128);                            // [2][128]
-    double *s_rt = reinterpret_cast<double *>(s_ex + 2 * 128);                      // [2][128]
-    uint64_t *bar_full = reinterpret_cast<uint64_t *>(s_rt + 2 * 128);              // [2]
-    const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
-    const int lq = warp & 3, h = warp >> 2, t = 32 * lq + lane;                     // warp in warpgroup, state half, pattern in tile
-    const size_t Sp = a.Sp;
-    float4 *cond4 = reinterpret_cast<float4 *>(a.cond);
-
-    if (tid == 0) {
-        mbar_init(bar_full, 1);
-        mbar_init(bar_full + 1, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    const uint32_t xs_addr = smem_u32(Xs);
-    uint32_t n_step = 0;
-    bool bailed = false;
-
-    const int r = blockIdx.x % w.K;
-    const int i_begin = w.lane_start[r], i_end = w.lane_start[r + 1];
-    if (w.trace_cta_times && tid == 0) {
-        uint32_t smid; unsigned long long gt;
-        asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
-        long long *q = w.trace_cta_times + (size_t)blockIdx.x * 4;
-        q[0] = smid; q[1] = clock64(); q[3] = (long long)gt;
-    }
-
-    auto stage_step = [&](int cat, int tile, int2 st, uint32_t m) {
-        const int child = st.x & WALK_ID_MASK;
-        const bool internal = child >= a.L;
-        float *dst = stage_base + (m & 1u) * WALK_STAGE_FLOATS;
-        uint64_t *bar = bar_full + (m & 1u);
-        if (st.x & WALK_MUL) {
-            mbar_expect_tx(bar, 0u);
-            prefetch_l2_bulk(cond4 + cond_f4(cat, child - a.L, tile, 0, 0, w.NI, w.T), 32768u);
-            return;
-        }
-        const size_t slot = (size_t)cat * a.B + child;
-        mbar_expect_tx(bar, (uint32_t)(TC_PTF_FLOATS * 4) + (internal ? 32768u : 0u));
-        bulk_g2s(dst, a.PTf + slot * TC_PTF_FLOATS, (uint32_t)(TC_PTF_FLOATS * 4), bar);
-        if (internal) {
-            bulk_g2s(dst + 64 * WALK_PT_ROW, a.PB + slot * TC_PB_FLOATS, 32768u, bar);
-            if (!(st.x & WALK_CHAIN)) prefetch_l2_bulk(cond4 + cond_f4(cat, child - a.L, tile, 0, 0, w.NI, w.T), 32768u);
-        }
-    };
-
-    // this thread's 9 words of another node's tile: its 8 chunks (32 states) + the exponent word; `await` as in the first kernel
-    auto load_half_row = [&](const float4 *xrow, const int *scp, bool await, uint32_t want, uint4 (&x4)[8], uint32_t &sc) {
-#pragma unroll
-        for (int q = 0; q < 8; q++) x4[q] = __ldcg(reinterpret_cast<const uint4 *>(xrow + (size_t)q * 128));
-        sc = (uint32_t)__ldcg(scp);
-        if (await) {
-            unsigned long long t0 = 0;
-            for (int it = 0; !bailed; it++) {
-                uint32_t bad = (sc << 31) ^ want;
-#pragma unroll
-                for (int q = 0; q < 8; q++) bad |= (x4[q].x ^ want) | (x4[q].y ^ want) | (x4[q].z ^ want) | (x4[q].w ^ want);
-                if (!(bad >> 31)) break;
-                if ((it & 255) == 255) {
-                    const unsigned long long now = globaltimer_ns();
-                    if (t0 == 0) t0 = now;
-                    else if (now - t0 > HB2_WAIT_LIMIT_NS) { atomicExch(a.err, 2); bailed = true; }
-                }
-#pragma unroll
-                for (int q = 0; q < 8; q++) x4[q] = ld_relaxed_u4(xrow + (size_t)q * 128);
-                sc = ld_relaxed_u32(scp);
-            }
-        }
-    };
-
-    for (int ct = blockIdx.x / w.K; ct < w.ncls * w.T; ct += w.nslots) {
-        const int cat = a.cat0 + ct / w.T;
-        const int tile = ct % w.T;
-        const size_t s = (size_t)tile * TC_TILE_P + t;
-        float v[32];
-        int ex = 0;
-        if (i_begin == i_end) continue;
-        int2 st = __ldg(w.steps + i_begin);
-        int2 nx = (i_begin + 1 < i_end) ? __ldg(w.steps + i_begin + 1) : make_int2(0, 0);
-        __syncthreads();
-        if (warp == 7 && elect_one()) stage_step(cat, tile, st, n_step);
-        auto step_aux = [&](int2 q) -> int {
-            const int ch = q.x & WALK_ID_MASK;
-            if (ch < a.L) return (ch == a.forced_node) ? __ldg(a.forced + s) : __ldg(a.leaf + (size_t)ch * Sp + s);
-            return (q.x & WALK_WAIT) ? __ldg(w.gen + (size_t)cat * w.NI + (ch - a.L)) : 0;
-        };
-        int next_code = step_aux(st);
-        for (int i = i_begin; i < i_end; i++) {
-            const int enc = st.x;
-            const int child = enc & WALK_ID_MASK;
-            const int par = st.y & WALK_ID_MASK;
-            const int flags = st.y;
-            const int code = next_code;
-            const uint32_t tagbit = (flags & STEP_LAST) ? ((uint32_t)__ldg(w.gen + (size_t)cat * w.NI + par) << 31) : 0u;
-            const bool has_next = (i + 1 < i_end);
-            const int2 nx2 = (i + 2 < i_end) ? __ldg(w.steps + i + 2) : make_int2(0, 0);
-            const bool tr = w.trace && tid == 0 && (int)blockIdx.x == w.trace_cta;
-            long long *trp = tr ? w.trace + (size_t)(i - i_begin) * 12 : nullptr;
-            if (tr) { trp[0] = ((long long)st.x << 32) | (unsigned)st.y; trp[1] = clock64(); }
-            __syncthreads();                  // (1) everyone is done with step i-1: ring slot (n_step+1)&1 and the exchange arrays are free
-            if (has_next) {
-                if (warp == 7 && elect_one()) stage_step(cat, tile, nx, n_step + 1);
-                next_code = step_aux(nx);
-            }
-            if ((flags & STEP_FIRST) && !(enc & WALK_CHAIN)) {
-#pragma unroll
-                for (int k = 0; k < 32; k++) v[k] = 1.f;
-                ex = 0;
-            }
-            const float *tab = stage_base + (n_step & 1u) * WALK_STAGE_FLOATS;
-            if (tr) trp[2] = clock64();
-            if (child < a.L) {
-                mbar_wait(bar_full + (n_step & 1u), (n_step >> 1) & 1u, a.err);
-                if (tr) trp[3] = clock64();
-                if (code >= 0) {
-                    const float4 *row = reinterpret_cast<const float4 *>(tab + code * WALK_PT_ROW + 32 * h);
-#pragma unroll
-                    for (int q = 0; q < 8; q++) {
-                        const float4 rr = row[q];
-                        v[4 * q] *= rr.x; v[4 * q + 1] *= rr.y; v[4 * q + 2] *= rr.z; v[4 * q + 3] *= rr.w;
-                    }
-                } else {
-                    float acc[32];
-#pragma unroll
-                    for (int k = 0; k < 32; k++) acc[k] = 0.f;
-                    const double *amb = a.ambig + (size_t)(-code - 1) * 64;
-                    for (int jj = 0; jj < a.D; jj++) {
-                        if (__ldg(amb + jj) != 0.0) {
-                            const float4 *row = reinterpret_cast<const float4 *>(tab + jj * WALK_PT_ROW + 32 * h);
-#pragma unroll
-                            for (int q = 0; q < 8; q++) {
-                                const float4 rr = row[q];
-                                acc[4 * q] += rr.x; acc[4 * q + 1] += rr.y; acc[4 * q + 2] += rr.z; acc[4 * q + 3] += rr.w;
-                            }
-                        }
-                    }
-#pragma unroll
-                    for (int k = 0; k < 32; k++) v[k] *= acc[k];
-                }
-            } else if (enc & WALK_MUL) {
-                const int cin = child - a.L;
-                const bool await = (enc & WALK_WAIT) != 0;
-                uint4 x4[8];
-                uint32_t sc;
-                load_half_row(cond4 + cond_f4(cat, cin, tile, 8 * h, t, w.NI, w.T), a.scal + ((size_t)cat * w.NI + cin) * Sp + s, await,
-                              await ? ((uint32_t)code << 31) : 0u, x4, sc);
-#pragma unroll
-                for (int q = 0; q < 8; q++) {
-                    v[4 * q] *= __uint_as_float(x4[q].x & 0x7fffffffu); v[4 * q + 1] *= __uint_as_float(x4[q].y & 0x7fffffffu);
-                    v[4 * q + 2] *= __uint_as_float(x4[q].z & 0x7fffffffu); v[4 * q + 3] *= __uint_as_float(x4[q].w & 0x7fffffffu);
-                }
-                ex += (int)sc >> 1;
-                if (tr) trp[3] = clock64();
-            } else {
-                const int cin = child - a.L;
-                const float4 *xrow = cond4 + cond_f4(cat, cin, tile, 0, t, w.NI, w.T);      // chunk 0 of the pattern's row (all 64 states)
-                uint32_t am = 0;                                                         // anchors of this half (bit k <-> state 32h + k)
-                float xa[32];                                                            // this half's values (anchor values are taken from here)
-                if (enc & WALK_CHAIN) {
-#pragma unroll
-                    for (int k = 0; k < 32; k++) { xa[k] = v[k]; v[k] = 1.f; }
-                } else {
-                    const bool await = (enc & WALK_WAIT) != 0;
-                    const uint32_t want = await ? ((uint32_t)code << 31) : 0u;
-                    uint4 x4[8];
-                    uint32_t sc;
-                    load_half_row(xrow + (size_t)8 * h * 128, a.scal + ((size_t)cat * w.NI + cin) * Sp + s, await, want, x4, sc);
-#pragma unroll
-                    for (int q = 0; q < 8; q++) {
-                        xa[4 * q] = __uint_as_float(x4[q].x & 0x7fffffffu); xa[4 * q + 1] = __uint_as_float(x4[q].y & 0x7fffffffu);
-                        xa[4 * q + 2] = __uint_as_float(x4[q].z & 0x7fffffffu); xa[4 * q + 3] = __uint_as_float(x4[q].w & 0x7fffffffu);
-                    }
-                    ex += (int)sc >> 1;
-                }
-                // split in 4-state chunks (registers): anchors out, tf32 hi / lo -> A operand chunks 8h..8h+7 of pattern t
-#pragma unroll
-                for (int q = 0; q < 8; q++) {
-                    uint32_t hi[4], lo[4];
-#pragma unroll
-                    for (int u = 0; u < 4; u++) {
-                        const float xv = xa[4 * q + u];
-                        const bool big = xv >= w.anchor_thr;
-                        if (big) am |= 1u << (4 * q + u);
-                        const float x = big ? 0.f : xv;
-                        const float hh = tf32_rn(x);
-                        hi[u] = __float_as_uint(hh);
-                        lo[u] = __float_as_uint(x - hh);
-                    }
-                    store_x_chunk(Xs, 8 * h + q, t, hi, lo);
-                }
-                if (tr) trp[8] = clock64();
-                s_am[h * 128 + t] = am;                                              // for both threads of the pattern
-                if (tr) trp[9] = clock64();
-                fence_proxy_async();
-                if (tr) { trp[10] = clock64(); trp[3] = trp[10]; }
-                __syncthreads();             // (2) A operand complete in shared memory, anchor lists published; previous D consumed
-                if (tr) trp[4] = clock64();
-                // warpgroup h: the 24 wgmma of pattern half h, issued once the branch's operands have landed
-                mbar_wait(bar_full + (n_step & 1u), (n_step >> 1) & 1u, a.err);
-                if (tr) trp[5] = clock64();
-                float d[32];
-                wg_fence();
-                wg_issue_tf32x3(d, xs_addr, smem_u32(tab + 64 * WALK_PT_ROW), h);
-                wg_commit();
-                // anchors of BOTH halves on the CUDA cores while the tensor core works: this thread's 32 parent states.  Values
-                // are re-read from the child's block in L2 (loaded, or stored by the two threads of this pattern a moment ago --
-                // barrier (2) made those stores visible), a handful of loads in flight under the MMAs.
-                unsigned long long amask = (unsigned long long)s_am[t] | ((unsigned long long)s_am[128 + t] << 32);
-                const float *xrow_f = reinterpret_cast<const float *>(xrow);
-                int ak[WALK_FAST_ANCHORS];
-                float av[WALK_FAST_ANCHORS];
-#pragma unroll
-                for (int ai = 0; ai < WALK_FAST_ANCHORS; ai++) {
-                    ak[ai] = -1; av[ai] = 0.f;
-                    if (amask) {
-                        const int kk = __ffsll((long long)amask) - 1;
-                        amask &= amask - 1;
-                        ak[ai] = kk;
-                        av[ai] = __ldcg(xrow_f + ((size_t)(kk >> 2) * 128) * 4 + (kk & 3));
-                    }
-                }
-                float acc[32];
-                const float *tabh = tab + 32 * h;
-                {
-                    const float xv = ak[0] >= 0 ? fabsf(av[0]) : 0.f;
-                    const float4 *row = reinterpret_cast<const float4 *>(tabh + max(ak[0], 0) * WALK_PT_ROW);
-#pragma unroll
-                    for (int q = 0; q < 8; q++) {
-                        const float4 rr = row[q];
-                        acc[4 * q] = xv * rr.x; acc[4 * q + 1] = xv * rr.y; acc[4 * q + 2] = xv * rr.z; acc[4 * q + 3] = xv * rr.w;
-                    }
-                }
-#pragma unroll
-                for (int ai = 1; ai < WALK_FAST_ANCHORS; ai++) {
-                    if (ak[ai] >= 0) {
-                        const float xv = fabsf(av[ai]);
-                        const float4 *row = reinterpret_cast<const float4 *>(tabh + ak[ai] * WALK_PT_ROW);
-#pragma unroll
-                        for (int q = 0; q < 8; q++) {
-                            const float4 rr = row[q];
-                            acc[4 * q] = fmaf(xv, rr.x, acc[4 * q]); acc[4 * q + 1] = fmaf(xv, rr.y, acc[4 * q + 1]);
-                            acc[4 * q + 2] = fmaf(xv, rr.z, acc[4 * q + 2]); acc[4 * q + 3] = fmaf(xv, rr.w, acc[4 * q + 3]);
-                        }
-                    }
-                }
-                while (amask) {                  // more than four entries above the threshold (diffuse vectors): rare
-                    const int kk = __ffsll((long long)amask) - 1;
-                    amask &= amask - 1;
-                    const float xv = fabsf(__ldcg(xrow_f + ((size_t)(kk >> 2) * 128) * 4 + (kk & 3)));
-                    const float4 *row = reinterpret_cast<const float4 *>(tabh + kk * WALK_PT_ROW);
-#pragma unroll
-                    for (int q = 0; q < 8; q++) {
-                        const float4 rr = row[q];
-                        acc[4 * q] = fmaf(xv, rr.x, acc[4 * q]); acc[4 * q + 1] = fmaf(xv, rr.y, acc[4 * q + 1]);
-                        acc[4 * q + 2] = fmaf(xv, rr.z, acc[4 * q + 2]); acc[4 * q + 3] = fmaf(xv, rr.w, acc[4 * q + 3]);
-                    }
-                }
-                wg_wait_all();
-                wg_pin(d);
-                if (tr) trp[6] = clock64();
-                wg_store_d(Ds, d, 64 * h, lq, lane);
-                __syncthreads();             // (3) every row of D is in the read-back buffer
-                {
-                    const float4 *drow = reinterpret_cast<const float4 *>(Ds + (size_t)t * TC_D_ROW + 32 * h);
-#pragma unroll
-                    for (int q = 0; q < 8; q++) {
-                        const float4 dd = drow[q];
-                        v[4 * q] *= (dd.x + acc[4 * q]); v[4 * q + 1] *= (dd.y + acc[4 * q + 1]);
-                        v[4 * q + 2] *= (dd.z + acc[4 * q + 2]); v[4 * q + 3] *= (dd.w + acc[4 * q + 3]);
-                    }
-                }
-            }
-            n_step++;
-            if (!(flags & STEP_LAST)) {
-                renorm_half(v, ex);
-            } else {
-                if (a.L + par == a.forced_node) {                                      // pinned internal node
-                    const int f = __ldg(a.forced + s) - 32 * h;
-#pragma unroll
-                    for (int k = 0; k < 32; k++) if (k != f) v[k] = 0.f;
-                }
-                // the job is complete: ONE power-of-two scale for the whole row.  Exchange (half maximum, half exponent).
-                float m0 = v[0], m1 = v[1], m2 = v[2], m3 = v[3];
-#pragma unroll
-                for (int k = 4; k < 32; k += 4) { m0 = fmaxf(m0, v[k]); m1 = fmaxf(m1, v[k + 1]); m2 = fmaxf(m2, v[k + 2]); m3 = fmaxf(m3, v[k + 3]); }
-                const float mh = fmaxf(fmaxf(m0, m1), fmaxf(m2, m3));
-                s_mx[h * 128 + t] = mh;
-                s_ex[h * 128 + t] = ex;
-                __syncthreads();             // (3) once per job
-                const float mp = s_mx[(h ^ 1) * 128 + t];
-                const int exp_p = s_ex[(h ^ 1) * 128 + t];
-                // true exponent of each half's maximum (m = f * 2^e, f in [0.5,1)); a half that is all zero does not count
-                const bool okh = mh > 0.f && mh < INFINITY, okp = mp > 0.f && mp < INFINITY;
-                const int Eh = ex + max((int)((__float_as_uint(mh) >> 23) & 0xffu) - 126, -125);
-                const int Ep = exp_p + max((int)((__float_as_uint(mp) >> 23) & 0xffu) - 126, -125);
-                const int Et = (okh && okp) ? max(Eh, Ep) : okh ? Eh : okp ? Ep : ex;
-                if (okh || okp) {
-                    const int d = max(-127, min(ex - Et, 127));                         // this half's values are multiplied by 2^d
-                    if (d != 0) {
-                        const float sc = d < -126 ? 0.f : __uint_as_float((uint32_t)(127 + d) << 23);
-#pragma unroll
-                        for (int k = 0; k < 32; k++) v[k] *= sc;
-                    }
-                    ex = Et;
-                }
-                float4 *outp = cond4 + cond_f4(cat, par, tile, 8 * h, t, w.NI, w.T);
-#pragma unroll
-                for (int q = 0; q < 8; q++)
-                    __stcg(reinterpret_cast<uint4 *>(outp + (size_t)q * 128),
-                           make_uint4(__float_as_uint(v[4 * q]) | tagbit, __float_as_uint(v[4 * q + 1]) | tagbit,
-                                      __float_as_uint(v[4 * q + 2]) | tagbit, __float_as_uint(v[4 * q + 3]) | tagbit));
-                if (h == 0) __stcg(a.scal + ((size_t)cat * w.NI + par) * Sp + s, (int)(((uint32_t)ex << 1) | (tagbit >> 31)));
-                if (par == a.I - 1) {
-                    double rr = 0.0;
-#pragma unroll
-                    for (int k = 0; k < 32; k++) rr = fma((double)v[k], a.pi[32 * h + k], rr);
-                    s_rt[h * 128 + t] = rr;
-                    __syncthreads();
-                    if (h == 0) {
-                        a.rootL[(size_t)cat * Sp + s] = s_rt[t] + s_rt[128 + t];
-                        a.rootE[(size_t)cat * Sp + s] = ex;
-                    }
                 }
             }
             if (tr) trp[7] = clock64();

@@ -467,8 +467,7 @@ def test_protein_sized_states_ambiguity_partial_forced_readback(D, taxa, sites, 
     ls[hit] = -(rng.integers(0, 7, size=hit.sum()) + 1)
     w.leaf_states = ls
     lf = LF(w, "fp64")
-    if os.environ.get("HB2_SMALL_DMMA", "1") != "0":
-        assert lf.part.pruning_kernel == "prune_small_dmma_kernel"
+    assert lf.part.pruning_kernel == "prune_small_dmma_kernel"
     lf.set_all_matrices()
     got = lf.compute()
     ref, _ = port.lnl(w, sparse_storage=False)
