@@ -53,6 +53,46 @@ __device__ __forceinline__ double exp2i(int e) {   // exact 2^e for |e| < 1022
     return __longlong_as_double((long long)(e + 1023) << 52);
 }
 
+// Rescaling inside a node.  The pruning kernels multiply all children of a node together and renormalise once, at the end
+// of the node.  For a node with many children (a polytomy, a star tree) the running product can fall below the smallest
+// normal double before that: 400 codon leaves on branches of mean length 2 reach about 2^-1300.  So from the third child on,
+// a running product whose maximum has fallen below RESCALE_BELOW is brought back to [0.5, 1) by an exact power of two and
+// the exponent is carried, as the reference rescales after every child (tree.cpp:161-205).  The rescaling is exact, so a
+// product that does not underflow gives the same bits with or without it; binary nodes never take it.
+constexpr double RESCALE_BELOW = 0x1p-256;
+
+template <int N>
+__device__ __forceinline__ void rescale_running(double (&v)[N], int &ex) {      // one thread holds the pattern's N values
+    double m = 0.0;
+#pragma unroll
+    for (int k = 0; k < N; k++) m = fmax(m, v[k]);
+    if (m > 0.0 && m < RESCALE_BELOW) {
+        const int e = ilogb(m) + 1;
+        const double s1 = exp2i(-(e / 2)), s2 = exp2i(-(e - e / 2));
+#pragma unroll
+        for (int k = 0; k < N; k++) v[k] = v[k] * s1 * s2;
+        ex += e;
+    }
+}
+
+// The same for a pattern whose values are spread over the 4 lanes q4 = 0..3 of a quad (FP64 tensor-pipe kernels).  Called
+// by the whole warp.
+template <int NT>
+__device__ __forceinline__ void rescale_running_quad(double (&v)[NT][2], int &ex) {
+    double m = 0.0;
+#pragma unroll
+    for (int t = 0; t < NT; t++) m = fmax(m, fmax(v[t][0], v[t][1]));
+    m = fmax(m, __shfl_xor_sync(0xffffffffu, m, 1));
+    m = fmax(m, __shfl_xor_sync(0xffffffffu, m, 2));
+    if (m > 0.0 && m < RESCALE_BELOW) {
+        const int e = ilogb(m) + 1;
+        const double s1 = exp2i(-(e / 2)), s2 = exp2i(-(e - e / 2));
+#pragma unroll
+        for (int t = 0; t < NT; t++) { v[t][0] = v[t][0] * s1 * s2; v[t][1] = v[t][1] * s1 * s2; }
+        ex += e;
+    }
+}
+
 // ------------------------------------------------------------------------------------------------
 // Matrix exponential.  One CTA per matrix (expm64_dmma_kernel, expm_small_kernel), or the shared-powers path below.
 //   in : Q [n][D*D] row-major rate matrices (Q*t, diagonal = -rowsum), dst[n] = slot index into PT
@@ -854,6 +894,14 @@ __global__ void __launch_bounds__(128) prune_small_walk_kernel(PruneArgs a, cons
 #pragma unroll
                 for (int k = 0; k < DP; k++) v[k] *= acc[k];
             }
+            if (ci - c_begin >= 1 && ci + 1 < c_end) {       // wide node: before its third and later children
+                if (a.L + par == a.forced_node) {           // pinned: rescale by the forced state, the only one that survives
+                    const int f = __ldg(a.forced + s);
+#pragma unroll
+                    for (int k = 0; k < DP; k++) if (k != f) v[k] = 0.0;
+                }
+                rescale_running(v, ex);
+            }
         }
         if (a.L + par == a.forced_node) {
             const int f = __ldg(a.forced + s);
@@ -989,6 +1037,17 @@ __global__ void __launch_bounds__(128, 6) prune_small_walk_ilp_kernel(PruneArgs 
                 for (int u = 0; u < PP; u++)
 #pragma unroll
                     for (int k = 0; k < DP; k++) v[u][k] *= acc[u][k];
+            }
+            if (ci - c_begin >= 1 && ci + 1 < c_end) {       // wide node: before its third and later children
+#pragma unroll
+                for (int u = 0; u < PP; u++) {
+                    if (a.L + par == a.forced_node) {       // pinned: rescale by the forced state, the only one that survives
+                        const int f = __ldg(a.forced + s[u]);
+#pragma unroll
+                        for (int k = 0; k < DP; k++) if (k != f) v[u][k] = 0.0;
+                    }
+                    rescale_running(v[u], ex[u]);
+                }
             }
         }
         const bool pinned = a.L + par == a.forced_node;
@@ -1408,8 +1467,24 @@ __global__ void __launch_bounds__(64) prune_batch_kernel(BatchPruneArgs a) {
     for (int par = 0; par < a.I; par++) {
         double v = k < a.D ? 1.0 : 0.0;
         int ex = 0;
+        // max over the 64 threads; if it lies below `below`, an exact power of two brings it to [0.5, 1)
+        auto renorm = [&](double below) {
+            double mx = v;
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+            __syncthreads();
+            if ((k & 31) == 0) red[k >> 5] = mx;
+            __syncthreads();
+            mx = fmax(red[0], red[1]);
+            if (mx > 0.0 && mx < below) {
+                const int e = ilogb(mx) + 1;
+                v = v * exp2i(-(e / 2)) * exp2i(-(e - e / 2));
+                ex += e;
+            }
+        };
         const int c_begin = a.tree.child_start[par], c_end = a.tree.child_start[par + 1];
         for (int ci = c_begin; ci < c_end; ci++) {
+            if (ci - c_begin >= 2) renorm(RESCALE_BELOW);       // wide node: keep the running product normal
             const int child = a.tree.child_ids[ci];
             const double *PT = PTs + (size_t)child * 4096;
             double m = 0.0;
@@ -1430,19 +1505,7 @@ __global__ void __launch_bounds__(64) prune_batch_kernel(BatchPruneArgs a) {
             }
             v *= m;
         }
-        // renormalise: max over the 64 threads -> [0.5, 1)
-        double mx = v;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-        __syncthreads();
-        if ((k & 31) == 0) red[k >> 5] = mx;
-        __syncthreads();
-        mx = fmax(red[0], red[1]);
-        if (mx > 0.0 && mx < INFINITY) {
-            const int e = ilogb(mx) + 1;
-            v = v * exp2i(-(e / 2)) * exp2i(-(e - e / 2));
-            ex += e;
-        }
+        renorm(INFINITY);                        // end of the node: max -> [0.5, 1)
         cs[(size_t)par * 64 + k] = v;
         if (k == 0) node_ex[par] = ex;
         __syncthreads();                         // node_ex / cond of this node visible to the block before a parent reads them

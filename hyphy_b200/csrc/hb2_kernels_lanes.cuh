@@ -118,6 +118,7 @@ __global__ void __launch_bounds__(LANES_THREADS, LANES_CTAS_PER_SM) prune64_lane
         const size_t s = (size_t)s0 + row;        // this thread's pattern
         double v[8][2];
         int ex = 0;
+        int nmul = 0;                             // factors multiplied into v since the job's first step
         __syncthreads();                          // previous (class, tile): the buffers are free
         int4 st_a = __ldg(w.steps + i_begin);
         int4 st_b = (i_begin + 1 < i_end) ? __ldg(w.steps + i_begin + 1) : make_int4(0, 0, -1, 0);
@@ -148,6 +149,18 @@ __global__ void __launch_bounds__(LANES_THREADS, LANES_CTAS_PER_SM) prune64_lane
                 ex = 0;
 #pragma unroll
                 for (int j = 0; j < 8; j++) { v[j][0] = 1.0; v[j][1] = 1.0; }
+            }
+            if (flags & STEP_FIRST) nmul = 0;
+            if (nmul++ >= 2) {                    // wide node (hb2_kernels_fp64.cuh); uniform over the CTA
+                if (a.L + (job >= a.I ? job - a.I : job) == a.forced_node) {   // pinned: rescale by the forced state alone
+                    const int f = __ldg(a.forced + s);
+#pragma unroll
+                    for (int j = 0; j < 8; j++) {
+                        if (c0s + 8 * j != f) v[j][0] = 0.0;
+                        if (c0s + 8 * j + 1 != f) v[j][1] = 0.0;
+                    }
+                }
+                rescale_running_quad(v, ex);
             }
             if (child < a.L) {
                 // leaf: column gather PT[state][k]; ambiguous: sum_j amb[j] PT[j][k]
@@ -414,6 +427,17 @@ __global__ void __launch_bounds__(32 * NW, NW == 4 ? 9 : (DP == 32 ? 3 : 4)) pru
                 ex += sc;
 #pragma unroll
                 for (int t = 0; t < NT; t++) { v[t][0] *= acc[t][0]; v[t][1] *= acc[t][1]; }
+            }
+            if (ci - c_begin >= 1 && ci + 1 < c_end) {   // wide node (hb2_kernels_fp64.cuh): before its third and later children
+                if (a.L + par == a.forced_node) {          // pinned: rescale by the forced state alone
+                    const int f = __ldg(a.forced + s);
+#pragma unroll
+                    for (int t = 0; t < NT; t++) {
+                        if (8 * t + 2 * q4 != f) v[t][0] = 0.0;
+                        if (8 * t + 2 * q4 + 1 != f) v[t][1] = 0.0;
+                    }
+                }
+                rescale_running_quad(v, ex);
             }
         }
         if (a.L + par == a.forced_node) {

@@ -588,7 +588,10 @@ __global__ void __launch_bounds__(128, 1) prune64_tc_walk_kernel(WalkArgs w) {
                     }
                 }
             }
-            if ((flags & STEP_LAST) && a.L + par == a.forced_node) {   // pinned internal node (never a side-product slot)
+            // Pinned internal node: only the forced state survives.  Masked after every step of the node and of its side product
+            // (slot I + n), not only at its end: renorm_f32 then follows the forced state itself.  Masked at the end only, a
+            // forced state far less likely than the node's best one fell below the fp32 range on a node with many children.
+            if (a.forced_node >= a.L && a.L + (par >= a.I ? par - a.I : par) == a.forced_node) {
                 const int f = __ldg(a.forced + s);
 #pragma unroll
                 for (int k = 0; k < 64; k++) if (k != f) v[k] = 0.f;
