@@ -316,6 +316,21 @@ int plan_shared(hb2_partition *p, const int *h_dst, int64_t n, int kind, const i
     return 0;
 }
 
+// A template's definition or column frequencies changed.  Its groups' cached power tables were built from matrices the
+// template no longer describes, and the classification compares formula values only, so they must not serve another
+// entry; the formula values its slots keep for hb2_time_resident no longer assemble to the matrices they hold, so those
+// slots cannot be replayed until handed over again.  Stream-ordered after everything flushed so far.
+int void_template_cache(hb2_partition *p, int tmpl) {
+    for (int c = 0; p->ex.d_groups && c < (int)p->C; c++) {
+        const int g = tmpl * (int)p->C + c;
+        if (g >= p->ex.G) break;
+        CU(cudaMemsetAsync(static_cast<hb2::ExpmGroup *>(p->ex.d_groups) + g, 0, sizeof(hb2::ExpmGroup), p->stream));
+        p->ex.kind[g] = 0;
+    }
+    for (size_t k = 0; k < p->is_rate.size(); k++) if (p->is_rate[k] == 2 && p->res_tmpl[k] == tmpl) p->is_rate[k] = 0;
+    return 0;
+}
+
 // One CTA per listed matrix.  is_trans: 0 rate matrices (exponentiated), 1 transition matrices (transposed/padded only),
 // 2 compiled template (dQ = formula values).  pt_override: write the results there instead of the P cache (mixture
 // components go to a scratch area first); pack_tc: also emit the tensor-path operands of the slot.  sp: shared-powers plan
@@ -1472,16 +1487,7 @@ int hb2_set_rate_template_id(hb2_partition *p, int64_t templateId, int64_t nnz, 
     // resident formula values of every slot (replay, shared-powers classification); cached directions of this template's
     // groups are void now
     CU(cudaMalloc(&t.d_Vres, (size_t)p->C * p->B * nFormulas * sizeof(double)));
-    if (p->ex.d_groups) {
-        for (int c = 0; c < (int)p->C; c++) {
-            const int g = (int)templateId * (int)p->C + c;
-            if (g < p->ex.G) {
-                CU(cudaMemset(static_cast<hb2::ExpmGroup *>(p->ex.d_groups) + g, 0, sizeof(hb2::ExpmGroup)));
-                p->ex.kind[g] = 0;
-            }
-        }
-    }
-    for (size_t k = 0; k < p->is_rate.size(); k++) if (p->is_rate[k] == 2 && p->res_tmpl[k] == templateId) p->is_rate[k] = 0;
+    if (void_template_cache(p, (int)templateId)) return 1;
     CU(cudaMallocHost(&t.h_V, (size_t)p->q_capacity * nFormulas * sizeof(double)));
     CU(cudaMallocHost(&t.h_vdst, p->q_capacity * sizeof(int)));
     CU(cudaMemcpy(t.d_index, idx.data(), nnz * sizeof(int), cudaMemcpyHostToDevice));
@@ -1509,7 +1515,7 @@ int hb2_set_template_frequencies(hb2_partition *p, int64_t templateId, const dou
     CU(cudaMemcpyAsync(t.d_colfreq, t.h_colfreq, p->D * sizeof(double), cudaMemcpyHostToDevice, p->stream));
     CU(cudaEventRecord(p->ev_staging, p->stream));
     p->staging_busy = true;
-    return 0;
+    return void_template_cache(p, (int)templateId);
 }
 
 int hb2_set_matrices_compiled_id(hb2_partition *p, int64_t templateId, int64_t cat, int64_t n, const int64_t *nodeIds, const double *formulaValues) {
@@ -1642,7 +1648,10 @@ int hb2_batch_site_likelihoods(hb2_partition *p, int64_t templateId, int64_t nSe
         for (int64_t s = 0; s < nb; s++)
             for (int64_t b = 0; b < B; b++) grp[s * B + b] = (int)(s * p->b_groups_per_set + (branchGroup ? branchGroup[b] : 0));
         SharedPlan sp;
-        std::fill(p->bex.kind.begin(), p->bex.kind.end(), 0);                     // every chunk rebuilds its tables
+        // every chunk rebuilds its tables: a group with fewer than 4 branches must not be compared with a direction cached by
+        // an earlier chunk or call, whose table may come from another template or other column frequencies
+        std::fill(p->bex.kind.begin(), p->bex.kind.end(), 0);
+        CU(cudaMemsetAsync(p->bex.d_groups, 0, (size_t)p->bex.G * sizeof(hb2::ExpmGroup), p->stream));
         if (plan_shared(p, p->h_bdst, ne, 1, grp.data(), sp, (int)templateId, &p->bex, 4)) return 1;
         CU(cudaEventRecord(p->ev_staging, p->stream));
         p->staging_busy = true;
@@ -2001,7 +2010,9 @@ int hb2_time_resident(hb2_partition *p, const double *weights, const double *roo
     std::vector<int> dst;
     int res_kind = 0;
     for (int64_t k = (int64_t)p->own0 * p->B; k < (int64_t)(p->own0 + p->ownN) * p->B; k++) {
-        if (!p->is_rate[k]) return fail("hb2_time_resident needs HB2_MATRIX_RATE matrices in every slot");
+        if (!p->is_rate[k])
+            return fail("hb2_time_resident needs a rate matrix (dense or compiled) in every slot, handed over after its template last "
+                        "changed: class %lld, branch %lld has none", (long long)(k / p->B), (long long)(k % p->B));
         if (res_kind && res_kind != p->is_rate[k]) return fail("hb2_time_resident: hand all matrices over the same way (dense or compiled) before timing");
         if (p->is_rate[k] == 2 && p->res_tmpl[k] != 0) return fail("hb2_time_resident replays template 0 only");
         res_kind = p->is_rate[k];
