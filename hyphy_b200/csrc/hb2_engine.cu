@@ -666,12 +666,19 @@ int plan_walk(const std::vector<std::vector<int>> &children, const std::vector<i
 int run_walk(hb2_partition *p, int cat0, int ncls, const std::vector<std::vector<int>> &levels) {
     const int I = (int)p->I, L = (int)p->L;
     const int T = (int)(p->Sp / hb2::TC_TILE_P);
-    const int CT = ncls * T;
-    int K = std::max(1, std::min(p->walk_lane_cap, p->walk_max_resident / std::max(CT, 1)));
+    // A CTA runs a unit of two tiles of one class (one per warpgroup) or of one.  Lanes are planned over pairs of tiles.
+    int K = std::max(1, std::min(p->walk_lane_cap, p->walk_max_resident / std::max(ncls * ((T + 1) / 2), 1)));
     int total = 0;
     for (auto &lv : levels) total += (int)lv.size();
     if (total == 0) return 0;
     K = std::min(K, total);
+    int pairs = T / 2;                           // two-tile units per class; the rest of the tiles are units of one
+    if (K == 1) {
+        // one lane per unit: split pairs back into single tiles while that leaves no resident CTA without a unit
+        const int units = std::min(T, std::max((T + 1) / 2, p->walk_max_resident / std::max(ncls, 1)));
+        pairs = T - units;
+    }
+    const int CT = ncls * (T - pairs);
     const int nslots = (K == 1) ? std::min(CT, p->walk_max_resident) : CT;
     std::vector<char> dirty(I, 0);
     for (auto &lv : levels) for (int n : lv) dirty[n] = 1;
@@ -710,8 +717,8 @@ int run_walk(hb2_partition *p, int cat0, int ncls, const std::vector<std::vector
     t.L = a.L; t.I = a.I; t.B = a.B; t.D = a.D; t.Sp = a.Sp; t.cat0 = a.cat0;
     t.forced = a.forced; t.forced_node = a.forced_node;
     w.lane_start = p->d_walk; w.steps = reinterpret_cast<const int2 *>(p->d_walk + 16);
-    w.gen = p->d_walk + gen_off; w.NI = 2 * I; w.K = K; w.T = T; w.ncls = ncls; w.nslots = nslots;
-    if (getenv("HB2_DEBUG")) fprintf(stderr, "[hb2] walk: jobs=%d steps=%d K=%d T=%d ncls=%d nslots=%d grid=%d resident=%d\n", total, ns, K, T, ncls, nslots, nslots * K, p->walk_max_resident);
+    w.gen = p->d_walk + gen_off; w.NI = 2 * I; w.K = K; w.T = T; w.ncls = ncls; w.nslots = nslots; w.pairs = pairs;
+    if (getenv("HB2_DEBUG")) fprintf(stderr, "[hb2] walk: jobs=%d steps=%d K=%d T=%d ncls=%d pairs/class=%d units=%d nslots=%d grid=%d resident=%d\n", total, ns, K, T, ncls, pairs, CT, nslots, nslots * K, p->walk_max_resident);
     w.trace = nullptr; w.trace_cta = 0; w.trace_cta_times = nullptr;
     { static const float thr = getenv("HB2_ANCHOR_THR") ? (float)atof(getenv("HB2_ANCHOR_THR")) : hb2::TC_ANCHOR_THR; w.anchor_thr = thr; }
     const char *trace_path = getenv("HB2_WALK_TRACE");
@@ -725,7 +732,7 @@ int run_walk(hb2_partition *p, int cat0, int ncls, const std::vector<std::vector
         w.trace = d_trace;
         w.trace_cta_times = d_trace + (size_t)(ns + 1) * 12;
     }
-    hb2::prune64_tc_walk_kernel<<<nslots * K, 128, hb2::WALK_SMEM_BYTES, p->stream>>>(w);
+    hb2::prune64_tc_walk_kernel<<<nslots * K, 256, hb2::WALK_SMEM_BYTES, p->stream>>>(w);
     if (d_trace) {
         std::vector<long long> ht((size_t)(ns + 1) * 12 + (size_t)nslots * K * 4);
         CU(cudaStreamSynchronize(p->stream));
@@ -1209,7 +1216,7 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
             int per_sm = 0, sms = 0;
             CUP(cudaFuncSetAttribute(hb2::prune64_tc_walk_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
             const void *wk = (const void *)hb2::prune64_tc_walk_kernel;
-            const int wk_threads = 128, wk_smem = hb2::WALK_SMEM_BYTES;
+            const int wk_threads = 256, wk_smem = hb2::WALK_SMEM_BYTES;
             CUP(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, wk, wk_threads, wk_smem));
             if (getenv("HB2_DEBUG")) {
                 cudaFuncAttributes fa; cudaFuncGetAttributes(&fa, wk);
@@ -1220,8 +1227,8 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
             CUP(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
             {   // The lane count is planned from the resources (registers, shared memory) as well as from the occupancy API.
                 // Correctness does not depend on it: blocks are dispatched in index order and a lane only waits for lanes of
-                // its own (class, tile) slot -- adjacent block indices -- with time-bounded waits, so fewer resident CTAs
-                // than planned only make the pass slower.
+                // its own unit (class and a pair or a single tile) -- adjacent block indices -- with time-bounded waits, so
+                // fewer resident CTAs than planned only make the pass slower.
                 cudaFuncAttributes fa;
                 CUP(cudaFuncGetAttributes(&fa, wk));
                 cudaDeviceProp dp; CUP(cudaGetDeviceProperties(&dp, device));

@@ -223,9 +223,14 @@ __device__ __forceinline__ void renorm_f32(float (&v)[64], int &ex, bool force) 
 // Persistent "walk" kernel: the whole pruning pass of one evaluation in ONE launch.
 //
 // Patterns are independent, so all dependencies are tile-local: tile t of node p needs tile t of p's children only.
-// CTA (c, t, r) owns rate class c, pattern tile t and "lane" r (one of K in-order queues of JOBS the host planner
+// CTA (c, u, r) owns rate class c, pattern UNIT u and "lane" r (one of K in-order queues of JOBS the host planner
 // fills, hb2_engine.cu run_walk: a job is an internal node or the side product of a node -- all its children but the
 // deepest -- kept in node slot I + n); it executes its lane's STEPS (one per child of every job) back to back.
+//   * A unit is two tiles (t, t+1) or one.  The CTA has two warpgroups, one per tile of its unit; each runs the
+//     per-pattern code below for its own tile, synchronised only with itself (named barriers).  Every tile of a class
+//     executes the same step list, so both warpgroups need the same branch operands at every step: they share one
+//     staging ring.  One CTA per SM holds 255 registers x 256 threads; while one warpgroup splits, loads or
+//     renormalises, the other's MMAs (or loads) run.  In a single-tile unit warpgroup 1 idles.
 //   * A child computed by another lane of the same (c, t) is awaited on the DATA ITSELF ("tags"): every job has a
 //     generation bit that the host flips each time the job is re-pruned; the producer writes it into the sign bit of
 //     every conditional (they are non-negative) and into bit 0 of the exponent word, and the consumer thread -- which
@@ -237,10 +242,13 @@ __device__ __forceinline__ void renorm_f32(float (&v)[64], int &ex, bool force) 
 //
 // The pass is bound by (tree depth x per-step latency), so every operand of step i+1 is staged while step i runs:
 //   * per step, the branch's fp32 P^T table (64 rows x 256 B, padded to 272 B rows) and -- for a contraction -- its
-//     Ph|Pl operand tiles are bulk-copied (TMA engine, mbarrier tx completion) into a 2-stage shared-memory ring by thread 0
-//     right after the step-begin barrier; leaf column gathers and anchor rows are then shared-memory reads;
-//   * the 32 KB conditional block of the next contraction is prefetched into L2 (cp.async.bulk.prefetch.L2) and the next
-//     leaf's state codes (or the awaited child's generation bit) into a register;
+//     Ph|Pl operand tiles are bulk-copied (TMA engine, mbarrier tx completion) into a 2-stage shared-memory ring;
+//     leaf column gathers and anchor rows are then shared-memory reads.  Ring slot s is released once per use by each
+//     warpgroup of the unit (at its step-begin barrier, a shared-memory counter; the one warpgroup of a single-tile
+//     unit counts twice) and the LAST warpgroup to release it issues the copy of the step after next into it, so the
+//     staging stays a step ahead of whichever warpgroup runs behind;
+//   * the unit's 32 or 64 KB conditional block of the next contraction is prefetched into L2
+//     (cp.async.bulk.prefetch.L2) and the next leaf's state codes (or the awaited child's generation bit) into a register;
 //   * conditionals are stored tile-wise as [16 chunks][128 patterns][4 floats] (the K-major core-matrix order), so
 //     thread t's 16-byte accesses are perfectly coalesced for both the producer and the consumer of a tile.
 // Step encoding: x = child id | WALK_WAIT | WALK_CHAIN | WALK_MUL ; y = job's node slot | STEP_FIRST | STEP_LAST.
@@ -253,7 +261,11 @@ constexpr int STEP_FIRST = 1 << 28;
 constexpr int STEP_LAST = 1 << 29;
 constexpr int WALK_PT_ROW = TC_PTF_ROW;        // same padded rows in shared memory: one flat bulk copy stages the table
 constexpr int WALK_STAGE_FLOATS = 64 * WALK_PT_ROW + 8192;     // P^T table + Ph|Pl tiles
-constexpr int WALK_SMEM_BYTES = 2 * WALK_STAGE_FLOATS * 4 + TC_X_BYTES + TC_D_BYTES + 64;   // ring, A, D, barriers
+// ring (shared), then per warpgroup an A buffer whose first TC_D_BYTES double as the accumulator read-back buffer (A is
+// dead between a warpgroup's wgmma wait and its next split), then the ring's barriers and release counters
+constexpr int WALK_SMEM_BYTES = 2 * WALK_STAGE_FLOATS * 4 + 2 * TC_X_BYTES + 64;
+static_assert(TC_D_BYTES <= TC_X_BYTES, "the accumulator read-back buffer aliases the A operand");
+static_assert(WALK_SMEM_BYTES <= 232448, "one CTA per SM: the sm_90 opt-in limit per block");
 
 struct WalkArgs {
     PruneTcArgs a;
@@ -261,6 +273,7 @@ struct WalkArgs {
     const int2 *steps;
     const int *gen;             // [C][NI] generation bit of every job's conditionals AFTER this pass (see "tags" above)
     int K, T, ncls, nslots;
+    int pairs;                  // two-tile units per class (tiles 0..2*pairs-1); the remaining T - 2*pairs tiles are units of one
     int NI;                     // node slots per class in cond/scal/gen: I real nodes + I side products
     long long *trace;           // nullable debug buffer: 12 clock64 stamps per step of CTA `trace_cta` (HB2_WALK_TRACE)
     long long *trace_cta_times; // nullable: per CTA {smid, clock64 at entry, clock64 at exit, globaltimer at entry}
@@ -287,21 +300,44 @@ __device__ __forceinline__ void prefetch_l2_bulk(const void *p, uint32_t bytes) 
 __device__ __forceinline__ size_t cond_f4(int cat, int node, int tile, int q, int t, int I, int T) {
     return ((((size_t)cat * I + node) * T + tile) * 16 + q) * 128 + t;
 }
+// barrier of the 128 threads of this thread's warpgroup (named barrier 1 + tid/128; 0 is __syncthreads).  The id is
+// re-read from %tid.x: the walk kernel has no register to spare for it.
+__device__ __forceinline__ void wg_bar() {
+    asm volatile("{\n\t.reg .u32 t;\n\tmov.u32 t, %%tid.x;\n\tshr.u32 t, t, 7;\n\tadd.u32 t, t, 1;\n\tbar.sync t, 128;\n\t}" ::"n"(0) : "memory");
+}
+// warp index within the warpgroup, re-read from %tid.x at the use: held in a register across a step it is spilled
+__device__ __forceinline__ int warp_in_wg() {
+    uint32_t q;
+    asm volatile("{\n\t.reg .u32 t;\n\tmov.u32 t, %%tid.x;\n\tbfe.u32 %0, t, 5, 2;\n\t}" : "=r"(q));
+    return (int)q;
+}
+// One warpgroup releases a ring slot (weight 1, or 2 when it is alone in its unit); true for the release that completes
+// the slot's count, i.e. for the last of the two warpgroups.  The counter only grows: it is even between uses.
+__device__ __forceinline__ bool ring_release(uint32_t *cnt, uint32_t weight) {
+    uint32_t old;
+    asm volatile("atom.acq_rel.cta.shared::cta.add.u32 %0, [%1], %2;" : "=r"(old) : "r"(smem_u32(cnt)), "r"(weight) : "memory");
+    return ((old + weight) & 1u) == 0u;
+}
 
-__global__ void __launch_bounds__(128, 1) prune64_tc_walk_kernel(WalkArgs w) {
+__global__ void __launch_bounds__(256, 1) prune64_tc_walk_kernel(WalkArgs w) {
     extern __shared__ __align__(1024) uint8_t smem[];
     const PruneTcArgs &a = w.a;
+    const int wg = threadIdx.x >> 7;                                                // warpgroup = tile of the unit
     float *stage_base = reinterpret_cast<float *>(smem);                           // 2 x [P^T table | Ph | Pl]
-    uint8_t *Xs = smem + 2 * WALK_STAGE_FLOATS * 4;                                 // A operand: Xh | Xl
-    float *Ds = reinterpret_cast<float *>(Xs + TC_X_BYTES);                         // [128][TC_D_ROW] accumulator read-back
-    uint64_t *bar_full = reinterpret_cast<uint64_t *>(Xs + TC_X_BYTES + TC_D_BYTES); // [2]
-    const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
+    uint8_t *Xs = smem + 2 * WALK_STAGE_FLOATS * 4 + wg * TC_X_BYTES;               // A operand: Xh | Xl
+    float *Ds = reinterpret_cast<float *>(Xs);                                      // [128][TC_D_ROW] accumulator read-back
+    uint64_t *bar_full = reinterpret_cast<uint64_t *>(smem + 2 * WALK_STAGE_FLOATS * 4 + 2 * TC_X_BYTES); // [2]
+    uint32_t *ring_rel = reinterpret_cast<uint32_t *>(bar_full + 2);                // [2] release counters
+    int *unit_info = reinterpret_cast<int *>(ring_rel + 2);   // class, first tile, tiles of the unit: read by the stager
+    const int tid = threadIdx.x & 127, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
     const size_t Sp = a.Sp;
     float4 *cond4 = reinterpret_cast<float4 *>(a.cond);
 
-    if (tid == 0) {
+    if (threadIdx.x == 0) {
         mbar_init(bar_full, 1);
         mbar_init(bar_full + 1, 1);
+        ring_rel[0] = 0u;
+        ring_rel[1] = 0u;
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -311,7 +347,7 @@ __global__ void __launch_bounds__(128, 1) prune64_tc_walk_kernel(WalkArgs w) {
 
     const int r = blockIdx.x % w.K;
     const int i_begin = w.lane_start[r], i_end = w.lane_start[r + 1];
-    if (w.trace_cta_times && tid == 0) {
+    if (w.trace_cta_times && threadIdx.x == 0) {
         uint32_t smid; unsigned long long gt;
         asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
         asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
@@ -320,14 +356,15 @@ __global__ void __launch_bounds__(128, 1) prune64_tc_walk_kernel(WalkArgs w) {
     }
 
     // one lane of warp 3: stage the operands of one step into ring slot (m & 1): two flat bulk copies + one L2 prefetch
-    auto stage_step = [&](int cat, int tile, int2 st, uint32_t m) {
+    // of the unit's tiles (adjacent in memory)
+    auto stage_step = [&](int cat, int tile0, int ntiles, int2 st, uint32_t m) {
         const int child = st.x & WALK_ID_MASK;
         const bool internal = child >= a.L;
         float *dst = stage_base + (m & 1u) * WALK_STAGE_FLOATS;
         uint64_t *bar = bar_full + (m & 1u);
         if (st.x & WALK_MUL) {               // side product: no matrix involved; the slot's phase still has to complete
             mbar_expect_tx(bar, 0u);
-            prefetch_l2_bulk(cond4 + cond_f4(cat, child - a.L, tile, 0, 0, w.NI, w.T), 32768u);
+            prefetch_l2_bulk(cond4 + cond_f4(cat, child - a.L, tile0, 0, 0, w.NI, w.T), 32768u * ntiles);
             return;
         }
         const size_t slot = (size_t)cat * a.B + child;
@@ -335,8 +372,8 @@ __global__ void __launch_bounds__(128, 1) prune64_tc_walk_kernel(WalkArgs w) {
         bulk_g2s(dst, a.PTf + slot * TC_PTF_FLOATS, (uint32_t)(TC_PTF_FLOATS * 4), bar);
         if (internal) {
             bulk_g2s(dst + 64 * WALK_PT_ROW, a.PB + slot * TC_PB_FLOATS, 32768u, bar);
-            if (!(st.x & WALK_CHAIN))      // pull the child's conditional block towards L2 (it may still be in DRAM)
-                prefetch_l2_bulk(cond4 + cond_f4(cat, child - a.L, tile, 0, 0, w.NI, w.T), 32768u);
+            if (!(st.x & WALK_CHAIN))      // pull the child's conditional blocks towards L2 (they may still be in DRAM)
+                prefetch_l2_bulk(cond4 + cond_f4(cat, child - a.L, tile0, 0, 0, w.NI, w.T), 32768u * ntiles);
         }
     };
 
@@ -366,17 +403,27 @@ __global__ void __launch_bounds__(128, 1) prune64_tc_walk_kernel(WalkArgs w) {
         }
     };
 
-    for (int ct = blockIdx.x / w.K; ct < w.ncls * w.T; ct += w.nslots) {
-        const int cat = a.cat0 + ct / w.T;
-        const int tile = ct % w.T;
+    const int units = w.T - w.pairs;         // units per class: `pairs` of two tiles, then single tiles
+    for (int ct = blockIdx.x / w.K; ct < w.ncls * units; ct += w.nslots) {
+        const int cat = a.cat0 + ct / units;
+        const int u = ct % units;
+        const int tile0 = u < w.pairs ? 2 * u : w.pairs + u;
+        const int ntiles = u < w.pairs ? 2 : 1;
+        const int tile = tile0 + wg;
         const size_t s = (size_t)tile * TC_TILE_P + tid;
         float v[64];
         int ex = 0;
         if (i_begin == i_end) continue;
         int2 st = __ldg(w.steps + i_begin);
         int2 nx = (i_begin + 1 < i_end) ? __ldg(w.steps + i_begin + 1) : make_int2(0, 0);
-        __syncthreads();                      // previous (class, tile): every read of the ring is complete
-        if (warp == 3 && elect_one()) stage_step(cat, tile, st, n_step);     // an elected lane of warp 3 stages
+        __syncthreads();                      // previous unit: every read of the ring and of unit_info is complete
+        if (threadIdx.x == 0) { unit_info[0] = cat; unit_info[1] = tile0; unit_info[2] = ntiles; }
+        __syncthreads();                      // (kept in shared memory: held in registers, they cost a spill)
+        if (wg == 0 && warp == 3 && elect_one()) stage_step(cat, tile0, ntiles, st, n_step);   // an elected lane of warp 3 stages
+        if (wg >= ntiles) {                   // single-tile unit: warpgroup 1 idles; its ring phases advance all the same
+            n_step += (uint32_t)(i_end - i_begin);
+            continue;
+        }
         // fetched one step ahead: a leaf's state code, or (contractions) the generation bit the child's words must carry
         auto step_aux = [&](int2 q) -> int {
             const int ch = q.x & WALK_ID_MASK;
@@ -393,12 +440,13 @@ __global__ void __launch_bounds__(128, 1) prune64_tc_walk_kernel(WalkArgs w) {
             const uint32_t tagbit = (flags & STEP_LAST) ? ((uint32_t)__ldg(w.gen + (size_t)cat * w.NI + par) << 31) : 0u;   // used at the end
             const bool has_next = (i + 1 < i_end);
             const int2 nx2 = (i + 2 < i_end) ? __ldg(w.steps + i + 2) : make_int2(0, 0);   // descriptors run two steps ahead
-            const bool tr = w.trace && tid == 0 && (int)blockIdx.x == w.trace_cta;
+            const bool tr = w.trace && threadIdx.x == 0 && (int)blockIdx.x == w.trace_cta;      // warpgroup 0
             long long *trp = tr ? w.trace + (size_t)(i - i_begin) * 12 : nullptr;
             if (tr) { trp[0] = ((long long)st.x << 32) | (unsigned)st.y; trp[1] = clock64(); }
-            __syncthreads();                  // (1) everyone is done with step i-1: ring slot (n_step+1)&1 is free
+            wg_bar();                       // (1) the warpgroup is done with step i-1 (ring slot (n_step+1)&1, D rows)
             if (has_next) {
-                if (warp == 3 && elect_one()) stage_step(cat, tile, nx, n_step + 1);
+                if (warp == 3 && elect_one() && ring_release(ring_rel + ((n_step + 1) & 1u), 3u - (uint32_t)unit_info[2]))
+                    stage_step(unit_info[0], unit_info[1], unit_info[2], nx, n_step + 1);
                 next_code = step_aux(nx);
             }
             if ((flags & STEP_FIRST) && !(enc & WALK_CHAIN)) {
@@ -523,7 +571,7 @@ __global__ void __launch_bounds__(128, 1) prune64_tc_walk_kernel(WalkArgs w) {
                     }
                 }
                 if (tr) trp[3] = clock64();
-                __syncthreads();             // (2) A operand complete in shared memory; every thread is done reading the previous D
+                wg_bar();                  // (2) A operand complete in shared memory
                 if (tr) trp[4] = clock64();
                 // 48 wgmma (per 64-pattern half: Xl*Ph, Xh*Pl, Xh*Ph; 8 K-steps of 8 each) into one accumulator per half,
                 // issued by the whole warpgroup once the branch's operands have landed
@@ -575,9 +623,10 @@ __global__ void __launch_bounds__(128, 1) prune64_tc_walk_kernel(WalkArgs w) {
                 wg_pin(d0);
                 wg_pin(d1);
                 if (tr) trp[6] = clock64();
-                wg_store_d(Ds, d0, 0, warp, lane);
-                wg_store_d(Ds, d1, 64, warp, lane);
-                __syncthreads();             // (3) every row of D is in the read-back buffer
+                wg_bar();                  // every warp's MMAs are complete: A is dead and D may overwrite it
+                wg_store_d(Ds, d0, 0, warp_in_wg(), lane);
+                wg_store_d(Ds, d1, 64, warp_in_wg(), lane);
+                wg_bar();                  // (3) every row of D is in the read-back buffer
                 {
                     const float4 *drow = reinterpret_cast<const float4 *>(Ds + (size_t)tid * TC_D_ROW);
 #pragma unroll
@@ -621,7 +670,7 @@ __global__ void __launch_bounds__(128, 1) prune64_tc_walk_kernel(WalkArgs w) {
             nx = nx2;
         }
     }
-    if (w.trace_cta_times && tid == 0) w.trace_cta_times[(size_t)blockIdx.x * 4 + 2] = clock64();
+    if (w.trace_cta_times && threadIdx.x == 0) w.trace_cta_times[(size_t)blockIdx.x * 4 + 2] = clock64();
 }
 
 }  // namespace hb2
