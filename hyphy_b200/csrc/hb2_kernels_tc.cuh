@@ -15,16 +15,19 @@
 // round-to-nearest fp32 FMAs against fp32 rows of P^T while the MMAs run; the tensor core only contracts the diffuse
 // remainder, whose rounding bias is scaled down by its share.
 //
-// Operand staging (wgmma.mma_async m64n64k8, one warpgroup = 128 threads per 64-pattern half of the tile):
-//   A (= X, 128 x 64, K-major) comes from SHARED MEMORY: each of the 128 threads owns one pattern, loads its fp32 row
-//     from HBM, splits it in registers and writes Xh / Xl into the canonical no-swizzle layout (8x16-byte core
-//     matrices; LBO = 2048 B between K chunks, SBO = 128 B between 8-row groups) -- the same [chunk][pattern][4] order
-//     the conditionals have in HBM, so a thread's stores are 16-byte and conflict-free.
-//   B (= P, 64 x 64, K-major) comes from SHARED MEMORY in the same layout (LBO = 1024 B, SBO = 128 B).  The expm stage
-//     writes P already split and tiled that way (the ExpmTcOut epilogues of hb2_kernels_fp64.cuh, mix_reduce_kernel),
-//     so one 32 KB cp.async.bulk (TMA engine, mbarrier completion) per child stages Ph and Pl.
-//   D (128 x 64 fp32) is accumulated in registers (two m64 fragments per warpgroup thread), written to a shared row
-//     buffer and read back one row per thread, multiplied into the running product of the parent held in registers.
+// Operand staging (wgmma.mma_async m64n128k8, one warpgroup = 128 threads = one 128-pattern tile).  The contraction
+// runs transposed, D^T[64 parents][128 patterns] = P * X^T, so that one instruction covers the whole tile: per FMA it
+// reads 3/4 of the shared-memory operand bytes of the m64n64k8 shape with X as A, and it needs half the instructions.
+//   A (= P, 64 x 64, K-major) comes from SHARED MEMORY in the canonical no-swizzle layout (8x16-byte core matrices;
+//     LBO = 1024 B between K chunks, SBO = 128 B between 8-row groups).  The expm stage writes P already split and tiled
+//     that way (the ExpmTcOut epilogues of hb2_kernels_fp64.cuh, mix_reduce_kernel), so one 32 KB cp.async.bulk (TMA
+//     engine, mbarrier completion) per child stages Ph and Pl.
+//   B (= X, 128 x 64, K-major) comes from SHARED MEMORY in the same layout (LBO = 2048 B, SBO = 128 B): each of the 128
+//     threads owns one pattern, loads its fp32 row from HBM, splits it in registers and writes Xh / Xl -- the same
+//     [chunk][pattern][4] order the conditionals have in HBM, so a thread's stores are 16-byte and conflict-free.
+//   D^T (64 x 128 fp32) is accumulated in registers (one 64-register fragment per thread), written to a shared buffer of
+//     one row per pattern and read back one row per thread, multiplied into the running product of the parent held in
+//     registers.
 //
 // Replaces (for D in 33..64) reference tree_evaluator.cpp:3875-4008 (_hy_mvp_blocked<61> + _hy_vvmult_sum<61>).
 #pragma once
@@ -34,12 +37,12 @@
 
 namespace hb2 {
 
-constexpr int TC_TILE_P = 128;                 // patterns per CTA (two wgmma M = 64 halves)
+constexpr int TC_TILE_P = 128;                 // patterns per warpgroup (the wgmma N)
 constexpr int TC_PB_FLOATS = 2 * 4096;         // per (class, branch): Ph tile + Pl tile in canonical layout
 constexpr int TC_PTF_ROW = 68;                 // floats per row of the fp32 P^T table (64 + 4 padding: 272-byte rows)
 constexpr int TC_PTF_FLOATS = 64 * TC_PTF_ROW; // per (class, branch)
-constexpr int TC_X_BYTES = 2 * 16 * 128 * 16;  // A operand: Xh | Xl, [16 chunks][128 patterns][4] fp32 each
-constexpr int TC_D_ROW = 68;                   // floats per row of the shared accumulator read-back buffer
+constexpr int TC_X_BYTES = 2 * 16 * 128 * 16;  // B operand: Xh | Xl, [16 chunks][128 patterns][4] fp32 each
+constexpr int TC_D_ROW = 68;                   // floats per pattern row of the shared accumulator read-back buffer
 constexpr int TC_D_BYTES = 128 * TC_D_ROW * 4;
 constexpr int WALK_FAST_ANCHORS = 4;           // anchors handled by the unrolled fast path of the walk kernel; more go to a loop
 constexpr float TC_ANCHOR_THR = 0.015625f;     // 2^-6 (rows are normalised to max in [0.5,1))
@@ -127,44 +130,51 @@ __device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.s
 // generic-proxy stores to shared memory -> visible to the async proxy (the wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 // keeps the compiler from moving accumulator registers across the asynchronous MMA
-__device__ __forceinline__ void wg_pin(float (&d)[32]) {
+__device__ __forceinline__ void wg_pin(float (&d)[64]) {
 #pragma unroll
-    for (int i = 0; i < 32; i++) asm volatile("" : "+f"(d[i])::"memory");
+    for (int i = 0; i < 64; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
-// D[64 x 64] (+)= A[64 x 8] * B[64 x 8]^T, tf32 operands from shared memory, fp32 accumulator fragment d
-__device__ __forceinline__ void wg_mma_tf32(float (&d)[32], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+// D[64 x 128] (+)= A[64 x 8] * B[128 x 8]^T, tf32 operands from shared memory, fp32 accumulator fragment d
+__device__ __forceinline__ void wg_mma_tf32_n128(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
     asm volatile(
         "{\n\t"
         ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %34, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1;\n\t"
         "}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
         : "l"(a_desc), "l"(b_desc), "r"(accumulate) : "memory");
 }
-// Issues the 24 MMAs of one 64-pattern half m of the tile (small terms first: Xl*Ph, Xh*Pl, then Xh*Ph; 8 K-steps each)
-// into ONE accumulator.  xs: A buffer (TC_X_BYTES, Xh then Xl), pb: Ph then Pl (16 KB each).  The caller brackets the
-// issue with wg_fence() / wg_commit() and waits with wg_wait_all().
-__device__ __forceinline__ void wg_issue_tf32x3(float (&d)[32], uint32_t xs, uint32_t pb, int m) {
-    const uint32_t xh = xs + (uint32_t)m * 1024u, xl = xh + TC_X_BYTES / 2, ph = pb, pl = pb + 16384u;
+// Issues the 24 MMAs of one step, D^T[64 parents][128 patterns] = P * X^T (small terms first: Ph*Xl^T, Pl*Xh^T, then
+// Ph*Xh^T; 8 K-steps each) into ONE accumulator.  pb: Ph then Pl (16 KB each, the A operand), xs: the warpgroup's X
+// buffer (TC_X_BYTES, Xh then Xl, the B operand).  The caller brackets the issue with wg_fence() / wg_commit() and waits
+// with wg_wait_all().
+__device__ __forceinline__ void wg_issue_tf32x3(float (&d)[64], uint32_t pb, uint32_t xs) {
+    const uint32_t ph = pb, pl = pb + 16384u, xh = xs, xl = xs + TC_X_BYTES / 2;
 #pragma unroll
-    for (int kk = 0; kk < 8; kk++) wg_mma_tf32(d, wg_desc(xl + kk * 4096u, 2048u, 128u), wg_desc(ph + kk * 2048u, 1024u, 128u), kk > 0);
+    for (int kk = 0; kk < 8; kk++) wg_mma_tf32_n128(d, wg_desc(ph + kk * 2048u, 1024u, 128u), wg_desc(xl + kk * 4096u, 2048u, 128u), kk > 0);
 #pragma unroll
-    for (int kk = 0; kk < 8; kk++) wg_mma_tf32(d, wg_desc(xh + kk * 4096u, 2048u, 128u), wg_desc(pl + kk * 2048u, 1024u, 128u), 1u);
+    for (int kk = 0; kk < 8; kk++) wg_mma_tf32_n128(d, wg_desc(pl + kk * 2048u, 1024u, 128u), wg_desc(xh + kk * 4096u, 2048u, 128u), 1u);
 #pragma unroll
-    for (int kk = 0; kk < 8; kk++) wg_mma_tf32(d, wg_desc(xh + kk * 4096u, 2048u, 128u), wg_desc(ph + kk * 2048u, 1024u, 128u), 1u);
+    for (int kk = 0; kk < 8; kk++) wg_mma_tf32_n128(d, wg_desc(ph + kk * 2048u, 1024u, 128u), wg_desc(xh + kk * 4096u, 2048u, 128u), 1u);
 }
-// Accumulator fragment of warp q (of its warpgroup), lane l -> rows row0 + 16q + l/4 (+8), columns 8j + 2(l%4) (+1) of
-// the shared [128][TC_D_ROW] read-back buffer.
-__device__ __forceinline__ void wg_store_d(float *Ds, const float (&d)[32], int row0, int q, int lane) {
-    float *r0 = Ds + (size_t)(row0 + 16 * q + (lane >> 2)) * TC_D_ROW + 2 * (lane & 3);
+// Read-back buffer: one row of TC_D_ROW floats per pattern; within the 16-float group g of a row, position 2a + h holds
+// parent 16g + a + 8h.  Accumulator fragment of warp q (of its warpgroup), lane l holds parents 16q + l/4 (+8) x
+// patterns 8j + 2(l%4) (+1), j < 16: its two parents of one pattern are adjacent in that order, so each pattern takes
+// one 8-byte store, and with 68-float rows a warp's stores hit every bank once per half-warp.  The reading thread
+// undoes the permutation in its (compile-time) register indices: see wg_parent.
+__device__ __forceinline__ void wg_store_d(float *Ds, const float (&d)[64], int q, int lane) {
+    float *r0 = Ds + (size_t)(2 * (lane & 3)) * TC_D_ROW + 16 * q + 2 * (lane >> 2);
 #pragma unroll
-    for (int j = 0; j < 8; j++) {
-        *reinterpret_cast<float2 *>(r0 + 8 * j) = make_float2(d[4 * j], d[4 * j + 1]);
-        *reinterpret_cast<float2 *>(r0 + 8 * TC_D_ROW + 8 * j) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+    for (int j = 0; j < 16; j++) {
+        *reinterpret_cast<float2 *>(r0 + 8 * j * TC_D_ROW) = make_float2(d[4 * j], d[4 * j + 2]);
+        *reinterpret_cast<float2 *>(r0 + (8 * j + 1) * TC_D_ROW) = make_float2(d[4 * j + 1], d[4 * j + 3]);
     }
 }
-// One pattern's split row (16 chunks of hi and lo, chunk q = states 4q..4q+3) into the A buffer.
+// parent state at position x of a read-back row
+__host__ __device__ constexpr int wg_parent(int x) { return (x & ~15) + ((x & 15) >> 1) + 8 * (x & 1); }
+// One pattern's split row (16 chunks of hi and lo, chunk q = states 4q..4q+3) into the X buffer.
 __device__ __forceinline__ void store_x_chunk(uint8_t *xs, int q, int pattern, const uint32_t *hi, const uint32_t *lo) {
     *reinterpret_cast<uint4 *>(xs + (size_t)q * 2048 + pattern * 16) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
     *reinterpret_cast<uint4 *>(xs + TC_X_BYTES / 2 + (size_t)q * 2048 + pattern * 16) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
@@ -261,10 +271,10 @@ constexpr int STEP_FIRST = 1 << 28;
 constexpr int STEP_LAST = 1 << 29;
 constexpr int WALK_PT_ROW = TC_PTF_ROW;        // same padded rows in shared memory: one flat bulk copy stages the table
 constexpr int WALK_STAGE_FLOATS = 64 * WALK_PT_ROW + 8192;     // P^T table + Ph|Pl tiles
-// ring (shared), then per warpgroup an A buffer whose first TC_D_BYTES double as the accumulator read-back buffer (A is
+// ring (shared), then per warpgroup an X buffer whose first TC_D_BYTES double as the accumulator read-back buffer (X is
 // dead between a warpgroup's wgmma wait and its next split), then the ring's barriers and release counters
 constexpr int WALK_SMEM_BYTES = 2 * WALK_STAGE_FLOATS * 4 + 2 * TC_X_BYTES + 64;
-static_assert(TC_D_BYTES <= TC_X_BYTES, "the accumulator read-back buffer aliases the A operand");
+static_assert(TC_D_BYTES <= TC_X_BYTES, "the accumulator read-back buffer aliases the X (B) operand");
 static_assert(WALK_SMEM_BYTES <= 232448, "one CTA per SM: the sm_90 opt-in limit per block");
 
 struct WalkArgs {
@@ -324,7 +334,7 @@ __global__ void __launch_bounds__(256, 1) prune64_tc_walk_kernel(WalkArgs w) {
     const PruneTcArgs &a = w.a;
     const int wg = threadIdx.x >> 7;                                                // warpgroup = tile of the unit
     float *stage_base = reinterpret_cast<float *>(smem);                           // 2 x [P^T table | Ph | Pl]
-    uint8_t *Xs = smem + 2 * WALK_STAGE_FLOATS * 4 + wg * TC_X_BYTES;               // A operand: Xh | Xl
+    uint8_t *Xs = smem + 2 * WALK_STAGE_FLOATS * 4 + wg * TC_X_BYTES;               // B operand: Xh | Xl
     float *Ds = reinterpret_cast<float *>(Xs);                                      // [128][TC_D_ROW] accumulator read-back
     uint64_t *bar_full = reinterpret_cast<uint64_t *>(smem + 2 * WALK_STAGE_FLOATS * 4 + 2 * TC_X_BYTES); // [2]
     uint32_t *ring_rel = reinterpret_cast<uint32_t *>(bar_full + 2);                // [2] release counters
@@ -571,17 +581,15 @@ __global__ void __launch_bounds__(256, 1) prune64_tc_walk_kernel(WalkArgs w) {
                     }
                 }
                 if (tr) trp[3] = clock64();
-                wg_bar();                  // (2) A operand complete in shared memory
+                wg_bar();                  // (2) X operand complete in shared memory
                 if (tr) trp[4] = clock64();
-                // 48 wgmma (per 64-pattern half: Xl*Ph, Xh*Pl, Xh*Ph; 8 K-steps of 8 each) into one accumulator per half,
-                // issued by the whole warpgroup once the branch's operands have landed
+                // 24 wgmma (Ph*Xl^T, Pl*Xh^T, Ph*Xh^T; 8 K-steps of 8 each) into one accumulator, issued by the whole
+                // warpgroup once the branch's operands have landed
                 mbar_wait(bar_full + (n_step & 1u), (n_step >> 1) & 1u, a.err);
                 if (tr) trp[5] = clock64();
-                const uint32_t baddr = smem_u32(tab + 64 * WALK_PT_ROW);
-                float d0[32], d1[32];
+                float d[64];
                 wg_fence();
-                wg_issue_tf32x3(d0, xs_addr, baddr, 0);
-                wg_issue_tf32x3(d1, xs_addr, baddr, 1);
+                wg_issue_tf32x3(d, smem_u32(tab + 64 * WALK_PT_ROW), xs_addr);
                 wg_commit();
                 // anchors on the CUDA cores while the tensor core works (rows of the P^T table in shared memory)
                 float acc[64];
@@ -620,20 +628,19 @@ __global__ void __launch_bounds__(256, 1) prune64_tc_walk_kernel(WalkArgs w) {
                     }
                 }
                 wg_wait_all();
-                wg_pin(d0);
-                wg_pin(d1);
+                wg_pin(d);
                 if (tr) trp[6] = clock64();
-                wg_bar();                  // every warp's MMAs are complete: A is dead and D may overwrite it
-                wg_store_d(Ds, d0, 0, warp_in_wg(), lane);
-                wg_store_d(Ds, d1, 64, warp_in_wg(), lane);
+                wg_bar();                  // every warp's MMAs are complete: X is dead and D may overwrite it
+                wg_store_d(Ds, d, warp_in_wg(), lane);
                 wg_bar();                  // (3) every row of D is in the read-back buffer
                 {
                     const float4 *drow = reinterpret_cast<const float4 *>(Ds + (size_t)tid * TC_D_ROW);
 #pragma unroll
                     for (int q = 0; q < 16; q++) {
                         const float4 dd = drow[q];
-                        v[4 * q] *= (dd.x + acc[4 * q]); v[4 * q + 1] *= (dd.y + acc[4 * q + 1]);
-                        v[4 * q + 2] *= (dd.z + acc[4 * q + 2]); v[4 * q + 3] *= (dd.w + acc[4 * q + 3]);
+                        const int k0 = wg_parent(4 * q), k1 = wg_parent(4 * q + 1), k2 = wg_parent(4 * q + 2), k3 = wg_parent(4 * q + 3);
+                        v[k0] *= (dd.x + acc[k0]); v[k1] *= (dd.y + acc[k1]);
+                        v[k2] *= (dd.z + acc[k2]); v[k3] *= (dd.w + acc[k3]);
                     }
                 }
             }
