@@ -198,8 +198,11 @@ struct hb2_partition {
     ExBuf ex;                                 // the partition's own hand-overs
     ExBuf bex;                                // batched one-pattern likelihoods (hb2_batch_site_likelihoods): one group per set
     int64_t b_cap = 0;                        // sets per chunk of the batch buffers below
+    int64_t b_vcap = 0;                       // formula values d_bV holds
     double *d_bPT = nullptr, *d_bV = nullptr, *d_bcond = nullptr, *d_bout = nullptr;
+    double *d_bmixw = nullptr;                // mixture weights of a chunk [sets][rows]
     int *d_bdst = nullptr, *d_bpat = nullptr, *d_bnodeex = nullptr, *h_bdst = nullptr;
+    int *d_brow = nullptr;                    // first component row of each branch [B+1]
     int b_groups_per_set = 1;
     bool ex_enabled = true;                   // HB2_EXPM_SHARED=0 switches the path off (A/B testing)
     int64_t stage_launches[3] = {0, 0, 0};    // launches per evaluation of the last hb2_time_resident {expm, pruning, root}
@@ -1584,8 +1587,12 @@ int hb2_evaluate_classes(hb2_partition *p, const double *weights, int64_t nUpdat
     return evaluate_impl(p, 0, (int)p->C, weights, nUpdate, updateNodes, rootFreqs, lnL, siteL, siteScale);
 }
 
-int hb2_batch_site_likelihoods(hb2_partition *p, int64_t templateId, int64_t nSets, const int64_t *patternOf,
-                               const double *formulaValues, const int64_t *branchGroup, const double *rootFreqs, double *siteLnL) {
+// Body of both batch entry points.  weights == nullptr: one matrix per branch, row b = branch b (FEL's site model).
+// Otherwise branch b owns branchK[b] (NULL: K) consecutive component rows and its transition matrix is the weighted sum of
+// their exponentials, formed inside prune_batch_kernel<true> (MEME's site model).
+static int batch_sites(hb2_partition *p, int64_t templateId, int64_t nSets, const int64_t *patternOf, int64_t K, const int64_t *branchK,
+                       const double *formulaValues, const double *weights, const int64_t *branchGroup, const double *rootFreqs,
+                       double *siteLnL) {
     if (!p || !patternOf || !formulaValues || !rootFreqs || !siteLnL) return fail("null argument");
     if (nSets < 0) return fail("bad set count");
     if (p->Dp != 64) return fail("hb2_batch_site_likelihoods supports 33..64-state (codon) partitions only");
@@ -1603,20 +1610,37 @@ int hb2_batch_site_likelihoods(hb2_partition *p, int64_t templateId, int64_t nSe
     CU(cudaSetDevice(p->device));
     const hb2_partition::Tmpl &t = p->tmpls[templateId];
     const int64_t B = p->B, nF = t.nF;
-    // chunk buffers: P matrices of `cap` sets (32 KB per branch) capped at ~8 GB
-    int64_t cap = std::min<int64_t>(nSets, std::max<int64_t>(1, (int64_t)(8.0e9 / ((double)B * (4096 + 1024 + (double)nF) * 8))));
+    const bool mix = weights != nullptr;
+    // component rows of a set: branch b owns rows row_off[b] .. row_off[b+1]-1.  Component k of every tested branch is the
+    // same rate matrix up to the branch length, so the shared-powers group of a row is (set, branchGroup[b], k).
+    std::vector<int> row_off(B + 1, 0);
+    for (int64_t b = 0; b < B; b++) row_off[b + 1] = row_off[b] + (int)(mix && branchK ? branchK[b] : K);
+    const int64_t R = row_off[B];
+    const int gk = gps * (int)K;                // groups per set
+    // chunk buffers, capped at ~8 GB
+    int64_t cap;
+    if (!mix)                                   // P matrices of `cap` sets (32 KB per branch)
+        cap = std::min<int64_t>(nSets, std::max<int64_t>(1, (int64_t)(8.0e9 / ((double)B * (4096 + 1024 + (double)nF) * 8))));
+    else {                                      // a set's R component matrices, formula values, weights and colsum scratch,
+                                                // the power tables of its groups and its node vectors
+        const double per_set = (double)R * (4096 + 16 * 64 + (double)nF + 1) * 8 + (double)gk * hb2::EXPM_POW_TERMS * 4096 * 8 + (double)p->I * 64 * 8;
+        cap = std::min<int64_t>(nSets, std::max<int64_t>(1, (int64_t)(8.0e9 / per_set)));
+    }
     cap = std::min<int64_t>(cap, 1024);
-    if (cap > p->b_cap || gps > p->b_groups_per_set) {
+    // the buffers hold b_cap sets of up to bex.cap / b_cap rows; chunks are b_cap sets wherever they came from
+    if (cap > p->b_cap || gk > p->b_groups_per_set || p->b_cap * R > p->bex.cap || p->b_cap * R * nF > p->b_vcap) {
         CU(cudaStreamSynchronize(p->stream));
         hb2_partition::ExBuf &x = p->bex;
         for (void *d : {(void *)x.d_int, (void *)x.d_flag, (void *)x.d_weight, (void *)x.d_groups, (void *)x.d_pow, (void *)x.d_refvec, (void *)x.d_flags, (void *)x.d_colsum,
-                        (void *)p->d_bPT, (void *)p->d_bV, (void *)p->d_bcond, (void *)p->d_bout, (void *)p->d_bdst, (void *)p->d_bpat, (void *)p->d_bnodeex}) if (d) cudaFree(d);
+                        (void *)p->d_bPT, (void *)p->d_bV, (void *)p->d_bcond, (void *)p->d_bout, (void *)p->d_bdst, (void *)p->d_bpat, (void *)p->d_bnodeex,
+                        (void *)p->d_bmixw, (void *)p->d_brow}) if (d) cudaFree(d);
         if (x.h_int) cudaFreeHost(x.h_int);
         if (p->h_bdst) cudaFreeHost(p->h_bdst);
         x = hb2_partition::ExBuf();
-        p->d_bPT = p->d_bV = p->d_bcond = p->d_bout = nullptr; p->d_bdst = p->d_bpat = p->d_bnodeex = nullptr; p->h_bdst = nullptr; p->b_cap = 0;
-        const int64_t ne = cap * B;
-        x.G = (int)(cap * gps); x.cap = ne; x.stride = 4096; x.kind.assign(x.G, 0);
+        p->d_bPT = p->d_bV = p->d_bcond = p->d_bout = p->d_bmixw = nullptr; p->d_bdst = p->d_bpat = p->d_bnodeex = p->d_brow = nullptr; p->h_bdst = nullptr;
+        p->b_cap = 0; p->b_vcap = 0;
+        const int64_t ne = cap * R;
+        x.G = (int)(cap * gk); x.cap = ne; x.stride = 4096; x.kind.assign(x.G, 0);
         CU(cudaMalloc(&x.d_int, (size_t)(2 * ne + x.G) * sizeof(int)));
         CU(cudaMallocHost(&x.h_int, (size_t)(2 * ne + x.G) * sizeof(int)));
         CU(cudaMalloc(&x.d_flag, (size_t)ne * sizeof(int)));
@@ -1636,24 +1660,30 @@ int hb2_batch_site_likelihoods(hb2_partition *p, int64_t templateId, int64_t nSe
         CU(cudaMalloc(&p->d_bdst, (size_t)ne * sizeof(int)));
         CU(cudaMalloc(&p->d_bpat, (size_t)cap * sizeof(int)));
         CU(cudaMallocHost(&p->h_bdst, (size_t)(ne + cap) * sizeof(int)));
-        p->b_cap = cap; p->b_groups_per_set = gps;
+        CU(cudaMalloc(&p->d_bmixw, (size_t)ne * sizeof(double)));
+        CU(cudaMalloc(&p->d_brow, (size_t)(B + 1) * sizeof(int)));
+        p->b_cap = cap; p->b_groups_per_set = gk; p->b_vcap = ne * nF;
     }
     double *hs = p->h_small;
     CU(cudaStreamSynchronize(p->stream));
     for (int k = 0; k < p->Dp; k++) hs[k] = k < p->D ? rootFreqs[k] : 0.0;
     CU(cudaMemcpyAsync(p->d_pi, hs, p->Dp * sizeof(double), cudaMemcpyHostToDevice, p->stream));
+    if (mix) CU(cudaMemcpyAsync(p->d_brow, row_off.data(), (size_t)(B + 1) * sizeof(int), cudaMemcpyHostToDevice, p->stream));
     std::vector<int> grp;
     for (int64_t s0 = 0; s0 < nSets; s0 += p->b_cap) {
-        const int64_t nb = std::min<int64_t>(p->b_cap, nSets - s0), ne = nb * B;
+        const int64_t nb = std::min<int64_t>(p->b_cap, nSets - s0), ne = nb * R;
         CU(cudaStreamSynchronize(p->stream));          // previous chunk done: buffers and pinned arrays are free again
-        for (int64_t e = 0; e < ne; e++) p->h_bdst[e] = (int)e;                      // slot in the chunk's P area: set-major
+        for (int64_t e = 0; e < ne; e++) p->h_bdst[e] = (int)e;                      // slot in the chunk's P area: [set][row]
         for (int64_t s = 0; s < nb; s++) p->h_bdst[ne + s] = (int)patternOf[s0 + s];
         CU(cudaMemcpyAsync(p->d_bdst, p->h_bdst, (size_t)ne * sizeof(int), cudaMemcpyHostToDevice, p->stream));
         CU(cudaMemcpyAsync(p->d_bpat, p->h_bdst + ne, (size_t)nb * sizeof(int), cudaMemcpyHostToDevice, p->stream));
-        CU(cudaMemcpyAsync(p->d_bV, formulaValues + (size_t)s0 * B * nF, (size_t)ne * nF * sizeof(double), cudaMemcpyHostToDevice, p->stream));
+        CU(cudaMemcpyAsync(p->d_bV, formulaValues + (size_t)s0 * R * nF, (size_t)ne * nF * sizeof(double), cudaMemcpyHostToDevice, p->stream));
+        if (mix) CU(cudaMemcpyAsync(p->d_bmixw, weights + (size_t)s0 * R, (size_t)ne * sizeof(double), cudaMemcpyHostToDevice, p->stream));
         grp.resize(ne);
         for (int64_t s = 0; s < nb; s++)
-            for (int64_t b = 0; b < B; b++) grp[s * B + b] = (int)(s * p->b_groups_per_set + (branchGroup ? branchGroup[b] : 0));
+            for (int64_t b = 0; b < B; b++)
+                for (int k = 0; k < row_off[b + 1] - row_off[b]; k++)
+                    grp[s * R + row_off[b] + k] = (int)(s * p->b_groups_per_set + (branchGroup ? branchGroup[b] : 0) * K + k);
         SharedPlan sp;
         // every chunk rebuilds its tables: a group with fewer than 4 branches must not be compared with a direction cached by
         // an earlier chunk or call, whose table may come from another template or other column frequencies
@@ -1668,7 +1698,9 @@ int hb2_batch_site_likelihoods(hb2_partition *p, int64_t templateId, int64_t nSe
         ba.PT = p->d_bPT; ba.cond = p->d_bcond; ba.node_ex = p->d_bnodeex; ba.pat = p->d_bpat; ba.leaf = p->d_leaf; ba.ambig = p->d_ambig; ba.pi = p->d_pi;
         ba.tree.child_start = p->d_child_start; ba.tree.child_ids = p->d_child_ids; ba.out = p->d_bout;
         ba.L = (int)p->L; ba.I = (int)p->I; ba.B = (int)B; ba.D = (int)p->D; ba.Sp = (int)p->Sp;
-        hb2::prune_batch_kernel<<<(unsigned)nb, 64, 0, p->stream>>>(ba);
+        ba.mix_w = p->d_bmixw; ba.row_off = p->d_brow; ba.R = (int)R;
+        if (mix) hb2::prune_batch_kernel<true><<<(unsigned)nb, 64, 0, p->stream>>>(ba);
+        else hb2::prune_batch_kernel<false><<<(unsigned)nb, 64, 0, p->stream>>>(ba);
         p->launches++;
         CU(cudaGetLastError());
         CU(cudaMemcpyAsync(siteLnL + s0, p->d_bout, (size_t)nb * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
@@ -1678,6 +1710,24 @@ int hb2_batch_site_likelihoods(hb2_partition *p, int64_t templateId, int64_t nSe
     CU(cudaStreamSynchronize(p->stream));
     if (err) { cudaMemsetAsync(p->d_err, 0, sizeof(int), p->stream); return fail("a device-side wait timed out in the batched exponential (code %d)", err); }
     return 0;
+}
+
+int hb2_batch_site_likelihoods(hb2_partition *p, int64_t templateId, int64_t nSets, const int64_t *patternOf,
+                               const double *formulaValues, const int64_t *branchGroup, const double *rootFreqs, double *siteLnL) {
+    return batch_sites(p, templateId, nSets, patternOf, 1, nullptr, formulaValues, nullptr, branchGroup, rootFreqs, siteLnL);
+}
+
+int hb2_batch_site_mixture_likelihoods(hb2_partition *p, int64_t templateId, int64_t nSets, const int64_t *patternOf, int64_t K,
+                                       const int64_t *branchK, const double *formulaValues, const double *weights,
+                                       const int64_t *branchGroup, const double *rootFreqs, double *siteLnL) {
+    if (!p) return fail("null partition");
+    if (K < 1 || K > 4) return fail("K=%lld outside 1..4", (long long)K);
+    if (!weights) return fail("weights must not be null");
+    if (!formulaValues) return fail("formulaValues must not be null");
+    if (branchK)
+        for (int64_t b = 0; b < p->B; b++)
+            if (branchK[b] < 1 || branchK[b] > K) return fail("branchK[%lld]=%lld outside 1..%lld", (long long)b, (long long)branchK[b], (long long)K);
+    return batch_sites(p, templateId, nSets, patternOf, K, branchK, formulaValues, weights, branchGroup, rootFreqs, siteLnL);
 }
 
 int hb2_read_conditionals(hb2_partition *p, int64_t cat, int64_t inode, double *cond, int32_t *exp2) {
@@ -1968,7 +2018,7 @@ void hb2_destroy(hb2_partition *p) {
     void *dev[] = {p->d_leaf, p->d_scal, p->d_rootE, p->d_child_start, p->d_child_ids, p->d_jobs, p->d_dst, p->d_flag,
                    p->d_mix_dst, p->d_mix_Q, p->d_ambig, p->d_freq, p->d_cond, p->d_PT, p->d_Q, p->d_pi, p->d_rootL, p->d_weights,
                    p->d_partial, p->d_lnL, p->d_siteL, p->d_siteScale, p->d_Qres, p->d_condf, p->d_PB, p->d_PTf, p->d_err, p->d_mix_scratch, p->d_xsend, p->d_xrecv, p->d_xfreq, p->d_xpartial, p->d_bc_out, p->d_bc_outE, p->d_bc_sib, p->d_walk, p->d_forced, p->d_cond_side, p->d_lane_flags, p->d_root_counter, p->ex.d_int, p->ex.d_flag, p->ex.d_weight, p->ex.d_groups, p->ex.d_pow, p->ex.d_refvec, p->ex.d_flags, p->ex.d_colsum, p->bex.d_colsum, p->bex.d_int, p->bex.d_flag, p->bex.d_weight, p->bex.d_groups, p->bex.d_pow, p->bex.d_refvec, p->bex.d_flags,
-                   p->d_bPT, p->d_bV, p->d_bcond, p->d_bout, p->d_bdst, p->d_bpat, p->d_bnodeex};
+                   p->d_bPT, p->d_bV, p->d_bcond, p->d_bout, p->d_bdst, p->d_bpat, p->d_bnodeex, p->d_bmixw, p->d_brow};
     for (void *d : dev) if (d) cudaFree(d);
     if (p->h_Q) cudaFreeHost(p->h_Q);
     if (p->h_small) cudaFreeHost(p->h_small);

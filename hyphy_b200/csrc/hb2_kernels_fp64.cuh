@@ -1442,9 +1442,13 @@ __global__ void __launch_bounds__(256) class_merge_kernel(const double *gath, co
 // parent state k; a child's vector is broadcast from shared memory and column k of P is read from PT[.][j][k] -- 64
 // consecutive doubles per j, coalesced.  fp64 throughout; per-node power-of-two renormalisation like the main kernels.
 // Internal-node vectors live in global scratch cond[s][I][64] (L1/L2 resident: 512 bytes per node).
+// MIX (explicit-form mixtures, MEME's tested branches, MEME.bf:381-386): set s holds R component matrices PT[s][row];
+// branch b mixes rows row_off[b] .. row_off[b+1]-1 (at most 4).  The thread of parent state k forms each entry as
+// sum_c w_c PT_c[j][k], components in order as mix_reduce_kernel (tree.cpp:3047-3089), before it enters the contraction:
+// the mixed matrix never goes to memory.
 // ------------------------------------------------------------------------------------------------
 struct BatchPruneArgs {
-    const double *PT;         // [nSets][B][4096]
+    const double *PT;         // [nSets][B][4096]; MIX: [nSets][R][4096]
     double *cond;             // [nSets][I][64]
     int *node_ex;             // [nSets][I] binary exponents of the node vectors
     const int *pat;           // [nSets] pattern of the partition evaluated by each set
@@ -1454,14 +1458,18 @@ struct BatchPruneArgs {
     TreeDev tree;
     double *out;              // [nSets] log-likelihood of the pattern
     int L, I, B, D, Sp;
+    const double *mix_w;      // MIX: [nSets][R] component weights
+    const int *row_off;       // MIX: [B+1] first component row of each branch
+    int R;                    // MIX: component rows per set
 };
 
+template <bool MIX>
 __global__ void __launch_bounds__(64) prune_batch_kernel(BatchPruneArgs a) {
     __shared__ double xs[64];
     __shared__ double red[2];
     const int s = blockIdx.x, k = threadIdx.x;
     const int pattern = a.pat[s];
-    const double *PTs = a.PT + (size_t)s * a.B * 4096;
+    const double *PTs = a.PT + (size_t)s * (MIX ? a.R : a.B) * 4096;
     double *cs = a.cond + (size_t)s * a.I * 64;
     int *node_ex = a.node_ex + (size_t)s * a.I;
     for (int par = 0; par < a.I; par++) {
@@ -1486,21 +1494,42 @@ __global__ void __launch_bounds__(64) prune_batch_kernel(BatchPruneArgs a) {
         for (int ci = c_begin; ci < c_end; ci++) {
             if (ci - c_begin >= 2) renorm(RESCALE_BELOW);       // wide node: keep the running product normal
             const int child = a.tree.child_ids[ci];
-            const double *PT = PTs + (size_t)child * 4096;
+            const double *PT = PTs + (size_t)(MIX ? a.row_off[child] : child) * 4096;
+            // entry (j, k) of the branch's transition matrix
+            double wc[4];
+            int nc = 1;
+            if constexpr (MIX) {
+                const int r0 = a.row_off[child];
+                nc = a.row_off[child + 1] - r0;
+                const double *ws = a.mix_w + (size_t)s * a.R + r0;      // same address in every thread: a broadcast
+#pragma unroll
+                for (int c = 0; c < 4; c++) wc[c] = c < nc ? ws[c] : 0.0;
+            }
+            auto entry = [&](int j) {
+                if constexpr (!MIX) {
+                    return PT[j * 64 + k];
+                } else {
+                    double e = wc[0] * PT[j * 64 + k];
+#pragma unroll
+                    for (int c = 1; c < 4; c++)
+                        if (c < nc) e = fma(wc[c], PT[(size_t)c * 4096 + j * 64 + k], e);
+                    return e;
+                }
+            };
             double m = 0.0;
             if (child < a.L) {
                 const int code = a.leaf[(size_t)child * a.Sp + pattern];
-                if (code >= 0) m = PT[code * 64 + k];
+                if (code >= 0) m = entry(code);
                 else {
                     const double *amb = a.ambig + (size_t)(-code - 1) * 64;
-                    for (int j = 0; j < a.D; j++) { const double w = amb[j]; if (w != 0.0) m = fma(w, PT[j * 64 + k], m); }
+                    for (int j = 0; j < a.D; j++) { const double w = amb[j]; if (w != 0.0) m = fma(w, entry(j), m); }
                 }
             } else {
                 const int cin = child - a.L;
                 __syncthreads();                 // xs free
                 xs[k] = cs[(size_t)cin * 64 + k];
                 __syncthreads();
-                for (int j = 0; j < a.D; j++) m = fma(xs[j], PT[j * 64 + k], m);
+                for (int j = 0; j < a.D; j++) m = fma(xs[j], entry(j), m);
                 ex += node_ex[cin];
             }
             v *= m;

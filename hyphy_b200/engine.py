@@ -43,6 +43,7 @@ ABI = [
     ("hb2_evaluate_forced", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, _dp, C.c_int64, _ip, _dp, _dp, _ip]),
     ("hb2_evaluate_classes", C.c_int, [C.c_void_p, _dp, C.c_int64, _ip, _dp, _dp, _dp, _ip]),
     ("hb2_batch_site_likelihoods", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, _dp, _ip, _dp, _dp]),
+    ("hb2_batch_site_mixture_likelihoods", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, C.c_int64, _ip, _dp, _dp, _ip, _dp, _dp]),
     ("hb2_read_conditionals", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _dp, _i32p]),
     ("hb2_read_transition", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _dp]),
     ("hb2_comm_unique_id", C.c_int, [C.c_void_p]),
@@ -268,6 +269,32 @@ class Partition:
             assert bg.shape == (self.B,)
         out = np.empty(len(po))
         _check(self._lib.hb2_batch_site_likelihoods(self._h, int(template), len(po), ppo, pv, pbg, ppi, out.ctypes.data_as(_dp)))
+        return out
+
+    def batch_site_mixture_likelihoods(self, pattern_of, formula_values, weights, root_freqs, branch_k=None, branch_group=None,
+                                       template=0):
+        """MEME's site model: branch b mixes branch_k[b] components (None: weights.shape[1] / B on every branch).
+        formula_values: [nSets, R, nF], weights: [nSets, R], R = sum of branch_k; returns the nSets log-likelihoods."""
+        po, ppo = _i(pattern_of)
+        v, pv = _d(formula_values)
+        w, pw = _d(weights)
+        assert v.ndim == 3 and v.shape[0] == len(po) and w.shape == v.shape[:2]
+        pbk = None
+        if branch_k is None:
+            assert w.shape[1] % self.B == 0
+            K = w.shape[1] // self.B
+        else:
+            bk, pbk = _i(branch_k)
+            assert bk.shape == (self.B,) and bk.sum() == w.shape[1]
+            K = int(bk.max())
+        pi, ppi = _d(root_freqs)
+        pbg = None
+        if branch_group is not None:
+            bg, pbg = _i(branch_group)
+            assert bg.shape == (self.B,)
+        out = np.empty(len(po))
+        _check(self._lib.hb2_batch_site_mixture_likelihoods(self._h, int(template), len(po), ppo, K, pbk, pv, pw, pbg, ppi,
+                                                            out.ctypes.data_as(_dp)))
         return out
 
     # -- read-backs --------------------------------------------------------------------------------

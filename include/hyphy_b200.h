@@ -154,6 +154,20 @@ int hb2_batch_site_likelihoods(hb2_partition *p, int64_t templateId, int64_t nSe
                                const double *formulaValues, const int64_t *branchGroup, const double *rootFreqs,
                                double *siteLnL);
 
+/* The same with explicit-form mixtures on the branches (MEME's site model, MEME.bf:381-386 and :656-680): branch b of a
+ * set has branchK[b] components (branchK nullable, B entries in 1..K; NULL = K on every branch; K in 1..4) and its
+ * transition matrix is sum_k w_k Exp(Q_k), components added in order k = 0..branchK[b]-1.  With R = sum_b branchK[b]
+ * component rows per set, in branch order with the components of one branch consecutive:
+ *   formulaValues [nSets][R][nFormulas]  (compiled form of template `templateId`, one template for every row)
+ *   weights       [nSets][R]             (not normalised or checked; a plain branch is one component of weight 1.0)
+ * The shared-powers group of a row is (set, branchGroup[b], k): component k of the tested branches is one rate matrix up
+ * to the branch length.  Everything else as hb2_batch_site_likelihoods; a pattern of likelihood 0 gives -inf, a NaN
+ * weight NaN for its set only. */
+int hb2_batch_site_mixture_likelihoods(hb2_partition *p, int64_t templateId, int64_t nSets, const int64_t *patternOf,
+                                       int64_t K, const int64_t *branchK, const double *formulaValues,
+                                       const double *weights, const int64_t *branchGroup, const double *rootFreqs,
+                                       double *siteLnL);
+
 /* FillInConditionals-style read-back (tree.cpp:3335): conditionals of internal node `inode` (0..I-1), class cat,
  * as S*D doubles (original pattern order) and S binary exponents: true value = cond * 2^exp2. */
 int hb2_read_conditionals(hb2_partition *p, int64_t cat, int64_t inode, double *cond, int32_t *exp2);
