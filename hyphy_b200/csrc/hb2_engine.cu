@@ -156,7 +156,6 @@ struct hb2_partition {
     std::vector<int64_t> parents;
     std::vector<std::vector<int>> children;   // per internal node, flat ids
     std::vector<int> height;                  // per internal node: 0 = only leaf children
-    int max_height = 0;
     // device
     int *d_leaf = nullptr, *d_scal = nullptr, *d_rootE = nullptr, *d_child_start = nullptr, *d_child_ids = nullptr;
     int *d_jobs = nullptr, *d_dst = nullptr, *d_flag = nullptr;
@@ -502,26 +501,40 @@ int stage_matrix(hb2_partition *p, int64_t cat, int64_t node, const double *M, i
     return 0;
 }
 
-// Build the per-level job lists for a set of dirty nodes (closure: parents of dirty nodes and all their ancestors).
-// update == nullptr => whole tree.  Returns levels[h] = internal indices at height h to recompute.
-int plan_levels(hb2_partition *p, int64_t nUpdate, const int64_t *update, std::vector<std::vector<int>> &levels) {
-    levels.assign(p->max_height + 1, {});
-    std::vector<char> dirty(p->I, 0);
+// Checks a flat parent list (leaves 0..L-1, then the internal nodes in post-order, the root last with parent -1) and
+// fills each internal node's children (flat ids, ascending) and height (0 = only leaf children).
+int build_tree(const int64_t *flatParents, int64_t L, int64_t I, std::vector<std::vector<int>> &children, std::vector<int> &height) {
+    children.assign(I, {});
+    int roots = 0;
+    for (int64_t n = 0; n < L + I; n++) {
+        const int64_t par = flatParents[n];
+        if (par == -1) { roots++; if (n != L + I - 1) return fail("root must be the last node (found -1 parent at %lld)", (long long)n); continue; }
+        if (par < 0 || par >= I) return fail("flatParents[%lld]=%lld out of range", (long long)n, (long long)par);
+        if (n >= L && par <= n - L) return fail("internal nodes must be in post-order (node %lld has parent %lld)", (long long)n, (long long)par);
+        children[par].push_back((int)n);
+    }
+    if (roots != 1) return fail("tree must have exactly one root");
+    height.assign(I, 0);
+    for (int64_t i = 0; i < I; i++) {
+        if (children[i].empty()) return fail("internal node %lld has no children", (long long)i);
+        for (int ch : children[i]) if (ch >= L) height[i] = std::max(height[i], height[ch - L] + 1);
+    }
+    return 0;
+}
+
+// The internal nodes to re-prune when the nodes in `update` changed: the parent of each and all its ancestors.
+// update == nullptr or nUpdate < 0 marks every node.  dirty gets one entry per internal node.
+int dirty_nodes(const int64_t *flatParents, int64_t L, int64_t I, int64_t nUpdate, const int64_t *update, std::vector<char> &dirty) {
+    dirty.assign(I, 0);
     if (update == nullptr || nUpdate < 0) {
         std::fill(dirty.begin(), dirty.end(), 1);
-    } else {
-        for (int64_t k = 0; k < nUpdate; k++) {
-            int64_t n = update[k];
-            if (n < 0 || n >= p->L + p->I) return fail("updateNodes[%lld]=%lld out of range", (long long)k, (long long)n);
-            int64_t par = p->parents[n];
-            while (par >= 0 && !dirty[par]) {
-                dirty[par] = 1;
-                par = p->parents[p->L + par];
-            }
-        }
+        return 0;
     }
-    for (int64_t i = 0; i < p->I; i++)
-        if (dirty[i]) levels[p->height[i]].push_back((int)i);
+    for (int64_t k = 0; k < nUpdate; k++) {
+        const int64_t n = update[k];
+        if (n < 0 || n >= L + I) return fail("updateNodes[%lld]=%lld out of range", (long long)k, (long long)n);
+        for (int64_t par = flatParents[n]; par >= 0 && !dirty[par]; par = flatParents[L + par]) dirty[par] = 1;
+    }
     return 0;
 }
 
@@ -664,15 +677,78 @@ int plan_walk(const std::vector<std::vector<int>> &children, const std::vector<i
     return ns;
 }
 
+// The walk plan of a dirty set on K lanes, built into h_walk: lane_start[K+1] (16 ints) | steps (int2 each, from int
+// offset 16).  The plan depends on the tree, the dirty set and K only, and optimisers re-evaluate the same set again and
+// again: when these match the cached plan, h_walk is left as it is.  Returns the step count; *rebuilt tells whether the
+// plan was built anew.
+int cached_plan(hb2_partition *p, const std::vector<char> &dirty, int K, bool canonical_multi, bool *rebuilt = nullptr) {
+    const bool reuse = p->plan_steps > 0 && p->plan_K == K && p->plan_dirty == dirty;
+    if (!reuse) {
+        p->plan_steps = plan_walk(p->children, p->height, (int)p->L, (int)p->I, dirty, K, p->walk_split_nodes, p->h_walk,
+                                  p->h_walk + 16, p->plan_jdirty, canonical_multi);
+        p->plan_K = K; p->plan_dirty = dirty;
+    }
+    if (rebuilt) *rebuilt = !reuse;
+    return p->plan_steps;
+}
+
+// HB2_WALK_TRACE (bring-up aid): clock stamps of the steps of one CTA (HB2_WALK_TRACE_CTA, 12 per step) and, for the
+// tensor walk kernel, 4 stamps of every CTA, written to a text file after the launch.  tools/trace_stats.py and
+// tools/trace_stats_lanes.py parse the file.
+struct WalkTrace {
+    const char *path = getenv("HB2_WALK_TRACE");
+    int cta = 0, ns = 0, ctas = 0;
+    long long *d = nullptr;
+    size_t n = 0;
+    ~WalkTrace() { if (d) cudaFree(d); }
+    // Stamps of a pass of ns steps; ctas = CTAs that stamp their residence (0: none).  d stays null without a trace.
+    int alloc(hb2_partition *p, int ns_, int ctas_) {
+        if (!path) return 0;
+        if (const char *tc = getenv("HB2_WALK_TRACE_CTA")) cta = atoi(tc);
+        ns = ns_; ctas = ctas_;
+        n = (size_t)(ns + 1) * 12 + (size_t)ctas * 4;
+        CU(cudaMalloc(&d, n * sizeof(long long)));
+        CU(cudaMemsetAsync(d, 0, n * sizeof(long long), p->stream));
+        return 0;
+    }
+    // kernel: header prefix naming the kernel; columns: names of the 12 stamps of a step
+    int write(hb2_partition *p, const char *kernel, const char *columns, int K) {
+        if (!d) return 0;
+        std::vector<long long> ht(n);
+        CU(cudaStreamSynchronize(p->stream));
+        CU(cudaMemcpy(ht.data(), d, n * sizeof(long long), cudaMemcpyDeviceToHost));
+        FILE *f = fopen(path, "w");
+        if (!f) return 0;
+        const int *lane_start = p->h_walk, r = cta % K;
+        fprintf(f, "# %scta %d lane %d steps %d..%d ; columns: %s (cycles rel. to first)\n", kernel, cta, r, lane_start[r],
+                lane_start[r + 1], columns);
+        const long long t00 = ht[1];
+        for (int i = 0; i < lane_start[r + 1] - lane_start[r]; i++) {
+            const long long *q = ht.data() + (size_t)i * 12;
+            fprintf(f, "%d 0x%x 0x%x", i, (unsigned)(q[0] >> 32), (unsigned)(q[0] & 0xffffffff));
+            for (int c = 1; c < 12; c++) fprintf(f, " %lld", q[c] ? q[c] - t00 : -1LL);
+            fprintf(f, "\n");
+        }
+        if (ctas > 0) {   // per-CTA residence: "# C <block> <smid> <cycles> <start ns rel. to the earliest CTA>"
+            const long long *ct = ht.data() + (size_t)(ns + 1) * 12;
+            long long g0 = ct[3];
+            for (int b = 0; b < ctas; b++) g0 = std::min(g0, ct[(size_t)b * 4 + 3]);
+            for (int b = 0; b < ctas; b++)
+                fprintf(f, "# C %d %lld %lld %lld\n", b, ct[(size_t)b * 4], ct[(size_t)b * 4 + 2] - ct[(size_t)b * 4 + 1], ct[(size_t)b * 4 + 3] - g0);
+        }
+        fclose(f);
+        return 0;
+    }
+};
+
 // Walk plan for prune64_tc_walk_kernel: K lanes of jobs (nodes and side products, in schedule order), flattened into
 // one step per child.  Layout of the int buffer: lane_start[K+1] (16 ints) | steps (int2 each) | generation bits [C][2I]
-int run_walk(hb2_partition *p, int cat0, int ncls, const std::vector<std::vector<int>> &levels) {
-    const int I = (int)p->I, L = (int)p->L;
+int run_walk(hb2_partition *p, int cat0, int ncls, const std::vector<char> &dirty) {
+    const int I = (int)p->I;
     const int T = (int)(p->Sp / hb2::TC_TILE_P);
     // A CTA runs a unit of two tiles of one class (one per warpgroup) or of one.  Lanes are planned over pairs of tiles.
     int K = std::max(1, std::min(p->walk_lane_cap, p->walk_max_resident / std::max(ncls * ((T + 1) / 2), 1)));
-    int total = 0;
-    for (auto &lv : levels) total += (int)lv.size();
+    const int total = (int)std::count(dirty.begin(), dirty.end(), 1);
     if (total == 0) return 0;
     K = std::min(K, total);
     int pairs = T / 2;                           // two-tile units per class; the rest of the tiles are units of one
@@ -683,35 +759,16 @@ int run_walk(hb2_partition *p, int cat0, int ncls, const std::vector<std::vector
     }
     const int CT = ncls * (T - pairs);
     const int nslots = (K == 1) ? std::min(CT, p->walk_max_resident) : CT;
-    std::vector<char> dirty(I, 0);
-    for (auto &lv : levels) for (int n : lv) dirty[n] = 1;
-    int *buf = p->h_walk;                        // lane_start[K+1] | steps (int2, from int offset 16) | generation bits
-    int ns = p->plan_steps;
-    // the plan depends on the tree, the dirty set and K only: optimisers re-evaluate the same set again and again
-    const bool reuse = p->plan_steps > 0 && p->plan_K == K && p->plan_dirty == dirty;
-    if (!reuse) {
-    ns = plan_walk(p->children, p->height, L, I, dirty, K, p->walk_split_nodes, buf, buf + 16, p->plan_jdirty);
-    p->plan_steps = ns; p->plan_K = K; p->plan_dirty = dirty;
-    }   // !reuse
+    const int ns = cached_plan(p, dirty, K, false);
     // generation bits: every node re-pruned by this pass flips its bit (per class); the kernel tags what it writes with the
     // new bit and awaits cross-lane children on it.  The table travels behind the steps.
     for (int c = cat0; c < cat0 + ncls; c++)
         for (int j = 0; j < 2 * I; j++)
             if (p->plan_jdirty[j]) p->walk_gen[(size_t)c * 2 * I + j] ^= 1;
     const int gen_off = 16 + 2 * ns;
-    std::copy(p->walk_gen.begin(), p->walk_gen.end(), buf + gen_off);
+    std::copy(p->walk_gen.begin(), p->walk_gen.end(), p->h_walk + gen_off);
     const int nints = gen_off + (int)p->walk_gen.size();
-    {
-        cudaError_t ce = cudaMemcpyAsync(p->d_walk, p->h_walk, nints * sizeof(int), cudaMemcpyHostToDevice, p->stream);
-        if (ce != cudaSuccess) {
-            int cur = -1; cudaGetDevice(&cur);
-            cudaPointerAttributes pa{}, pb{};
-            cudaError_t e1 = cudaPointerGetAttributes(&pa, p->d_walk), e2 = cudaPointerGetAttributes(&pb, p->h_walk);
-            return fail("walk plan upload failed: %s; nints=%d ns=%d K=%d total=%d cur_dev=%d part_dev=%d d_walk=%p(type %d dev %d err %d) h_walk=%p(type %d dev %d err %d) stream=%p query=%d",
-                        cudaGetErrorString(ce), nints, ns, K, total, cur, p->device, (void *)p->d_walk, (int)pa.type, pa.device, (int)e1,
-                        (void *)p->h_walk, (int)pb.type, pb.device, (int)e2, (void *)p->stream, (int)cudaStreamQuery(p->stream));
-        }
-    }
+    CU(cudaMemcpyAsync(p->d_walk, p->h_walk, nints * sizeof(int), cudaMemcpyHostToDevice, p->stream));
     hb2::PruneArgs a = prune_args(p, cat0);
     hb2::WalkArgs w;
     hb2::PruneTcArgs &t = w.a;
@@ -722,70 +779,43 @@ int run_walk(hb2_partition *p, int cat0, int ncls, const std::vector<std::vector
     w.lane_start = p->d_walk; w.steps = reinterpret_cast<const int2 *>(p->d_walk + 16);
     w.gen = p->d_walk + gen_off; w.NI = 2 * I; w.K = K; w.T = T; w.ncls = ncls; w.nslots = nslots; w.pairs = pairs;
     if (getenv("HB2_DEBUG")) fprintf(stderr, "[hb2] walk: jobs=%d steps=%d K=%d T=%d ncls=%d pairs/class=%d units=%d nslots=%d grid=%d resident=%d\n", total, ns, K, T, ncls, pairs, CT, nslots, nslots * K, p->walk_max_resident);
-    w.trace = nullptr; w.trace_cta = 0; w.trace_cta_times = nullptr;
     { static const float thr = getenv("HB2_ANCHOR_THR") ? (float)atof(getenv("HB2_ANCHOR_THR")) : hb2::TC_ANCHOR_THR; w.anchor_thr = thr; }
-    const char *trace_path = getenv("HB2_WALK_TRACE");
-    long long *d_trace = nullptr;
-    if (trace_path) {          // bring-up aid: per-step clock stamps of one CTA -> text file
-        const char *tc = getenv("HB2_WALK_TRACE_CTA");
-        w.trace_cta = tc ? atoi(tc) : 0;
-        const size_t tr_n = (size_t)(ns + 1) * 12 + (size_t)nslots * K * 4;
-        CU(cudaMalloc(&d_trace, tr_n * sizeof(long long)));
-        CU(cudaMemsetAsync(d_trace, 0, tr_n * sizeof(long long), p->stream));
-        w.trace = d_trace;
-        w.trace_cta_times = d_trace + (size_t)(ns + 1) * 12;
-    }
+    WalkTrace trace;
+    if (trace.alloc(p, ns, nslots * K)) return 1;
+    w.trace = trace.d; w.trace_cta = trace.cta; w.trace_cta_times = trace.d ? trace.d + (size_t)(ns + 1) * 12 : nullptr;
     hb2::prune64_tc_walk_kernel<<<nslots * K, 256, hb2::WALK_SMEM_BYTES, p->stream>>>(w);
-    if (d_trace) {
-        std::vector<long long> ht((size_t)(ns + 1) * 12 + (size_t)nslots * K * 4);
-        CU(cudaStreamSynchronize(p->stream));
-        CU(cudaMemcpy(ht.data(), d_trace, ht.size() * sizeof(long long), cudaMemcpyDeviceToHost));
-        cudaFree(d_trace);
-        if (FILE *f = fopen(trace_path, "w")) {
-            const int r = w.trace_cta % K;
-            fprintf(f, "# cta %d lane %d steps %d..%d ; columns: child_enc parent_flags t_begin bar1 staged/ready tableready|split bar2 bfull mma_done end (cycles rel. to first)\n", w.trace_cta, r, buf[r], buf[r + 1]);
-            const long long t00 = ht[1];
-            for (int i = 0; i < buf[r + 1] - buf[r]; i++) {
-                const long long *q = ht.data() + (size_t)i * 12;
-                fprintf(f, "%d 0x%x 0x%x", i, (unsigned)(q[0] >> 32), (unsigned)(q[0] & 0xffffffff));
-                for (int c = 1; c < 12; c++) fprintf(f, " %lld", q[c] ? q[c] - t00 : -1LL);
-                fprintf(f, "\n");
-            }
-            {   // per-CTA residence: "# C <block> <smid> <cycles> <start ns rel. to the earliest CTA>"
-                const long long *ct = ht.data() + (size_t)(ns + 1) * 12;
-                long long g0 = ct[3];
-                for (int b = 0; b < nslots * K; b++) g0 = std::min(g0, ct[(size_t)b * 4 + 3]);
-                for (int b = 0; b < nslots * K; b++)
-                    fprintf(f, "# C %d %lld %lld %lld\n", b, ct[(size_t)b * 4], ct[(size_t)b * 4 + 2] - ct[(size_t)b * 4 + 1], ct[(size_t)b * 4 + 3] - g0);
-            }
-            fclose(f);
-        }
-    }
+    if (trace.write(p, "", "child_enc parent_flags t_begin bar1 staged/ready tableready|split bar2 bfull mma_done end", K)) return 1;
     p->launches++;
     CU(cudaGetLastError());
     return 0;
 }
 
-// 4 states: one or two patterns per thread -- (passes over the resident capacity) x (relative cost of a pass: a two-pattern
-// pass costs about 1.55 one-pattern passes)
-static bool small_two_patterns(const hb2_partition *p, int ncls) {
-    if (p->Dp != 4 || p->small_ilp == 1) return false;
-    if (p->small_ilp == 2) return true;
+// The pruning kernels, each of which prunes the dirty nodes of a pass in one launch: the tensor walk (33..64 states), the
+// fp64 lanes kernel (33..64 states with HB2_FLAG_FORCE_FP64) and the small-state walks (<= 32 padded states).
+enum PruneKernel { TC_WALK, FP64_LANES, SMALL_DMMA, SMALL_WALK_ILP, SMALL_WALK };
+const char *const PRUNE_KERNEL_NAME[] = {"prune64_tc_walk_kernel", "prune64_lanes_kernel", "prune_small_dmma_kernel",
+                                         "prune_small_walk_ilp_kernel", "prune_small_walk_kernel"};
+
+// The kernel that prunes ncls classes of p.  4 states: one or two patterns per thread -- (passes over the resident
+// capacity) x (relative cost of a pass: a two-pattern pass costs about 1.55 one-pattern passes)
+PruneKernel pruning_kernel(const hb2_partition *p, int ncls) {
+    if (p->use_tc) return TC_WALK;
+    if (p->Dp == 64) return FP64_LANES;
+    if (p->Dp >= 16) return SMALL_DMMA;
+    if (p->Dp != 4 || p->small_ilp == 1) return SMALL_WALK;
+    if (p->small_ilp == 2) return SMALL_WALK_ILP;
     const long ct1 = (long)(p->Sp / 128) * ncls, ct2 = (long)((p->Sp + 255) / 256) * ncls;
-    return 1.55 * std::ceil((double)ct2 / p->small_resident[1]) < std::ceil((double)ct1 / p->small_resident[0]);
+    return 1.55 * std::ceil((double)ct2 / p->small_resident[1]) < std::ceil((double)ct1 / p->small_resident[0]) ? SMALL_WALK_ILP : SMALL_WALK;
 }
 
-// Small state spaces: one launch, every CTA walking the dirty nodes in post-order.
-int run_small_walk(hb2_partition *p, int cat0, int ncls, const std::vector<std::vector<int>> &levels) {
-    std::vector<int> jobs;
-    for (auto &lv : levels) jobs.insert(jobs.end(), lv.begin(), lv.end());
-    if (jobs.empty()) return 0;
-    std::sort(jobs.begin(), jobs.end());                 // internal indices ascending == post-order
-    std::copy(jobs.begin(), jobs.end(), p->h_jobs);
-    CU(cudaMemcpyAsync(p->d_jobs, p->h_jobs, jobs.size() * sizeof(int), cudaMemcpyHostToDevice, p->stream));
+// Small state spaces: one launch, every CTA walking the dirty nodes in post-order (internal indices ascending).
+int run_small_walk(hb2_partition *p, int cat0, int ncls, const std::vector<char> &dirty, PruneKernel kernel) {
+    int n = 0;
+    for (int i = 0; i < (int)p->I; i++) if (dirty[i]) p->h_jobs[n++] = i;
+    if (n == 0) return 0;
+    CU(cudaMemcpyAsync(p->d_jobs, p->h_jobs, n * sizeof(int), cudaMemcpyHostToDevice, p->stream));
     hb2::PruneArgs a = prune_args(p, cat0);
-    const int n = (int)jobs.size();
-    if (p->Dp >= 16) {                           // 16 / 24 / 32 padded states: FP64 tensor pipe, 8 patterns per warp
+    if (kernel == SMALL_DMMA) {                  // 16 / 24 / 32 padded states: FP64 tensor pipe, 8 patterns per warp
         // every CTA walks the whole tree: the launch is a few long waves.  Shape with the smaller last-wave loss: 8 warps
         // (4 CTAs per SM; 3 at 32 states) or, up to 24 states, 4 warps (9 per SM).
         const double warps = (double)(p->Sp / 8) * ncls;
@@ -806,22 +836,16 @@ int run_small_walk(hb2_partition *p, int cat0, int ncls, const std::vector<std::
             if (p->Dp == 16) hb2::prune_small_dmma_kernel<16, 4><<<g, 128, 0, p->stream>>>(a, p->d_jobs, n);
             else hb2::prune_small_dmma_kernel<24, 4><<<g, 128, 0, p->stream>>>(a, p->d_jobs, n);
         }
-        p->launches++;
-        CU(cudaGetLastError());
-        return 0;
-    }
-    if (small_two_patterns(p, ncls)) {
+    } else if (kernel == SMALL_WALK_ILP) {
         dim3 g2((unsigned)((p->Sp + 255) / 256), (unsigned)ncls);
         hb2::prune_small_walk_ilp_kernel<4, 2><<<g2, 128, 0, p->stream>>>(a, p->d_jobs, n);
-        p->launches++;
-        CU(cudaGetLastError());
-        return 0;
-    }
-    dim3 grid((unsigned)(p->Sp / 128), (unsigned)ncls);   // 4 / 8 padded states: one thread per pattern
-    switch (p->Dp) {
-        case 4: hb2::prune_small_walk_kernel<4><<<grid, 128, 0, p->stream>>>(a, p->d_jobs, n); break;
-        case 8: hb2::prune_small_walk_kernel<8><<<grid, 128, 0, p->stream>>>(a, p->d_jobs, n); break;
-        default: return fail("unsupported padded state count %d", p->Dp);
+    } else {
+        dim3 grid((unsigned)(p->Sp / 128), (unsigned)ncls);   // 4 / 8 padded states: one thread per pattern
+        switch (p->Dp) {
+            case 4: hb2::prune_small_walk_kernel<4><<<grid, 128, 0, p->stream>>>(a, p->d_jobs, n); break;
+            case 8: hb2::prune_small_walk_kernel<8><<<grid, 128, 0, p->stream>>>(a, p->d_jobs, n); break;
+            default: return fail("unsupported padded state count %d", p->Dp);
+        }
     }
     p->launches++;
     CU(cudaGetLastError());
@@ -830,22 +854,17 @@ int run_small_walk(hb2_partition *p, int cat0, int ncls, const std::vector<std::
 
 // 33..64 states in fp64: one launch, K in-order lanes per (class, 32-pattern tile) (prune64_lanes_kernel).  Same
 // planner and plan cache as the tensor walk; the step list travels without a generation table (hand-over by pass id).
-int run_fp64_lanes(hb2_partition *p, int cat0, int ncls, const std::vector<std::vector<int>> &levels) {
+int run_fp64_lanes(hb2_partition *p, int cat0, int ncls, const std::vector<char> &dirty) {
     const int I = (int)p->I, L = (int)p->L;
-    int total = 0;
-    for (auto &lv : levels) total += (int)lv.size();
+    const int total = (int)std::count(dirty.begin(), dirty.end(), 1);
     if (total == 0) return 0;
     const int T = (int)(p->Sp / hb2::LANES_TILE_P), CT = ncls * T, resident = p->lanes_resident;
     const int K = std::max(1, std::min(std::min(p->walk_lane_cap, total), resident / std::max(CT, 1)));
     const int nslots = (K == 1) ? std::min(CT, resident) : CT;
-    std::vector<char> dirty(I, 0);
-    for (auto &lv : levels) for (int n : lv) dirty[n] = 1;
     int *buf = p->h_walk;
-    int ns = p->plan_steps;
-    const bool reuse = p->plan_steps > 0 && p->plan_K == K && p->plan_dirty == dirty;
-    if (!reuse) {
-        ns = plan_walk(p->children, p->height, L, I, dirty, K, p->walk_split_nodes, buf, buf + 16, p->plan_jdirty, true);
-        p->plan_steps = ns; p->plan_K = K; p->plan_dirty = dirty;
+    bool rebuilt = false;
+    const int ns = cached_plan(p, dirty, K, true, &rebuilt);
+    if (rebuilt) {
         // the kernel's descriptors: (child, job, branch id of the lane's next contraction, -) behind the planner's pairs
         int *d4 = buf + ((16 + 2 * ns + 3) & ~3);
         std::vector<char> awaited(2 * I, 0);                 // jobs some other lane waits for: only those publish a flag
@@ -872,46 +891,22 @@ int run_fp64_lanes(hb2_partition *p, int cat0, int ncls, const std::vector<std::
     w.flags = p->d_lane_flags; w.err = p->d_err;
     w.K = K; w.T = T; w.ncls = ncls; w.nslots = nslots; w.pass = ++p->lane_pass;
     if (getenv("HB2_DEBUG")) fprintf(stderr, "[hb2] fp64 lanes: jobs=%d steps=%d K=%d T=%d ncls=%d nslots=%d grid=%d resident=%d\n", total, ns, K, T, ncls, nslots, nslots * K, resident);
-    w.trace = nullptr; w.trace_cta = 0;
-    const char *trace_path = getenv("HB2_WALK_TRACE");
-    long long *d_trace = nullptr;
-    if (trace_path) {          // bring-up aid: per-step clock stamps of one CTA -> text file
-        const char *tc = getenv("HB2_WALK_TRACE_CTA");
-        w.trace_cta = tc ? atoi(tc) : 0;
-        CU(cudaMalloc(&d_trace, (size_t)(ns + 1) * 12 * sizeof(long long)));
-        CU(cudaMemsetAsync(d_trace, 0, (size_t)(ns + 1) * 12 * sizeof(long long), p->stream));
-        w.trace = d_trace;
-    }
+    WalkTrace trace;
+    if (trace.alloc(p, ns, 0)) return 1;
+    w.trace = trace.d; w.trace_cta = trace.cta;
     hb2::prune64_lanes_kernel<<<nslots * K, hb2::LANES_THREADS, hb2::LANES_SMEM_BYTES, p->stream>>>(w);
-    if (d_trace) {
-        std::vector<long long> ht((size_t)(ns + 1) * 12);
-        CU(cudaStreamSynchronize(p->stream));
-        CU(cudaMemcpy(ht.data(), d_trace, ht.size() * sizeof(long long), cudaMemcpyDeviceToHost));
-        cudaFree(d_trace);
-        if (FILE *f = fopen(trace_path, "w")) {
-            const int r = w.trace_cta % K;
-            fprintf(f, "# fp64 lanes kernel, cta %d lane %d steps %d..%d ; columns: child_enc job_flags begin staged landed barrier product barrier2 body_end stored barrier3 published (cycles rel. to first)\n", w.trace_cta, r, buf[r], buf[r + 1]);
-            const long long t00 = ht[1];
-            for (int i = 0; i < buf[r + 1] - buf[r]; i++) {
-                const long long *q = ht.data() + (size_t)i * 12;
-                fprintf(f, "%d 0x%x 0x%x", i, (unsigned)(q[0] >> 32), (unsigned)(q[0] & 0xffffffff));
-                for (int c = 1; c < 12; c++) fprintf(f, " %lld", q[c] ? q[c] - t00 : -1LL);
-                fprintf(f, "\n");
-            }
-            fclose(f);
-        }
-    }
+    if (trace.write(p, "fp64 lanes kernel, ", "child_enc job_flags begin staged landed barrier product barrier2 body_end stored barrier3 published", K)) return 1;
     p->launches++;
     CU(cudaGetLastError());
     return 0;
 }
 
-// One launch per evaluation: the tensor walk (33..64 states), the fp64 lanes kernel (33..64 states with
-// HB2_FLAG_FORCE_FP64) or the small-state walk (<= 32 padded states).
-int run_pruning(hb2_partition *p, int cat0, int ncls, const std::vector<std::vector<int>> &levels) {
-    if (p->use_tc) return run_walk(p, cat0, ncls, levels);
-    if (p->Dp == 64) return run_fp64_lanes(p, cat0, ncls, levels);
-    return run_small_walk(p, cat0, ncls, levels);
+// One launch per evaluation, of the kernel pruning_kernel chooses.
+int run_pruning(hb2_partition *p, int cat0, int ncls, const std::vector<char> &dirty) {
+    const PruneKernel kernel = pruning_kernel(p, ncls);
+    if (kernel == TC_WALK) return run_walk(p, cat0, ncls, dirty);
+    if (kernel == FP64_LANES) return run_fp64_lanes(p, cat0, ncls, dirty);
+    return run_small_walk(p, cat0, ncls, dirty, kernel);
 }
 
 // (Re)creates the peer-exchange buffers with room for `payload` doubles per rank and maps every other rank's buffer through
@@ -1108,14 +1103,12 @@ int evaluate_impl(hb2_partition *p, int c0, int nc, const double *weights, int64
     // classes never pruned before need the whole tree regardless of updateNodes (likefunc.cpp:10965-10967)
     bool all = (updateNodes == nullptr || nUpdate < 0);
     for (int c = c0; c < c0 + nc; c++) if (!p->evaluated_cat[c]) all = true;
-    std::vector<std::vector<int>> levels;
-    if (plan_levels(p, all ? -1 : nUpdate, all ? nullptr : updateNodes, levels)) return 1;
+    std::vector<char> dirty;
+    if (dirty_nodes(p->parents.data(), p->L, p->I, all ? -1 : nUpdate, all ? nullptr : updateNodes, dirty)) return 1;
     // the root must always be recomputed when anything changed; if nothing is dirty (only pi/weights changed)
     // the root tile products are still valid but rootL depends on pi -> recompute the root node
-    bool any = false;
-    for (auto &lv : levels) any = any || !lv.empty();
-    if (!any) levels[p->height[p->I - 1]].push_back((int)p->I - 1);
-    if (run_pruning(p, c0, nc, levels)) return 1;
+    if (std::count(dirty.begin(), dirty.end(), 1) == 0) dirty[p->I - 1] = 1;
+    if (run_pruning(p, c0, nc, dirty)) return 1;
     const bool want_sites = siteL != nullptr || siteScale != nullptr;
     if (run_root(p, c0, nc, weights != nullptr, want_sites)) return 1;
     CU(cudaMemcpyAsync(hs + p->Dp + p->C, p->d_lnL, sizeof(double), cudaMemcpyDeviceToHost, p->stream));
@@ -1132,6 +1125,30 @@ int evaluate_impl(hb2_partition *p, int c0, int nc, const double *weights, int64
     }
     *lnL = hs[p->Dp + p->C];
     for (int c = c0; c < c0 + nc; c++) p->evaluated_cat[c] = 1;
+    return 0;
+}
+
+// CTAs of a lane kernel (the tensor walk or the fp64 lanes kernel) that one SM holds: what the occupancy API reports or,
+// where that is more, what the registers and shared memory allow up to `cap` (the API under-reports for the tensor walk
+// kernel).  HB2_WALK_CTAS_PER_SM overrides the result.  Correctness does not depend on it: blocks are dispatched in index
+// order and a lane only waits for lanes of its own unit -- adjacent block indices -- with time-bounded waits, so fewer
+// resident CTAs than planned only make the pass slower.
+int lane_ctas_per_sm(const char *name, const void *fn, int threads, int smem, int cap, int device, int &per_sm) {
+    CU(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    CU(cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, threads, smem));
+    cudaFuncAttributes fa;
+    CU(cudaFuncGetAttributes(&fa, fn));
+    cudaDeviceProp dp;
+    CU(cudaGetDeviceProperties(&dp, device));
+    const int regs_per_cta = ((fa.numRegs + 7) / 8 * 8) * threads;
+    const size_t smem_per_cta = (size_t)smem + fa.sharedSizeBytes + dp.reservedSharedMemPerBlock;
+    const int by_res = std::min(dp.regsPerMultiprocessor / std::max(regs_per_cta, 1), (int)(dp.sharedMemPerMultiprocessor / smem_per_cta));
+    if (getenv("HB2_DEBUG"))
+        fprintf(stderr, "[hb2] %s occupancy: API %d, by resources %d CTAs/SM (regs/thread %d, static smem %zu, dyn smem %d, regs/SM %d, smem/SM %zu, reserved/block %zu)\n",
+                name, per_sm, by_res, fa.numRegs, fa.sharedSizeBytes, smem, dp.regsPerMultiprocessor, dp.sharedMemPerMultiprocessor, dp.reservedSharedMemPerBlock);
+    per_sm = std::max(per_sm, std::min(by_res, cap));
+    if (const char *ov = getenv("HB2_WALK_CTAS_PER_SM")) per_sm = atoi(ov);      // bring-up override
     return 0;
 }
 
@@ -1175,28 +1192,13 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
     const int64_t tile = (Dp == 64 && !p->use_tc) ? 64 : 128;
     p->Sp = (S + tile - 1) / tile * tile;
     p->parents.assign(flatParents, flatParents + L + I);
-    p->children.assign(I, {});
-    int roots = 0;
-    for (int64_t n = 0; n < L + I; n++) {
-        int64_t par = flatParents[n];
-        if (par == -1) { roots++; if (n != L + I - 1) { delete p; return fail("root must be the last node (found -1 parent at %lld)", (long long)n); } continue; }
-        if (par < 0 || par >= I) { delete p; return fail("flatParents[%lld]=%lld out of range", (long long)n, (long long)par); }
-        if (n >= L && par <= n - L) { delete p; return fail("internal nodes must be in post-order (node %lld has parent %lld)", (long long)n, (long long)par); }
-        p->children[par].push_back((int)n);
-    }
-    if (roots != 1) { delete p; return fail("tree must have exactly one root"); }
-    p->height.assign(I, 0);
-    for (int64_t i = 0; i < I; i++) {
-        if (p->children[i].empty()) { delete p; return fail("internal node %lld has no children", (long long)i); }
-        int h = 0;
-        for (int ch : p->children[i]) if (ch >= L) h = std::max(h, p->height[ch - L] + 1);
-        p->height[i] = h;
-        p->max_height = std::max(p->max_height, h);
-    }
+    if (build_tree(flatParents, L, I, p->children, p->height)) { delete p; return 1; }
     for (int64_t k = 0; k < L * S; k++) {
         int64_t c = leafState[k];
         if (c >= D || c < -nAmb) { delete p; return fail("leafState[%lld]=%lld out of range", (long long)k, (long long)c); }
     }
+    if (const char *ov = getenv("HB2_WALK_LANES")) p->walk_lane_cap = std::max(1, std::min(atoi(ov), 15));
+    { const char *ev = getenv("HB2_WALK_SPLIT_NODES"); p->walk_split_nodes = !(ev && ev[0] == '0'); }
 #define CUP(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { fail("%s failed: %s", #x, cudaGetErrorString(e_)); hb2_destroy(p); return 1; } } while (0)
     CUP(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
     for (auto &e : p->ev) CUP(cudaEventCreate(&e));
@@ -1214,47 +1216,21 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
         CUP(cudaMemsetAsync(p->d_condf, 0, (size_t)C * 2 * I * Sp * 64 * sizeof(float), p->stream));
         CUP(cudaMemsetAsync(p->d_PB, 0, (size_t)C * p->B * hb2::TC_PB_FLOATS * sizeof(float), p->stream));
         CUP(cudaMemsetAsync(p->d_PTf, 0, (size_t)C * p->B * hb2::TC_PTF_FLOATS * sizeof(float), p->stream));
-        CUP(cudaFuncSetAttribute(hb2::prune64_tc_walk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, hb2::WALK_SMEM_BYTES));
-        {
-            int per_sm = 0, sms = 0;
-            CUP(cudaFuncSetAttribute(hb2::prune64_tc_walk_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-            const void *wk = (const void *)hb2::prune64_tc_walk_kernel;
-            const int wk_threads = 256, wk_smem = hb2::WALK_SMEM_BYTES;
-            CUP(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, wk, wk_threads, wk_smem));
-            if (getenv("HB2_DEBUG")) {
-                cudaFuncAttributes fa; cudaFuncGetAttributes(&fa, wk);
-                cudaDeviceProp dp; cudaGetDeviceProperties(&dp, device);
-                fprintf(stderr, "[hb2] walk kernel occupancy: %d CTAs/SM (regs/thread %d, static smem %zu, dyn smem %d, regs/SM %d, smem/SM %zu, smem/block optin %zu, reserved/block %zu)\n",
-                        per_sm, fa.numRegs, fa.sharedSizeBytes, wk_smem, dp.regsPerMultiprocessor, dp.sharedMemPerMultiprocessor, dp.sharedMemPerBlockOptin, dp.reservedSharedMemPerBlock);
-            }
-            CUP(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
-            {   // The lane count is planned from the resources (registers, shared memory) as well as from the occupancy API.
-                // Correctness does not depend on it: blocks are dispatched in index order and a lane only waits for lanes of
-                // its own unit (class and a pair or a single tile) -- adjacent block indices -- with time-bounded waits, so
-                // fewer resident CTAs than planned only make the pass slower.
-                cudaFuncAttributes fa;
-                CUP(cudaFuncGetAttributes(&fa, wk));
-                cudaDeviceProp dp; CUP(cudaGetDeviceProperties(&dp, device));
-                const int regs_per_cta = ((fa.numRegs + 7) / 8 * 8) * wk_threads;
-                const size_t smem_per_cta = (size_t)wk_smem + fa.sharedSizeBytes + dp.reservedSharedMemPerBlock;
-                const int by_res = std::min(dp.regsPerMultiprocessor / std::max(regs_per_cta, 1), (int)(dp.sharedMemPerMultiprocessor / smem_per_cta));
-                per_sm = std::max(per_sm, std::min(by_res, 2));
-            }
-            if (const char *ov = getenv("HB2_WALK_CTAS_PER_SM")) per_sm = atoi(ov);      // bring-up override
-            if (const char *ov = getenv("HB2_WALK_LANES")) p->walk_lane_cap = std::max(1, std::min(atoi(ov), 15));
-            p->walk_max_resident = std::min(per_sm, 2) * sms;
-            if (p->walk_max_resident < 1) {
-                fail("prune64_tc_walk_kernel (%d B of shared memory) cannot be resident on device %d", wk_smem, device);
-                hb2_destroy(p);
-                return 1;
-            }
-            const size_t T = Sp / hb2::TC_TILE_P;
-            p->walk_gen.assign((size_t)C * 2 * I, 0);   // matches the zero-filled conditional and exponent buffers
-            const size_t walk_ints = 16 + 2 * (size_t)(L + 2 * I) + (size_t)C * 2 * I;
-            { const char *ev = getenv("HB2_WALK_SPLIT_NODES"); p->walk_split_nodes = !(ev && ev[0] == '0'); }
-            CUP(cudaMalloc(&p->d_walk, walk_ints * sizeof(int)));
-            CUP(cudaMallocHost(&p->h_walk, walk_ints * sizeof(int)));
+        int per_sm = 0;
+        if (lane_ctas_per_sm("prune64_tc_walk_kernel", (const void *)hb2::prune64_tc_walk_kernel, 256, hb2::WALK_SMEM_BYTES, 2, device, per_sm)) {
+            hb2_destroy(p);
+            return 1;
         }
+        p->walk_max_resident = std::min(per_sm, 2) * p->sm_count;
+        if (p->walk_max_resident < 1) {
+            fail("prune64_tc_walk_kernel (%d B of shared memory) cannot be resident on device %d", hb2::WALK_SMEM_BYTES, device);
+            hb2_destroy(p);
+            return 1;
+        }
+        p->walk_gen.assign((size_t)C * 2 * I, 0);   // matches the zero-filled conditional and exponent buffers
+        const size_t walk_ints = 16 + 2 * (size_t)(L + 2 * I) + (size_t)C * 2 * I;
+        CUP(cudaMalloc(&p->d_walk, walk_ints * sizeof(int)));
+        CUP(cudaMallocHost(&p->h_walk, walk_ints * sizeof(int)));
     } else {
         CUP(cudaMalloc(&p->d_cond, (size_t)C * I * Sp * Dp * sizeof(double)));
         CUP(cudaMemsetAsync(p->d_cond, 0, (size_t)C * I * Sp * Dp * sizeof(double), p->stream));
@@ -1268,27 +1244,13 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
             const size_t walk_ints = 16 + 6 * (size_t)(L + 2 * I) + 4;       // planner's pairs + the kernel's int4 descriptors
             CUP(cudaMalloc(&p->d_walk, walk_ints * sizeof(int)));
             CUP(cudaMallocHost(&p->h_walk, walk_ints * sizeof(int)));
-            { const char *ev = getenv("HB2_WALK_SPLIT_NODES"); p->walk_split_nodes = !(ev && ev[0] == '0'); }
-            if (const char *ov = getenv("HB2_WALK_LANES")) p->walk_lane_cap = std::max(1, std::min(atoi(ov), 15));
-            int sms = 0;
-            CUP(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
-            cudaDeviceProp dp; CUP(cudaGetDeviceProperties(&dp, device));
-            const void *fn = (const void *)hb2::prune64_lanes_kernel;
-            const int threads = hb2::LANES_THREADS, smem = hb2::LANES_SMEM_BYTES;
-            CUP(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-            CUP(cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
             int per_sm = 0;
-            CUP(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, threads, smem));
-            // same resource arithmetic as for the tensor walk kernel (the occupancy API under-reports there)
-            cudaFuncAttributes fa;
-            CUP(cudaFuncGetAttributes(&fa, fn));
-            const int regs_per_cta = ((fa.numRegs + 7) / 8 * 8) * threads;
-            const size_t smem_per_cta = (size_t)smem + fa.sharedSizeBytes + dp.reservedSharedMemPerBlock;
-            const int by_res = std::min(dp.regsPerMultiprocessor / std::max(regs_per_cta, 1), (int)(dp.sharedMemPerMultiprocessor / smem_per_cta));
-            if (getenv("HB2_DEBUG")) fprintf(stderr, "[hb2] fp64 lanes kernel: occupancy API %d, by resources %d (regs %d)\n", per_sm, by_res, fa.numRegs);
-            per_sm = std::max(per_sm, std::min(by_res, hb2::LANES_CTAS_PER_SM));
-            if (const char *ov = getenv("HB2_WALK_CTAS_PER_SM")) per_sm = atoi(ov);
-            p->lanes_resident = std::max(per_sm, 1) * sms;
+            if (lane_ctas_per_sm("prune64_lanes_kernel", (const void *)hb2::prune64_lanes_kernel, hb2::LANES_THREADS, hb2::LANES_SMEM_BYTES,
+                                 hb2::LANES_CTAS_PER_SM, device, per_sm)) {
+                hb2_destroy(p);
+                return 1;
+            }
+            p->lanes_resident = std::max(per_sm, 1) * p->sm_count;
         }
     }
     CUP(cudaMalloc(&p->d_err, sizeof(int)));
@@ -1870,27 +1832,11 @@ int hb2_plan_walk(int64_t L, int64_t I, const int64_t *flatParents, int64_t nUpd
                   int splitNodes, int32_t *laneStart, int32_t *steps, int64_t stepCapacity, int64_t *nSteps) {
     if (!flatParents || !laneStart || !steps || !nSteps) return fail("null argument");
     if (L < 2 || I < 1 || lanes < 1 || lanes > 15) return fail("bad sizes L=%lld I=%lld lanes=%d", (long long)L, (long long)I, lanes);
-    std::vector<std::vector<int>> children(I);
-    for (int64_t n = 0; n < L + I - 1; n++) {
-        const int64_t par = flatParents[n];
-        if (par < 0 || par >= I || (n >= L && par <= n - L)) return fail("flatParents[%lld]=%lld: not a post-ordered tree", (long long)n, (long long)par);
-        children[par].push_back((int)n);
-    }
-    if (flatParents[L + I - 1] != -1) return fail("root must be the last node");
-    std::vector<int> height(I, 0);
-    for (int64_t i = 0; i < I; i++) {
-        if (children[i].empty()) return fail("internal node %lld has no children", (long long)i);
-        for (int ch : children[i]) if (ch >= L) height[i] = std::max(height[i], height[ch - L] + 1);
-    }
-    std::vector<char> dirty(I, 0);
-    if (!updateNodes || nUpdate < 0) std::fill(dirty.begin(), dirty.end(), 1);
-    else
-        for (int64_t k = 0; k < nUpdate; k++) {                       // same closure as hb2_evaluate: parents and ancestors
-            if (updateNodes[k] < 0 || updateNodes[k] >= L + I) return fail("updateNodes[%lld] out of range", (long long)k);
-            for (int64_t par = flatParents[updateNodes[k]]; par >= 0 && !dirty[par]; par = flatParents[L + par]) dirty[par] = 1;
-        }
-    int total = 0;
-    for (char d : dirty) total += d;
+    std::vector<std::vector<int>> children;
+    std::vector<int> height;
+    std::vector<char> dirty;
+    if (build_tree(flatParents, L, I, children, height) || dirty_nodes(flatParents, L, I, nUpdate, updateNodes, dirty)) return 1;
+    const int total = (int)std::count(dirty.begin(), dirty.end(), 1);
     if (total == 0) { *nSteps = 0; for (int r = 0; r <= lanes; r++) laneStart[r] = 0; return 0; }
     const int K = std::min(lanes, total);
     if (stepCapacity < L + 2 * I) return fail("steps needs room for %lld entries", (long long)(L + 2 * I));
@@ -2045,14 +1991,7 @@ int hb2_stage_launches(const hb2_partition *p, int64_t *out3) {
     for (int k = 0; k < 3; k++) out3[k] = p->stage_launches[k];
     return 0;
 }
-const char *hb2_pruning_kernel(const hb2_partition *p) {
-    if (!p) return "";
-    if (p->use_tc) return "prune64_tc_walk_kernel";
-    if (p->Dp == 64) return "prune64_lanes_kernel";
-    if (p->Dp >= 16) return "prune_small_dmma_kernel";
-    if (small_two_patterns(p, p->ownN)) return "prune_small_walk_ilp_kernel";
-    return "prune_small_walk_kernel";
-}
+const char *hb2_pruning_kernel(const hb2_partition *p) { return p ? PRUNE_KERNEL_NAME[pruning_kernel(p, p->ownN)] : ""; }
 
 int hb2_time_resident(hb2_partition *p, const double *weights, const double *rootFreqs, int iters, double *msPerEval,
                       double *stageMs, double *lnL) {
@@ -2088,8 +2027,8 @@ int hb2_time_resident(hb2_partition *p, const double *weights, const double *roo
     for (int c = 0; c < p->C; c++) hs[p->Dp + c] = weights[c];
     CU(cudaMemcpyAsync(p->d_pi, hs, p->Dp * sizeof(double), cudaMemcpyHostToDevice, p->stream));
     CU(cudaMemcpyAsync(p->d_weights, hs + p->Dp, p->C * sizeof(double), cudaMemcpyHostToDevice, p->stream));
-    std::vector<std::vector<int>> levels;
-    if (plan_levels(p, -1, nullptr, levels)) return 1;
+    std::vector<char> dirty;
+    if (dirty_nodes(p->parents.data(), p->L, p->I, -1, nullptr, dirty)) return 1;
     double tot = 0, st[3] = {0, 0, 0};
     for (int it = 0; it < iters; it++) {
         CU(cudaEventRecord(p->ev[0], p->stream));
@@ -2099,7 +2038,7 @@ int hb2_time_resident(hb2_partition *p, const double *weights, const double *roo
         } else if (launch_expm(p, p->d_Qres + (size_t)p->own0 * p->B * p->D * p->D, p->d_dst, (int)dst.size(), 0, nullptr, true, nullptr, &sp)) return 1;
         const int64_t l1 = p->launches;
         CU(cudaEventRecord(p->ev[1], p->stream));
-        if (run_pruning(p, p->own0, p->ownN, levels)) return 1;
+        if (run_pruning(p, p->own0, p->ownN, dirty)) return 1;
         CU(cudaEventRecord(p->ev[2], p->stream));
         const int64_t l2 = p->launches;
         if (run_root(p, p->own0, p->ownN, true, false)) return 1;

@@ -1,5 +1,5 @@
-"""CPU suite: the host-side planner of the tensor-core pruning pass (hb2_plan_walk, the very code hb2_evaluate runs before
-it launches prune64_tc_walk_kernel).  The kernel trusts the plan blindly -- a lane waits for another lane's tile only
+"""CPU suite: the host-side planner of the tensor-core pruning pass (hb2_plan_walk: the tree parser, dirty-node closure
+and planner that hb2_create and hb2_evaluate run before they launch prune64_tc_walk_kernel).  The kernel trusts the plan blindly -- a lane waits for another lane's tile only
 where the plan says WAIT, takes registers where it says CHAIN -- so the plan's invariants are checked here for many
 trees, lane counts and dirty sets, and each plan is executed by a small in-order-lane simulator to prove that its
 cross-lane waits cannot deadlock."""
@@ -208,3 +208,15 @@ def test_planner_rejects_bad_input():
     bad[L] = 0                                            # an internal node that is its own ancestor
     with pytest.raises(engine.EngineError):
         engine.plan_walk(bad, L, None, 2)
+    # the tree checks hb2_create makes: one root, and it is the last node; no internal node without children
+    I = len(par) - L
+    two_roots = par.copy()
+    two_roots[0] = -1                                     # a leaf without a parent
+    root_not_last = par.copy()
+    root_not_last[L + I - 2], root_not_last[L + I - 1] = -1, I - 2   # the root's last child takes its place
+    childless = par.copy()
+    childless[0] = childless[1] = 1                       # internal node 0 loses both its leaves
+    for tree, why in ((two_roots, "root must be the last node"), (root_not_last, "root must be the last node"),
+                      (childless, "internal node 0 has no children")):
+        with pytest.raises(engine.EngineError, match=why):
+            engine.plan_walk(tree, L, None, 2)
