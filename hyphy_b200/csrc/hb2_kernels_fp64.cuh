@@ -1096,6 +1096,77 @@ __global__ void __launch_bounds__(128, 6) prune_small_walk_ilp_kernel(PruneArgs 
 // partial[block] = sum over the block's patterns of freq*lnL_s (tree reduction, deterministic);
 // flag[0] |= 1 if any pattern with freq>0 has L <= 0.
 // ------------------------------------------------------------------------------------------------
+// x = m * 2^k with |m| in [0.5, 1) for finite x != 0, subnormals included (frexp without its out-pointer)
+__device__ __forceinline__ double split_pow2(double x, int &k) {
+    int adj = 0;
+    if (fabs(x) < 0x1p-1022) { x *= 0x1p64; adj = 64; }
+    const long long b = __double_as_longlong(x);
+    k = (int)((b >> 52) & 0x7ff) - 1022 - adj;
+    return __longlong_as_double((b & (long long)0x800fffffffffffffULL) | 0x3fe0000000000000LL);
+}
+
+// The rate-class merge of one pattern, shared by every site that forms such a sum (combine_kernel, the class-group partials
+// and the merge of those partials, DESIGN §4.5).  term(c, w, l, e) yields weight w, value l and binary exponent e of term c;
+// returns sum and sets emax with sum_c w_c l_c 2^(e_c) = sum * 2^emax.  A term of weight 0 takes no part at all (not in the
+// exponent, not in the sum, not in the NaN check), as likefunc2.cpp:668 skips such a class.  A NaN value of weight != 0, or
+// a NaN weight, gives NaN; no positive term gives sum 0, emax INT_MIN.
+// The fast rule aligns on the largest e_c and drops terms more than 1000 bits below it.  It can lose a term that matters
+// when the class holding the largest e_c has a tiny weight, so when a term is dropped or the sum falls below 2^-900 the
+// pattern is redone aligned on the contributions w_c l_c 2^(e_c) themselves (w and l split into mantissa and exponent, so
+// a subnormal weight does not underflow) and the sum goes out normalised to [0.5, 1) with its true exponent.  Unless a
+// class of positive weight sits more than 1000 bits below the highest or the sum falls below 2^-900, that path is not
+// taken and the arithmetic is the fast rule's, bit for bit.
+template <class Term>
+__device__ __forceinline__ double merge_classes(int n, Term term, int &emax_out) {
+    double w, l;
+    int e;
+    int emax = INT_MIN;
+    bool nan_seen = false;
+    for (int c = 0; c < n; c++) {
+        term(c, w, l, e);
+        if (w == 0.0) continue;
+        if (l != l || w != w) nan_seen = true;
+        if (l > 0.0) emax = max(emax, e);
+    }
+    double sum = 0.0;
+    bool cut = false;
+    for (int c = 0; c < n; c++) {
+        term(c, w, l, e);
+        if (w == 0.0 || !(l > 0.0)) continue;
+        const int de = e - emax;                                   // <= 0
+        if (de < -1000) cut = true;
+        else sum += w * l * exp2i(de);
+    }
+    if (nan_seen) {
+        sum = __longlong_as_double(0x7ff8000000000000LL);
+    } else if (emax != INT_MIN && (cut || sum < 0x1p-900)) {
+        int ebest = INT_MIN;
+        for (int c = 0; c < n; c++) {
+            term(c, w, l, e);
+            if (w == 0.0 || !(l > 0.0)) continue;
+            int kw, kl;
+            split_pow2(w, kw); split_pow2(l, kl);
+            ebest = max(ebest, e + kw + kl);
+        }
+        sum = 0.0;
+        for (int c = 0; c < n; c++) {
+            term(c, w, l, e);
+            if (w == 0.0 || !(l > 0.0)) continue;
+            int kw, kl;
+            const double m = split_pow2(w, kw) * split_pow2(l, kl);  // |m| in [0.25, 1)
+            const int de = e + kw + kl - ebest;
+            if (de >= -1000) sum += m * exp2i(de);
+        }
+        if (sum > 0.0) {
+            int k;
+            sum = split_pow2(sum, k);                                // [0.5, 1)
+            emax = ebest + k;
+        }
+    }
+    emax_out = emax;
+    return sum;
+}
+
 struct CombineArgs {
     const double *rootL; const int *rootE; const double *weights; const double *freq;
     double *partial; int *flag; double *siteL; long long *siteScale;
@@ -1109,23 +1180,12 @@ __global__ void __launch_bounds__(256) combine_kernel(CombineArgs a) {
     const int s = blockIdx.x * 256 + threadIdx.x;
     double term = 0.0;
     if (s < a.S) {
-        int emax = INT_MIN;
-        for (int c = 0; c < a.nc; c++) {
-            const double l = a.rootL[(size_t)(a.c0 + c) * a.Sp + s];
-            if (l > 0.0) emax = max(emax, a.rootE[(size_t)(a.c0 + c) * a.Sp + s]);
-        }
-        double sum = 0.0;
-        bool nan_seen = false;
-        for (int c = 0; c < a.nc; c++) {
-            const double l = a.rootL[(size_t)(a.c0 + c) * a.Sp + s];
-            const double w = a.weights ? a.weights[c] : 1.0;
-            if (l != l) nan_seen = true;
-            if (l > 0.0) {
-                const int de = a.rootE[(size_t)(a.c0 + c) * a.Sp + s] - emax;       // <= 0
-                sum += w * l * (de < -1000 ? 0.0 : exp2i(de));
-            }
-        }
-        if (nan_seen) sum = __longlong_as_double(0x7ff8000000000000LL);
+        int emax;
+        double sum = merge_classes(a.nc, [&](int c, double &w, double &l, int &e) {
+            w = a.weights ? a.weights[c] : 1.0;
+            l = a.rootL[(size_t)(a.c0 + c) * a.Sp + s];
+            e = a.rootE[(size_t)(a.c0 + c) * a.Sp + s];
+        }, emax);
         if (emax == INT_MIN) emax = 0;
         const double f = a.freq[s];
         double lnl;
@@ -1357,21 +1417,11 @@ __global__ void __launch_bounds__(256) class_partial_kernel(const double *rootL,
     double sum = 0.0;
     int emax = 0;
     if (s < S) {
-        emax = INT_MIN;
-        bool nan_seen = false;
-        for (int c = 0; c < nc; c++) {
-            const double l = rootL[(size_t)(c0 + c) * Sp + s];
-            if (l != l) nan_seen = true;
-            if (l > 0.0) emax = max(emax, rootE[(size_t)(c0 + c) * Sp + s]);
-        }
-        for (int c = 0; c < nc; c++) {
-            const double l = rootL[(size_t)(c0 + c) * Sp + s];
-            if (l > 0.0) {
-                const int de = rootE[(size_t)(c0 + c) * Sp + s] - emax;
-                sum += weights[c0 + c] * l * (de < -1000 ? 0.0 : exp2i(de));
-            }
-        }
-        if (nan_seen) sum = __longlong_as_double(0x7ff8000000000000LL);
+        sum = merge_classes(nc, [&](int c, double &w, double &l, int &e) {
+            w = weights[c0 + c];
+            l = rootL[(size_t)(c0 + c) * Sp + s];
+            e = rootE[(size_t)(c0 + c) * Sp + s];
+        }, emax);
         if (emax == INT_MIN) emax = 0;
     }
     send[s] = sum;
@@ -1391,24 +1441,11 @@ __global__ void __launch_bounds__(256) class_merge_kernel(const double *gath, co
     if (idx < nShards * xs) {
         const int j = idx / xs, s = idx % xs;
         const double f = xfreq[(size_t)j * G * xs + s];
-        int emax = INT_MIN;
-        bool nan_seen = false;
-        for (int r = 0; r < G; r++) {
+        int emax;
+        double sum = merge_classes(G, [&](int r, double &w, double &m, int &e) {
             const double *q = gath + (size_t)(j * G + r) * 2 * xs;
-            const double m = q[s];
-            if (m != m) nan_seen = true;
-            if (m > 0.0) emax = max(emax, (int)q[xs + s]);
-        }
-        double sum = 0.0;
-        for (int r = 0; r < G; r++) {
-            const double *q = gath + (size_t)(j * G + r) * 2 * xs;
-            const double m = q[s];
-            if (m > 0.0) {
-                const int de = (int)q[xs + s] - emax;
-                sum += m * (de < -1000 ? 0.0 : exp2i(de));
-            }
-        }
-        if (nan_seen) sum = __longlong_as_double(0x7ff8000000000000LL);
+            w = 1.0; m = q[s]; e = (int)q[xs + s];
+        }, emax);
         if (emax == INT_MIN) emax = 0;
         double lnl;
         if (sum > 0.0) lnl = log(sum) + (double)emax * 0.693147180559945309417232121458;
@@ -1631,21 +1668,11 @@ __global__ void __launch_bounds__(256) class_exchange_kernel(ClassXchgArgs a) {
         double sum = 0.0;
         int emax = 0;
         if (s < a.S) {
-            emax = INT_MIN;
-            bool nan_seen = false;
-            for (int c = 0; c < a.nc; c++) {
-                const double l = a.rootL[(size_t)(a.c0 + c) * a.Sp + s];
-                if (l != l) nan_seen = true;
-                if (l > 0.0) emax = max(emax, a.rootE[(size_t)(a.c0 + c) * a.Sp + s]);
-            }
-            for (int c = 0; c < a.nc; c++) {
-                const double l = a.rootL[(size_t)(a.c0 + c) * a.Sp + s];
-                if (l > 0.0) {
-                    const int de = a.rootE[(size_t)(a.c0 + c) * a.Sp + s] - emax;
-                    sum += a.weights[a.c0 + c] * l * (de < -1000 ? 0.0 : exp2i(de));
-                }
-            }
-            if (nan_seen) sum = __longlong_as_double(0x7ff8000000000000LL);
+            sum = merge_classes(a.nc, [&](int c, double &w, double &l, int &e) {
+                w = a.weights[a.c0 + c];
+                l = a.rootL[(size_t)(a.c0 + c) * a.Sp + s];
+                e = a.rootE[(size_t)(a.c0 + c) * a.Sp + s];
+            }, emax);
             if (emax == INT_MIN) emax = 0;
         }
         for (int r = 0; r < b.R; r++) {
@@ -1668,24 +1695,11 @@ __global__ void __launch_bounds__(256) class_exchange_kernel(ClassXchgArgs a) {
     for (int idx = tid; idx < a.nShards * xs; idx += 256) {
         const int j = idx / xs, s = idx - j * xs;
         const double f = a.xfreq[(size_t)j * a.G * xs + s];
-        int emax = INT_MIN;
-        bool nan_seen = false;
-        for (int r = 0; r < a.G; r++) {
+        int emax;
+        double sum = merge_classes(a.G, [&](int r, double &w, double &m, int &e) {
             const double *q = peer_data(b, b.rank, j * a.G + r);
-            const double m = __ldcg(q + s);
-            if (m != m) nan_seen = true;
-            if (m > 0.0) emax = max(emax, (int)__ldcg(q + xs + s));
-        }
-        double sum = 0.0;
-        for (int r = 0; r < a.G; r++) {
-            const double *q = peer_data(b, b.rank, j * a.G + r);
-            const double m = __ldcg(q + s);
-            if (m > 0.0) {
-                const int de = (int)__ldcg(q + xs + s) - emax;
-                sum += m * (de < -1000 ? 0.0 : exp2i(de));
-            }
-        }
-        if (nan_seen) sum = __longlong_as_double(0x7ff8000000000000LL);
+            w = 1.0; m = __ldcg(q + s); e = (int)__ldcg(q + xs + s);
+        }, emax);
         if (emax == INT_MIN) emax = 0;
         double lnl;
         if (sum > 0.0) lnl = log(sum) + (double)emax * 0.693147180559945309417232121458;

@@ -123,7 +123,9 @@ int hb2_evaluate_forced(hb2_partition *p, int64_t cat, int64_t nUpdate, const in
 
 /* Fused replacement for the whole category loop PopulateConditionalProbabilities(WeightedSum) +
  * SumUpSiteLikelihoods (likefunc2.cpp:484-908, 1446-1506): all C classes pruned in one pass,
- * L_s = sum_c weights[c]*L_{c,s} combined on device, one lnL comes back.  Same outputs as hb2_evaluate. */
+ * L_s = sum_c weights[c]*L_{c,s} combined on device, one lnL comes back.  Same outputs as hb2_evaluate.  A class of
+ * weight 0 is ignored, as likefunc2.cpp:668 (its likelihoods, NaN included, do not reach the sum); a tiny or subnormal
+ * weight on a class far above the others does not hide them.  Negative weights are not supported. */
 int hb2_evaluate_classes(hb2_partition *p, const double *weights, int64_t nUpdate, const int64_t *updateNodes,
                          const double *rootFreqs, double *lnL, double *siteL, int64_t *siteScale);
 

@@ -12,6 +12,45 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 
+ZERO_WEIGHT_CASE = "class_groups_zero_weight"
+
+
+def zero_weight_class_groups(world, rank, local, dist):
+    """Two class groups, weights (0, 1): group 0 holds an identity class more than 1000 bits above group 1's uniform-row
+    class on every pattern.  The weight-0 class takes no part, so lnL is class 1's alone, D^-leaves per pattern.
+    Tolerances as on one GPU (class_merge_cases.tolerances: the tensor path's per-pattern bound grows with the tree)."""
+    import math
+    from hyphy_b200 import LikelihoodFunction, Partition, engine
+    from hyphy_b200.sharding import shard_bounds, exchange_unique_id
+    from tests import class_merge_cases as cm
+    name = "d61_identity_uniform"
+    D, n_leaves = cm.GAP_CASES[name][:2]
+    w, P = cm.gap_case(name, weights=(0.0, 1.0))
+    shards = world // 2
+    lo, hi = shard_bounds(w.S, shards, rank // 2)
+    want_site = -n_leaves * math.log(D)
+    want = float(w.pattern_freq.sum()) * want_site
+    out = []
+    for flags, mode in ((engine.FLAG_FORCE_FP64, "fp64"), (engine.FLAG_DEFAULT, "tc")):
+        rtol, atol = cm.tolerances(w, mode)
+        lf = LikelihoodFunction(w, device=local, flags=flags, pattern_slice=slice(lo, hi))
+        lf.part.comm_init(world, rank, exchange_unique_id(dist, rank, Partition.comm_unique_id))
+        lf.part.comm_class_groups(2)
+        for c in range(w.C):
+            lf.part.set_matrices(c, lf.all_nodes, P[c], engine.MATRIX_TRANS)
+        lnl, sl, ss = lf.compute(want_sites=True)
+        lf.close()
+        err = float(np.abs(np.log(sl) - 64.0 * np.log(2.0) * ss - want_site).max())
+        ok = math.isfinite(lnl) and abs(lnl - want) <= rtol * abs(want) and err <= atol
+        rec = {"mode": mode, "groups": 2, "shards": shards, "weights": [0.0, 1.0], "lnL": lnl, "want": want,
+               "site_err": err, "site_atol": atol, "ok": bool(ok)}
+        oks = [None] * world
+        dist.all_gather_object(oks, rec["ok"])
+        rec["ok_all_ranks"] = all(oks)
+        out.append(rec)
+    return out
+
+
 def main():
     import torch
     import torch.distributed as dist
@@ -23,6 +62,13 @@ def main():
     rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
     torch.cuda.set_device(local)
     dist.init_process_group("gloo")
+    if name == ZERO_WEIGHT_CASE:
+        out = {"case": name, "world": world, "layouts": zero_weight_class_groups(world, rank, local, dist)}
+        if rank == 0:
+            print("MULTIGPU " + json.dumps(out), flush=True)
+        dist.barrier()
+        dist.destroy_process_group()
+        sys.exit(0 if all(r["ok_all_ranks"] for r in out["layouts"]) else 1)
     w, g = gc.load(name)
     pat_golden = np.empty(w.S)
     pat_golden[w.site_to_pattern] = g["site_lnL"]

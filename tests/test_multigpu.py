@@ -19,8 +19,7 @@ def _world():
     return 8 if n >= 8 else 4 if n >= 4 else 2 if n >= 2 else 0
 
 
-@pytest.mark.parametrize("name", ["mg94_30x100_c4_ambig", "mg94_200x64_c4_scaling", "ns_mg94_200x2000_c4"])
-def test_sharded_layouts_match_reference_golden(name, engine_lib):
+def _run_worker(name):
     world = _world()
     if world < 2:
         pytest.skip("needs at least 2 GPUs")
@@ -36,3 +35,13 @@ def test_sharded_layouts_match_reference_golden(name, engine_lib):
         f.write(json.dumps(res) + "\n")
     assert pr.returncode == 0, res
     assert all(r["ok_all_ranks"] for r in res["layouts"]), res
+
+
+@pytest.mark.parametrize("name", ["mg94_30x100_c4_ambig", "mg94_200x64_c4_scaling", "ns_mg94_200x2000_c4"])
+def test_sharded_layouts_match_reference_golden(name, engine_lib):
+    _run_worker(name)
+
+
+def test_class_groups_ignore_zero_weight_class(engine_lib):
+    """Two class groups, the group of the highest class with weight 0: the other group's classes must not be flushed."""
+    _run_worker("class_groups_zero_weight")
