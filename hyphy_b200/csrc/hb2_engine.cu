@@ -19,8 +19,10 @@
 #include <string>
 #include <vector>
 #include <algorithm>
+#include <memory>
 #include <mutex>
 #include <unordered_map>
+#include <utility>
 
 #include <nccl.h>
 
@@ -62,7 +64,7 @@ struct BlockPool {
     static size_t size_class(size_t n) { size_t c = 256; while (c < n) c <<= 1; return c; }
     static unsigned long long key(bool host, int dev, size_t cls) { return ((unsigned long long)host << 63) | ((unsigned long long)(dev & 0xff) << 52) | (unsigned long long)cls; }
     cudaError_t alloc(void **p, size_t n, bool host) {
-        if (!enabled() || n > kMaxClass) return host ? (cudaMallocHost)(p, n) : (cudaMalloc)(p, n);
+        if (!enabled() || n > kMaxClass) return host ? cudaMallocHost(p, n) : cudaMalloc(p, n);
         int dev = 0;
         cudaGetDevice(&dev);
         const size_t cls = size_class(n);
@@ -77,7 +79,7 @@ struct BlockPool {
                 return cudaSuccess;
             }
         }
-        const cudaError_t e = host ? (cudaMallocHost)(p, cls) : (cudaMalloc)(p, cls);
+        const cudaError_t e = host ? cudaMallocHost(p, cls) : cudaMalloc(p, cls);
         if (e == cudaSuccess) { std::lock_guard<std::mutex> lk(mu); live[*p] = Info{cls, dev, host}; }
         return e;
     }
@@ -97,16 +99,46 @@ struct BlockPool {
                 }
             }
         }
-        return host ? (cudaFreeHost)(p) : (cudaFree)(p);
+        return host ? cudaFreeHost(p) : cudaFree(p);
     }
 };
 BlockPool g_pool;
-// every allocation of this file goes through the pool (buffers that are exported through CUDA IPC opt out with the
-// parenthesised runtime name)
-#define cudaMalloc(p, n) g_pool.alloc((void **)(p), (n), false)
-#define cudaMallocHost(p, n) g_pool.alloc((void **)(p), (n), true)
-#define cudaFree(p) g_pool.release((void *)(p), false)
-#define cudaFreeHost(p) g_pool.release((void *)(p), true)
+
+// Owner of one pool block of n elements of T: device memory, or pinned host memory when Pinned.  Every block of this file
+// is held by one, except the peer-exchange buffer, which is exported through CUDA IPC and never pooled.  alloc() and the
+// destructor return the block held so far to the pool, which may hand it out again at once: no work queued on any stream
+// may still use it by then.
+template <typename T, bool Pinned>
+class PoolBuffer {
+    T *ptr_ = nullptr;
+    size_t n_ = 0;
+public:
+    PoolBuffer() = default;
+    PoolBuffer(PoolBuffer &&o) noexcept : ptr_(std::exchange(o.ptr_, nullptr)), n_(std::exchange(o.n_, 0)) {}
+    PoolBuffer &operator=(PoolBuffer &&o) noexcept {
+        if (this != &o) { g_pool.release(ptr_, Pinned); ptr_ = std::exchange(o.ptr_, nullptr); n_ = std::exchange(o.n_, 0); }
+        return *this;
+    }
+    ~PoolBuffer() { g_pool.release(ptr_, Pinned); }
+    // On failure the owner is left empty.
+    int alloc(size_t n) {
+        g_pool.release(ptr_, Pinned);
+        ptr_ = nullptr; n_ = 0;
+        void *q = nullptr;
+        const cudaError_t e = g_pool.alloc(&q, n * sizeof(T), Pinned);
+        if (e != cudaSuccess) return fail("allocating %zu bytes of %s memory failed: %s", n * sizeof(T), Pinned ? "pinned" : "device", cudaGetErrorString(e));
+        ptr_ = static_cast<T *>(q); n_ = n;
+        return 0;
+    }
+    // Clears all n elements on `stream` (device buffers).
+    int zero(cudaStream_t stream) {
+        CU(cudaMemsetAsync(ptr_, 0, n_ * sizeof(T), stream));
+        return 0;
+    }
+    operator T *() const { return ptr_; }
+};
+template <typename T> using DeviceBuffer = PoolBuffer<T, false>;
+template <typename T> using PinnedBuffer = PoolBuffer<T, true>;
 
 // ---- NCCL through dlopen: single-GPU users never need the library -------------------------------
 struct NcclApi {
@@ -157,14 +189,12 @@ struct hb2_partition {
     std::vector<std::vector<int>> children;   // per internal node, flat ids
     std::vector<int> height;                  // per internal node: 0 = only leaf children
     // device
-    int *d_leaf = nullptr, *d_scal = nullptr, *d_rootE = nullptr, *d_child_start = nullptr, *d_child_ids = nullptr;
-    int *d_jobs = nullptr, *d_dst = nullptr, *d_flag = nullptr;
-    double *d_ambig = nullptr, *d_freq = nullptr, *d_cond = nullptr, *d_PT = nullptr, *d_Q = nullptr, *d_pi = nullptr;
-    double *d_rootL = nullptr, *d_weights = nullptr, *d_partial = nullptr, *d_lnL = nullptr, *d_siteL = nullptr;
-    long long *d_siteScale = nullptr;
+    DeviceBuffer<int> d_leaf, d_scal, d_rootE, d_child_start, d_child_ids, d_jobs, d_dst, d_flag;
+    DeviceBuffer<double> d_ambig, d_freq, d_cond, d_PT, d_Q, d_pi, d_rootL, d_weights, d_partial, d_lnL, d_siteL;
+    DeviceBuffer<long long> d_siteScale;
     // pinned host staging
-    double *h_Q = nullptr, *h_small = nullptr;   // h_small: pi (Dp) + weights (C) + lnL (1)
-    int *h_jobs = nullptr, *h_dst = nullptr;
+    PinnedBuffer<double> h_Q, h_small;        // h_small: pi (Dp) + weights (C) + lnL (1)
+    PinnedBuffer<int> h_jobs, h_dst;
     // pending matrices: entries [0, n_pending) of h_Q / h_dst, with kinds
     int64_t n_pending = 0;
     std::vector<int> pending_kind;
@@ -176,10 +206,11 @@ struct hb2_partition {
     int64_t q_capacity = 0;                   // in matrices
     std::vector<char> have_matrix;            // [C*B]
     std::vector<char> is_rate;                // [C*B] slot holds a rate matrix resident in d_Qres (for hb2_time_resident)
-    double *d_Qres = nullptr;                 // [C][B][D*D] last rate matrices, resident copy
+    DeviceBuffer<double> d_Qres;              // [C][B][D*D] last rate matrices, resident copy
     // explicit-form mixtures (hb2_set_mixture_matrices): own staging so that nothing is shared with the plain queues
-    double *d_mix_scratch = nullptr, *d_mix_Q = nullptr, *h_mix = nullptr;   // [cap][Dp*Dp], [cap][D*D], pinned [cap][D*D + 1]
-    int *d_mix_dst = nullptr;
+    DeviceBuffer<double> d_mix_scratch, d_mix_Q;   // [cap][Dp*Dp], [cap][D*D] | [cap] weights
+    PinnedBuffer<double> h_mix;                    // as d_mix_Q, then 2 cap ints
+    DeviceBuffer<int> d_mix_dst;
     int64_t mix_capacity = 0;
     cudaEvent_t ev_mix = nullptr;
     bool mix_busy = false;
@@ -187,21 +218,33 @@ struct hb2_partition {
     // C + mixture component; per-entry arrays are indexed like the batch
     struct ExBuf {
         int G = 0, stride = 0;                // groups, doubles per cached reference direction
-        int *d_int = nullptr, *h_int = nullptr, *d_flag = nullptr;     // [group cap | ref cap | refs G]
-        double *d_weight = nullptr, *d_pow = nullptr, *d_refvec = nullptr, *d_colsum = nullptr;   // colsum [cap][16][64]
-        void *d_groups = nullptr;
-        unsigned long long *d_flags = nullptr, gen = 0;   // generation flags of the coefficient matrices [G][EXPM_POW_TERMS]
+        DeviceBuffer<int> d_int, d_flag;      // d_int: [group cap | ref cap | refs G]
+        PinnedBuffer<int> h_int;
+        DeviceBuffer<double> d_weight, d_pow, d_refvec, d_colsum;   // colsum [cap][16][64]
+        DeviceBuffer<hb2::ExpmGroup> d_groups;
+        DeviceBuffer<unsigned long long> d_flags;   // generation flags of the coefficient matrices [G][EXPM_POW_TERMS]
+        unsigned long long gen = 0;
         std::vector<int> kind;                // host mirror: kind of the reference direction each group holds (0 none)
         int64_t cap = 0;
+        // (Re)allocates the buffers for G_ groups and cap_ entries, with no cached direction.
+        int alloc(int G_, int64_t cap_, cudaStream_t stream) {
+            G = G_; cap = cap_; stride = 4096; gen = 0;
+            kind.assign(G, 0);
+            return d_int.alloc(2 * cap + G) || h_int.alloc(2 * cap + G) || d_flag.alloc(cap) || d_weight.alloc(cap) ||
+                   d_colsum.alloc(cap * 16 * 64) || d_groups.alloc(G) || d_groups.zero(stream) ||
+                   d_pow.alloc((size_t)G * hb2::EXPM_POW_TERMS * 4096) || d_flags.alloc((size_t)G * hb2::EXPM_POW_TERMS) ||
+                   d_flags.zero(stream) || d_refvec.alloc((size_t)G * stride);
+        }
     };
     ExBuf ex;                                 // the partition's own hand-overs
     ExBuf bex;                                // batched one-pattern likelihoods (hb2_batch_site_likelihoods): one group per set
     int64_t b_cap = 0;                        // sets per chunk of the batch buffers below
     int64_t b_vcap = 0;                       // formula values d_bV holds
-    double *d_bPT = nullptr, *d_bV = nullptr, *d_bcond = nullptr, *d_bout = nullptr;
-    double *d_bmixw = nullptr;                // mixture weights of a chunk [sets][rows]
-    int *d_bdst = nullptr, *d_bpat = nullptr, *d_bnodeex = nullptr, *h_bdst = nullptr;
-    int *d_brow = nullptr;                    // first component row of each branch [B+1]
+    DeviceBuffer<double> d_bPT, d_bV, d_bcond, d_bout;
+    DeviceBuffer<double> d_bmixw;             // mixture weights of a chunk [sets][rows]
+    DeviceBuffer<int> d_bdst, d_bpat, d_bnodeex;
+    PinnedBuffer<int> h_bdst;
+    DeviceBuffer<int> d_brow;                 // first component row of each branch [B+1]
     int b_groups_per_set = 1;
     bool ex_enabled = true;                   // HB2_EXPM_SHARED=0 switches the path off (A/B testing)
     int64_t stage_launches[3] = {0, 0, 0};    // launches per evaluation of the last hb2_time_resident {expm, pruning, root}
@@ -211,28 +254,31 @@ struct hb2_partition {
     struct Tmpl {
         int64_t nnz = 0, nF = 0, n_pending = 0;
         bool has_colfreq = false;
-        int *d_index = nullptr, *d_formula = nullptr, *d_vdst = nullptr, *h_vdst = nullptr;
-        double *d_colfreq = nullptr, *h_colfreq = nullptr, *d_V = nullptr, *h_V = nullptr, *d_Vres = nullptr;
+        DeviceBuffer<int> d_index, d_formula, d_vdst;
+        PinnedBuffer<int> h_vdst;
+        DeviceBuffer<double> d_colfreq, d_V, d_Vres;
+        PinnedBuffer<double> h_colfreq, h_V;
     };
     std::vector<Tmpl> tmpls;
     std::vector<signed char> pend_tmpl;       // [C*B] template of the slot's pending compiled entry
     std::vector<signed char> res_tmpl;        // [C*B] template of the slot's resident formula values (is_rate == 2)
     // tensor-core path (33..64 states unless HB2_FLAG_FORCE_FP64): fp32 conditionals + split/tiled P operands
     bool use_tc = false;
-    float *d_condf = nullptr, *d_PB = nullptr, *d_PTf = nullptr;
-    int *d_err = nullptr;
-    unsigned *d_root_counter = nullptr;       // ticket counter of the fused root reduction (combine_kernel's last block)
-    int *d_forced = nullptr, *h_forced = nullptr;   // forced states of the current evaluation (hb2_evaluate_forced)
+    DeviceBuffer<float> d_condf, d_PB, d_PTf;
+    DeviceBuffer<int> d_err;
+    DeviceBuffer<unsigned> d_root_counter;    // ticket counter of the fused root reduction (combine_kernel's last block)
+    DeviceBuffer<int> d_forced;               // forced states of the current evaluation (hb2_evaluate_forced)
+    PinnedBuffer<int> h_forced;
     int forced_node = -1;
     // persistent walk kernel (one launch per evaluation): plan buffers, generation bits of the tagged hand-over, residency
     int small_ilp = 0, small_resident[2] = {1, 1};   // HB2_SMALL_ILP=1/2 forces one / two patterns per thread (4 states); co-resident CTAs of both
-    double *d_cond_side = nullptr;            // fp64 lanes kernel: side products [C][I][Sp][64] (exponents: second half of d_scal)
-    int *d_lane_flags = nullptr;              // [C][2I][Sp/64] pass id of the last production
+    DeviceBuffer<double> d_cond_side;         // fp64 lanes kernel: side products [C][I][Sp][64] (exponents: second half of d_scal)
+    DeviceBuffer<int> d_lane_flags;           // [C][2I][Sp/64] pass id of the last production
     int lane_pass = 0, lanes_resident = 0;    // co-resident CTAs of prune64_lanes_kernel
     int sm_count = 132;
     int walk_max_resident = 0;
     // single-branch shortcut (hb2_branch_cache_*): outside vectors of one branch, all owned classes
-    double *d_bc_out = nullptr; int *d_bc_outE = nullptr, *d_bc_sib = nullptr; int64_t bc_node = -1;
+    DeviceBuffer<double> d_bc_out; DeviceBuffer<int> d_bc_outE, d_bc_sib; int64_t bc_node = -1;
     int64_t bc_dirty_node = -1;               // first node other than bc_node whose matrix changed since the build
     std::vector<char> plan_jdirty;      // dirty jobs (nodes + side products) of the cached plan
     bool walk_split_nodes = true;       // HB2_WALK_SPLIT_NODES=0: no side products (A/B)
@@ -240,7 +286,8 @@ struct hb2_partition {
     int plan_K = 0, plan_steps = 0;
     std::vector<int> walk_gen;          // [C][I] generation bit of each node's resident conditionals (tc walk path)
     bool walk_reset = false;            // a pass was aborted: tags are inconsistent -> wipe and recompute everything
-    int *d_walk = nullptr, *h_walk = nullptr;
+    DeviceBuffer<int> d_walk;
+    PinnedBuffer<int> h_walk;
     int walk_lane_cap = 8;              // lanes (CTAs) that share one (class, tile) pair; HB2_WALK_LANES overrides (<= 15)
     bool first_eval_done = false;
     std::vector<char> evaluated_cat;          // [C] whole tree pruned at least once
@@ -249,17 +296,17 @@ struct hb2_partition {
     int n_ranks = 1, rank = 0;
     // class groups (hb2_comm_class_groups): this rank prunes classes [own0, own0 + ownN) only
     int cg_G = 1, cg_g = 0, own0 = 0, ownN = 0, xchg_len = 0;
-    double *d_xsend = nullptr, *d_xrecv = nullptr, *d_xfreq = nullptr, *d_xpartial = nullptr;
+    DeviceBuffer<double> d_xsend, d_xrecv, d_xfreq, d_xpartial;
     int n_partial_blocks = 0;
     // peer exchange (hb2_kernels_fp64.cuh "Peer exchange"): IPC-mapped buffers of all ranks; falls back to NCCL when the
     // mapping cannot be established (px_ok false)
     bool px_ok = false, px_enabled = true;
     int px_payload = 0;
     unsigned long long px_gen = 0;
-    double *px_local = nullptr;
+    double *px_local = nullptr;               // exported through CUDA IPC: a plain runtime allocation
     std::vector<double *> px_peer;            // host copy of the mapped pointers (entry rank = px_local)
-    double **d_px_peer = nullptr;
-    unsigned int *d_px_counter = nullptr;
+    DeviceBuffer<double *> d_px_peer;
+    DeviceBuffer<unsigned> d_px_counter;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
     cudaEvent_t ev_staging = nullptr;
     bool staging_busy = false;
@@ -326,7 +373,7 @@ int void_template_cache(hb2_partition *p, int tmpl) {
     for (int c = 0; p->ex.d_groups && c < (int)p->C; c++) {
         const int g = tmpl * (int)p->C + c;
         if (g >= p->ex.G) break;
-        CU(cudaMemsetAsync(static_cast<hb2::ExpmGroup *>(p->ex.d_groups) + g, 0, sizeof(hb2::ExpmGroup), p->stream));
+        CU(cudaMemsetAsync(p->ex.d_groups + g, 0, sizeof(hb2::ExpmGroup), p->stream));
         p->ex.kind[g] = 0;
     }
     for (size_t k = 0; k < p->is_rate.size(); k++) if (p->is_rate[k] == 2 && p->res_tmpl[k] == tmpl) p->is_rate[k] = 0;
@@ -346,7 +393,7 @@ int launch_expm(hb2_partition *p, const double *dQ, const int *d_dst, int n, int
     if (is_trans == 2) {                       // compiled template: dQ points at the formula values [n][nF]
         const hb2_partition::Tmpl &t = p->tmpls[tmpl];
         a.is_trans = 0; a.Q = nullptr; a.V = dQ; a.tmpl_index = t.d_index; a.tmpl_formula = t.d_formula;
-        a.tmpl_colfreq = t.has_colfreq ? t.d_colfreq : nullptr; a.tmpl_nnz = (int)t.nnz; a.nF = (int)t.nF;
+        a.tmpl_colfreq = t.has_colfreq ? t.d_colfreq : (double *)nullptr; a.tmpl_nnz = (int)t.nnz; a.nF = (int)t.nF;
     }
     pack_tc = pack_tc && p->use_tc && !pt_override;
     switch (p->Dp) {
@@ -357,7 +404,7 @@ int launch_expm(hb2_partition *p, const double *dQ, const int *d_dst, int n, int
             if (sp && sp->use && is_trans != 1) {
                 hb2_partition::ExBuf &x = *sp->x;
                 const int nV = sp->kind == 1 ? (int)p->tmpls[tmpl].nF : (int)(p->D * p->D);
-                const hb2::ExpmGroup *groups = static_cast<const hb2::ExpmGroup *>(x.d_groups);
+                const hb2::ExpmGroup *groups = x.d_groups;
                 hb2::ExpmClassifyArgs ca{};
                 ca.V = dQ; ca.nV = nV; ca.kind = sp->kind; ca.dst = d_dst; ca.group = x.d_int + off;
                 ca.ref = x.d_int + x.cap + off; ca.groups = groups; ca.refvec = x.d_refvec; ca.refvec_stride = x.stride;
@@ -371,7 +418,7 @@ int launch_expm(hb2_partition *p, const double *dQ, const int *d_dst, int n, int
                 a.Qres = nullptr;                    // the classification stage keeps the resident copy
                 if (sp->n_refs > 0) {
                     hb2::ExpmPowersArgs pa{};
-                    pa.a = a; pa.refs = x.d_int + 2 * x.cap; pa.groups = static_cast<hb2::ExpmGroup *>(x.d_groups);
+                    pa.a = a; pa.refs = x.d_int + 2 * x.cap; pa.groups = x.d_groups;
                     pa.pow = x.d_pow; pa.refvec = x.d_refvec; pa.refvec_stride = x.stride; pa.nV = nV; pa.kind = sp->kind; pa.Vin = dQ;
                     pa.flags = x.d_flags; pa.gen = ++x.gen; pa.err = p->d_err;
                     hb2::expm_powers_kernel<<<dim3(hb2::EXPM_POW_TERMS - 1, (unsigned)sp->n_refs), 256, smem, p->stream>>>(pa);
@@ -410,7 +457,7 @@ int flush_compiled(hb2_partition *p) {
         if (plan_shared(p, t.h_vdst, n, 1, nullptr, sp, (int)ti)) return 1;
         CU(cudaEventRecord(p->ev_staging, p->stream));
         p->staging_busy = true;
-        if (launch_expm(p, t.d_V, t.d_vdst, (int)n, 2, sp.use ? nullptr : p->d_Qres, true, nullptr, &sp, 0, (int)ti)) return 1;
+        if (launch_expm(p, t.d_V, t.d_vdst, (int)n, 2, sp.use ? nullptr : (double *)p->d_Qres, true, nullptr, &sp, 0, (int)ti)) return 1;
         for (int64_t k = 0; k < n; k++)
             if (t.h_vdst[k] >= 0) { p->is_rate[t.h_vdst[k]] = sp.use ? 2 : 1; p->res_tmpl[t.h_vdst[k]] = (signed char)ti; p->pend_pos[t.h_vdst[k]] = -1; }
         t.n_pending = 0;
@@ -441,7 +488,7 @@ int flush_matrices(hb2_partition *p) {
         int64_t j = i;
         while (j < n && p->pending_kind[j] == p->pending_kind[i]) j++;
         const int is_trans = p->pending_kind[i] == HB2_MATRIX_TRANS;
-        if (launch_expm(p, p->d_Q + i * dd, p->d_dst + i, (int)(j - i), is_trans, is_trans ? nullptr : p->d_Qres, true, nullptr, &sp, i)) return 1;
+        if (launch_expm(p, p->d_Q + i * dd, p->d_dst + i, (int)(j - i), is_trans, is_trans ? nullptr : (double *)p->d_Qres, true, nullptr, &sp, i)) return 1;
         i = j;
     }
     for (int64_t k = 0; k < n; k++)
@@ -698,18 +745,15 @@ int cached_plan(hb2_partition *p, const std::vector<char> &dirty, int K, bool ca
 struct WalkTrace {
     const char *path = getenv("HB2_WALK_TRACE");
     int cta = 0, ns = 0, ctas = 0;
-    long long *d = nullptr;
+    DeviceBuffer<long long> d;
     size_t n = 0;
-    ~WalkTrace() { if (d) cudaFree(d); }
     // Stamps of a pass of ns steps; ctas = CTAs that stamp their residence (0: none).  d stays null without a trace.
     int alloc(hb2_partition *p, int ns_, int ctas_) {
         if (!path) return 0;
         if (const char *tc = getenv("HB2_WALK_TRACE_CTA")) cta = atoi(tc);
         ns = ns_; ctas = ctas_;
         n = (size_t)(ns + 1) * 12 + (size_t)ctas * 4;
-        CU(cudaMalloc(&d, n * sizeof(long long)));
-        CU(cudaMemsetAsync(d, 0, n * sizeof(long long), p->stream));
-        return 0;
+        return d.alloc(n) || d.zero(p->stream);
     }
     // kernel: header prefix naming the kernel; columns: names of the 12 stamps of a step
     int write(hb2_partition *p, const char *kernel, const char *columns, int K) {
@@ -916,10 +960,8 @@ void peer_teardown(hb2_partition *p) {
     for (size_t r = 0; r < p->px_peer.size(); r++)
         if ((int)r != p->rank && p->px_peer[r]) cudaIpcCloseMemHandle(p->px_peer[r]);
     p->px_peer.clear();
-    if (p->px_local) (cudaFree)(p->px_local);                 // IPC-exported: never pooled
-    if (p->d_px_peer) cudaFree(p->d_px_peer);
-    if (p->d_px_counter) cudaFree(p->d_px_counter);
-    p->px_local = nullptr; p->d_px_peer = nullptr; p->d_px_counter = nullptr; p->px_ok = false;
+    if (p->px_local) cudaFree(p->px_local);
+    p->px_local = nullptr; p->d_px_peer = {}; p->d_px_counter = {}; p->px_ok = false;
 }
 
 int peer_setup(hb2_partition *p, int payload) {
@@ -931,7 +973,7 @@ int peer_setup(hb2_partition *p, int payload) {
     int ok = p->px_enabled ? 1 : 0;
     cudaIpcMemHandle_t mine;
     memset(&mine, 0, sizeof mine);
-    if (ok && (cudaMalloc)((void **)&p->px_local, doubles * sizeof(double)) != cudaSuccess) { cudaGetLastError(); p->px_local = nullptr; ok = 0; }
+    if (ok && cudaMalloc(&p->px_local, doubles * sizeof(double)) != cudaSuccess) { cudaGetLastError(); p->px_local = nullptr; ok = 0; }
     if (ok) {
         CU(cudaMemsetAsync(p->px_local, 0, doubles * sizeof(double), p->stream));
         if (cudaIpcGetMemHandle(&mine, p->px_local) != cudaSuccess) { cudaGetLastError(); ok = 0; }
@@ -941,15 +983,13 @@ int peer_setup(hb2_partition *p, int payload) {
     std::vector<unsigned char> sendrec(rec, 0), all(rec * R, 0);
     memcpy(sendrec.data(), &ok, sizeof(int));
     memcpy(sendrec.data() + 8, &mine, sizeof mine);
-    unsigned char *d_send = nullptr, *d_all = nullptr;
-    CU(cudaMalloc(&d_send, rec));
-    CU(cudaMalloc(&d_all, rec * R));
+    DeviceBuffer<unsigned char> d_send, d_all;
+    if (d_send.alloc(rec) || d_all.alloc(rec * R)) return 1;
     CU(cudaMemcpyAsync(d_send, sendrec.data(), rec, cudaMemcpyHostToDevice, p->stream));
     ncclResult_t nr = g_nccl.AllGather(d_send, d_all, rec, ncclChar, p->comm, p->stream);
-    if (nr != ncclSuccess) { cudaFree(d_send); cudaFree(d_all); return fail("ncclAllGather (IPC handles): %s", g_nccl.GetErrorString(nr)); }
+    if (nr != ncclSuccess) return fail("ncclAllGather (IPC handles): %s", g_nccl.GetErrorString(nr));
     CU(cudaMemcpyAsync(all.data(), d_all, rec * R, cudaMemcpyDeviceToHost, p->stream));
     CU(cudaStreamSynchronize(p->stream));
-    cudaFree(d_send); cudaFree(d_all);
     int all_ok = 1;
     for (int r = 0; r < R; r++) { int o; memcpy(&o, all.data() + rec * r, sizeof(int)); all_ok = all_ok && o; }
     p->px_peer.assign(R, nullptr);
@@ -964,25 +1004,23 @@ int peer_setup(hb2_partition *p, int payload) {
         }
     }
     // the mapping must have worked on EVERY rank: agree with a max-reduce of "failed"
-    int *d_flag2 = nullptr;
-    CU(cudaMalloc(&d_flag2, sizeof(int)));
+    DeviceBuffer<int> d_flag2;
+    if (d_flag2.alloc(1)) return 1;
     int failed = all_ok ? 0 : 1;
     CU(cudaMemcpyAsync(d_flag2, &failed, sizeof(int), cudaMemcpyHostToDevice, p->stream));
     nr = g_nccl.AllReduce(d_flag2, d_flag2, 1, ncclInt32, ncclMax, p->comm, p->stream);
-    if (nr != ncclSuccess) { cudaFree(d_flag2); return fail("ncclAllReduce (IPC agreement): %s", g_nccl.GetErrorString(nr)); }
+    if (nr != ncclSuccess) return fail("ncclAllReduce (IPC agreement): %s", g_nccl.GetErrorString(nr));
     CU(cudaMemcpyAsync(&failed, d_flag2, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
     CU(cudaStreamSynchronize(p->stream));
-    cudaFree(d_flag2);
     if (failed) {
         const bool wanted = p->px_enabled;
         peer_teardown(p);
         if (wanted && getenv("HB2_DEBUG")) fprintf(stderr, "[hb2] rank %d: peer exchange unavailable (CUDA IPC), using NCCL collectives\n", p->rank);
         return 0;
     }
-    CU(cudaMalloc(&p->d_px_peer, R * sizeof(double *)));
-    CU(cudaMemcpy(p->d_px_peer, p->px_peer.data(), R * sizeof(double *), cudaMemcpyHostToDevice));
-    CU(cudaMalloc(&p->d_px_counter, sizeof(unsigned int)));
-    CU(cudaMemset(p->d_px_counter, 0, sizeof(unsigned int)));
+    if (p->d_px_peer.alloc(R)) return 1;
+    CU(cudaMemcpyAsync(p->d_px_peer, p->px_peer.data(), R * sizeof(double *), cudaMemcpyHostToDevice, p->stream));
+    if (p->d_px_counter.alloc(1) || p->d_px_counter.zero(p->stream)) return 1;
     p->px_payload = payload; p->px_gen = 0; p->px_ok = true;
     return 0;
 }
@@ -997,9 +1035,9 @@ int run_root(hb2_partition *p, int c0, int nc, bool use_weights, bool want_sites
     if (p->cg_G > 1) CU(cudaMemsetAsync(p->d_flag, 0, sizeof(int), p->stream));
     hb2::CombineArgs c;
     c.counter = nullptr; c.out = nullptr;
-    c.rootL = p->d_rootL; c.rootE = p->d_rootE; c.weights = use_weights ? p->d_weights : nullptr; c.freq = p->d_freq;
-    c.partial = p->d_partial; c.flag = p->d_flag; c.siteL = want_sites ? p->d_siteL : nullptr;
-    c.siteScale = want_sites ? p->d_siteScale : nullptr;
+    c.rootL = p->d_rootL; c.rootE = p->d_rootE; c.weights = use_weights ? p->d_weights : (double *)nullptr; c.freq = p->d_freq;
+    c.partial = p->d_partial; c.flag = p->d_flag; c.siteL = want_sites ? p->d_siteL : (double *)nullptr;
+    c.siteScale = want_sites ? p->d_siteScale : (long long *)nullptr;
     c.Sp = (int)p->Sp; c.S = (int)p->S; c.c0 = c0; c.nc = nc;
     if (p->cg_G > 1 && p->px_ok) {
         // class groups over NVLink peer memory: ONE kernel computes this rank's class partials, stores them into every
@@ -1064,10 +1102,8 @@ int evaluate_impl(hb2_partition *p, int c0, int nc, const double *weights, int64
     if (forcedNode >= 0) {
         if (forcedNode >= p->L + p->I) return fail("forced node %lld out of range", (long long)forcedNode);
         if (!forcedStates) return fail("forced states are null");
-        if (!p->d_forced) {
-            CU(cudaMalloc(&p->d_forced, p->Sp * sizeof(int)));
-            CU(cudaMallocHost(&p->h_forced, p->Sp * sizeof(int)));
-        }
+        // keyed on the last of the pair: after a failed allocation the next call allocates both again
+        if (!p->h_forced && (p->d_forced.alloc(p->Sp) || p->h_forced.alloc(p->Sp))) return 1;
         CU(cudaStreamSynchronize(p->stream));         // h_forced may still be in flight from the previous forced evaluation
         for (int64_t s = 0; s < p->Sp; s++) {
             const int64_t f = s < p->S ? forcedStates[s] : 0;
@@ -1087,9 +1123,7 @@ int evaluate_impl(hb2_partition *p, int c0, int nc, const double *weights, int64
     if (p->cg_G > 1) nc = p->ownN;
     if (flush_matrices(p)) return 1;
     if (p->walk_reset) {                      // an earlier pass was aborted half-way: its tags are inconsistent
-        CU(cudaMemsetAsync(p->d_condf, 0, (size_t)p->C * 2 * p->I * p->Sp * 64 * sizeof(float), p->stream));
-        CU(cudaMemsetAsync(p->d_scal, 0, (size_t)p->C * 2 * p->I * p->Sp * sizeof(int), p->stream));
-        CU(cudaMemsetAsync(p->d_err, 0, sizeof(int), p->stream));
+        if (p->d_condf.zero(p->stream) || p->d_scal.zero(p->stream) || p->d_err.zero(p->stream)) return 1;
         std::fill(p->walk_gen.begin(), p->walk_gen.end(), 0);
         std::fill(p->evaluated_cat.begin(), p->evaluated_cat.end(), 0);
         p->walk_reset = false;
@@ -1183,7 +1217,7 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
     if (device < 0 || device >= ndev) return fail("device %d out of range (%d visible)", device, ndev);
     CU(cudaSetDevice(device));
 
-    hb2_partition *p = new hb2_partition();
+    std::unique_ptr<hb2_partition, decltype(&hb2_destroy)> p(new hb2_partition(), hb2_destroy);   // destroyed on any early return
     cudaDeviceGetAttribute(&p->sm_count, cudaDevAttrMultiProcessorCount, device);
     p->device = device; p->flags = flags; p->S = S; p->D = D; p->L = L; p->I = I; p->C = C; p->B = L + I - 1; p->nAmb = nAmb;
     p->Dp = Dp;
@@ -1192,100 +1226,63 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
     const int64_t tile = (Dp == 64 && !p->use_tc) ? 64 : 128;
     p->Sp = (S + tile - 1) / tile * tile;
     p->parents.assign(flatParents, flatParents + L + I);
-    if (build_tree(flatParents, L, I, p->children, p->height)) { delete p; return 1; }
+    if (build_tree(flatParents, L, I, p->children, p->height)) return 1;
     for (int64_t k = 0; k < L * S; k++) {
         int64_t c = leafState[k];
-        if (c >= D || c < -nAmb) { delete p; return fail("leafState[%lld]=%lld out of range", (long long)k, (long long)c); }
+        if (c >= D || c < -nAmb) return fail("leafState[%lld]=%lld out of range", (long long)k, (long long)c);
     }
     if (const char *ov = getenv("HB2_WALK_LANES")) p->walk_lane_cap = std::max(1, std::min(atoi(ov), 15));
     { const char *ev = getenv("HB2_WALK_SPLIT_NODES"); p->walk_split_nodes = !(ev && ev[0] == '0'); }
-#define CUP(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { fail("%s failed: %s", #x, cudaGetErrorString(e_)); hb2_destroy(p); return 1; } } while (0)
-    CUP(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
-    for (auto &e : p->ev) CUP(cudaEventCreate(&e));
-    CUP(cudaEventCreateWithFlags(&p->ev_staging, cudaEventDisableTiming));
-    CUP(cudaEventCreateWithFlags(&p->ev_mix, cudaEventDisableTiming));
+    CU(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
+    for (auto &e : p->ev) CU(cudaEventCreate(&e));
+    CU(cudaEventCreateWithFlags(&p->ev_staging, cudaEventDisableTiming));
+    CU(cudaEventCreateWithFlags(&p->ev_mix, cudaEventDisableTiming));
     const size_t Sp = p->Sp, dpdp = (size_t)Dp * Dp, dd = (size_t)D * D;
-    CUP(cudaMalloc(&p->d_leaf, L * Sp * sizeof(int)));
-    CUP(cudaMalloc(&p->d_ambig, std::max<int64_t>(nAmb, 1) * Dp * sizeof(double)));
-    CUP(cudaMalloc(&p->d_freq, Sp * sizeof(double)));
+    cudaStream_t st = p->stream;
+    if (p->d_leaf.alloc(L * Sp) || p->d_ambig.alloc(std::max<int64_t>(nAmb, 1) * Dp) || p->d_freq.alloc(Sp)) return 1;
     if (p->use_tc) {
         // 2I node slots per class: I nodes + I side products of the walk kernel
-        CUP(cudaMalloc(&p->d_condf, (size_t)C * 2 * I * Sp * 64 * sizeof(float)));
-        CUP(cudaMalloc(&p->d_PB, (size_t)C * p->B * hb2::TC_PB_FLOATS * sizeof(float)));
-        CUP(cudaMalloc(&p->d_PTf, (size_t)C * p->B * hb2::TC_PTF_FLOATS * sizeof(float)));
-        CUP(cudaMemsetAsync(p->d_condf, 0, (size_t)C * 2 * I * Sp * 64 * sizeof(float), p->stream));
-        CUP(cudaMemsetAsync(p->d_PB, 0, (size_t)C * p->B * hb2::TC_PB_FLOATS * sizeof(float), p->stream));
-        CUP(cudaMemsetAsync(p->d_PTf, 0, (size_t)C * p->B * hb2::TC_PTF_FLOATS * sizeof(float), p->stream));
+        if (p->d_condf.alloc((size_t)C * 2 * I * Sp * 64) || p->d_PB.alloc((size_t)C * p->B * hb2::TC_PB_FLOATS) ||
+            p->d_PTf.alloc((size_t)C * p->B * hb2::TC_PTF_FLOATS) || p->d_condf.zero(st) || p->d_PB.zero(st) || p->d_PTf.zero(st))
+            return 1;
         int per_sm = 0;
-        if (lane_ctas_per_sm("prune64_tc_walk_kernel", (const void *)hb2::prune64_tc_walk_kernel, 256, hb2::WALK_SMEM_BYTES, 2, device, per_sm)) {
-            hb2_destroy(p);
-            return 1;
-        }
+        if (lane_ctas_per_sm("prune64_tc_walk_kernel", (const void *)hb2::prune64_tc_walk_kernel, 256, hb2::WALK_SMEM_BYTES, 2, device, per_sm)) return 1;
         p->walk_max_resident = std::min(per_sm, 2) * p->sm_count;
-        if (p->walk_max_resident < 1) {
-            fail("prune64_tc_walk_kernel (%d B of shared memory) cannot be resident on device %d", hb2::WALK_SMEM_BYTES, device);
-            hb2_destroy(p);
-            return 1;
-        }
+        if (p->walk_max_resident < 1)
+            return fail("prune64_tc_walk_kernel (%d B of shared memory) cannot be resident on device %d", hb2::WALK_SMEM_BYTES, device);
         p->walk_gen.assign((size_t)C * 2 * I, 0);   // matches the zero-filled conditional and exponent buffers
         const size_t walk_ints = 16 + 2 * (size_t)(L + 2 * I) + (size_t)C * 2 * I;
-        CUP(cudaMalloc(&p->d_walk, walk_ints * sizeof(int)));
-        CUP(cudaMallocHost(&p->h_walk, walk_ints * sizeof(int)));
+        if (p->d_walk.alloc(walk_ints) || p->h_walk.alloc(walk_ints)) return 1;
     } else {
-        CUP(cudaMalloc(&p->d_cond, (size_t)C * I * Sp * Dp * sizeof(double)));
-        CUP(cudaMemsetAsync(p->d_cond, 0, (size_t)C * I * Sp * Dp * sizeof(double), p->stream));
+        if (p->d_cond.alloc((size_t)C * I * Sp * Dp) || p->d_cond.zero(st)) return 1;
         if (Dp == 64) {
             // lanes kernel: side products, hand-over flags, the step list, and how many CTAs can be co-resident
             const size_t T = Sp / hb2::LANES_TILE_P;
-            CUP(cudaMalloc(&p->d_cond_side, (size_t)C * I * Sp * 64 * sizeof(double)));
-            CUP(cudaMemsetAsync(p->d_cond_side, 0, (size_t)C * I * Sp * 64 * sizeof(double), p->stream));
-            CUP(cudaMalloc(&p->d_lane_flags, (size_t)C * 2 * I * T * sizeof(int)));
-            CUP(cudaMemsetAsync(p->d_lane_flags, 0, (size_t)C * 2 * I * T * sizeof(int), p->stream));
             const size_t walk_ints = 16 + 6 * (size_t)(L + 2 * I) + 4;       // planner's pairs + the kernel's int4 descriptors
-            CUP(cudaMalloc(&p->d_walk, walk_ints * sizeof(int)));
-            CUP(cudaMallocHost(&p->h_walk, walk_ints * sizeof(int)));
+            if (p->d_cond_side.alloc((size_t)C * I * Sp * 64) || p->d_cond_side.zero(st) || p->d_lane_flags.alloc((size_t)C * 2 * I * T) ||
+                p->d_lane_flags.zero(st) || p->d_walk.alloc(walk_ints) || p->h_walk.alloc(walk_ints))
+                return 1;
             int per_sm = 0;
             if (lane_ctas_per_sm("prune64_lanes_kernel", (const void *)hb2::prune64_lanes_kernel, hb2::LANES_THREADS, hb2::LANES_SMEM_BYTES,
-                                 hb2::LANES_CTAS_PER_SM, device, per_sm)) {
-                hb2_destroy(p);
+                                 hb2::LANES_CTAS_PER_SM, device, per_sm))
                 return 1;
-            }
             p->lanes_resident = std::max(per_sm, 1) * p->sm_count;
         }
     }
-    CUP(cudaMalloc(&p->d_err, sizeof(int)));
-    CUP(cudaMemsetAsync(p->d_err, 0, sizeof(int), p->stream));
-    CUP(cudaMalloc(&p->d_scal, (size_t)C * 2 * I * Sp * sizeof(int)));      // 2I: see d_condf
-    CUP(cudaMalloc(&p->d_PT, (size_t)C * p->B * dpdp * sizeof(double)));
-    CUP(cudaMalloc(&p->d_Qres, (size_t)C * p->B * dd * sizeof(double)));
+    if (p->d_err.alloc(1) || p->d_err.zero(st)) return 1;
+    if (p->d_scal.alloc((size_t)C * 2 * I * Sp) || p->d_PT.alloc((size_t)C * p->B * dpdp) || p->d_Qres.alloc((size_t)C * p->B * dd)) return 1;   // 2I: see d_condf
     p->q_capacity = C * p->B;
-    CUP(cudaMalloc(&p->d_Q, (size_t)p->q_capacity * dd * sizeof(double)));
-    CUP(cudaMalloc(&p->d_dst, p->q_capacity * sizeof(int)));
-    CUP(cudaMalloc(&p->d_pi, Dp * sizeof(double)));
-    CUP(cudaMalloc(&p->d_rootL, (size_t)C * Sp * sizeof(double)));
-    CUP(cudaMalloc(&p->d_rootE, (size_t)C * Sp * sizeof(int)));
-    CUP(cudaMalloc(&p->d_weights, C * sizeof(double)));
+    if (p->d_Q.alloc((size_t)p->q_capacity * dd) || p->d_dst.alloc(p->q_capacity) || p->d_pi.alloc(Dp) || p->d_rootL.alloc((size_t)C * Sp) ||
+        p->d_rootE.alloc((size_t)C * Sp) || p->d_weights.alloc(C))
+        return 1;
     p->n_partial_blocks = (int)((S + 255) / 256);
-    CUP(cudaMalloc(&p->d_partial, p->n_partial_blocks * sizeof(double)));
-    CUP(cudaMalloc(&p->d_lnL, sizeof(double)));
-    CUP(cudaMalloc(&p->d_flag, sizeof(int)));
-    CUP(cudaMemsetAsync(p->d_flag, 0, sizeof(int), p->stream));
-    CUP(cudaMalloc(&p->d_root_counter, sizeof(unsigned)));
-    CUP(cudaMemsetAsync(p->d_root_counter, 0, sizeof(unsigned), p->stream));
-    CUP(cudaMalloc(&p->d_siteL, Sp * sizeof(double)));
-    CUP(cudaMalloc(&p->d_siteScale, Sp * sizeof(long long)));
-    CUP(cudaMalloc(&p->d_jobs, I * sizeof(int)));
-    CUP(cudaMalloc(&p->d_child_start, (I + 1) * sizeof(int)));
-    CUP(cudaMalloc(&p->d_child_ids, (L + I) * sizeof(int)));
-    CUP(cudaMallocHost(&p->h_Q, (size_t)p->q_capacity * dd * sizeof(double)));
-    CUP(cudaMallocHost(&p->h_dst, p->q_capacity * sizeof(int)));
-    CUP(cudaMallocHost(&p->h_small, (Dp + C + 8) * sizeof(double)));
-    CUP(cudaMallocHost(&p->h_jobs, I * sizeof(int)));
-    CUP(cudaMemsetAsync(p->d_scal, 0, (size_t)C * 2 * I * Sp * sizeof(int), p->stream));
-    CUP(cudaMemsetAsync(p->d_PT, 0, (size_t)C * p->B * dpdp * sizeof(double), p->stream));
-    CUP(cudaMemsetAsync(p->d_rootL, 0, (size_t)C * Sp * sizeof(double), p->stream));
-    CUP(cudaMemsetAsync(p->d_rootE, 0, (size_t)C * Sp * sizeof(int), p->stream));
-    {   // static uploads (pageable host vectors: synchronous copies are fine at setup time)
+    if (p->d_partial.alloc(p->n_partial_blocks) || p->d_lnL.alloc(1) || p->d_flag.alloc(1) || p->d_flag.zero(st) || p->d_root_counter.alloc(1) ||
+        p->d_root_counter.zero(st))
+        return 1;
+    if (p->d_siteL.alloc(Sp) || p->d_siteScale.alloc(Sp) || p->d_jobs.alloc(I) || p->d_child_start.alloc(I + 1) || p->d_child_ids.alloc(L + I)) return 1;
+    if (p->h_Q.alloc((size_t)p->q_capacity * dd) || p->h_dst.alloc(p->q_capacity) || p->h_small.alloc(Dp + C + 8) || p->h_jobs.alloc(I)) return 1;
+    if (p->d_scal.zero(st) || p->d_PT.zero(st) || p->d_rootL.zero(st) || p->d_rootE.zero(st)) return 1;
+    {   // static uploads (pageable host vectors: released once the copies are enqueued)
         std::vector<int> leaf((size_t)L * Sp, 0);          // padding patterns: state 0 everywhere, frequency 0
         for (int64_t l = 0; l < L; l++)
             for (int64_t s = 0; s < S; s++) leaf[l * Sp + s] = (int)leafState[l * S + s];
@@ -1297,34 +1294,20 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
         std::vector<int> cs(I + 1, 0), ci;
         for (int64_t i = 0; i < I; i++) { cs[i] = (int)ci.size(); for (int ch : p->children[i]) ci.push_back(ch); }
         cs[I] = (int)ci.size();
-        CUP(cudaStreamSynchronize(p->stream));
-        CUP(cudaMemcpy(p->d_leaf, leaf.data(), leaf.size() * sizeof(int), cudaMemcpyHostToDevice));
-        CUP(cudaMemcpy(p->d_ambig, amb.data(), amb.size() * sizeof(double), cudaMemcpyHostToDevice));
-        CUP(cudaMemcpy(p->d_freq, fr.data(), fr.size() * sizeof(double), cudaMemcpyHostToDevice));
-        CUP(cudaMemcpy(p->d_child_start, cs.data(), cs.size() * sizeof(int), cudaMemcpyHostToDevice));
-        CUP(cudaMemcpy(p->d_child_ids, ci.data(), ci.size() * sizeof(int), cudaMemcpyHostToDevice));
+        CU(cudaMemcpyAsync(p->d_leaf, leaf.data(), leaf.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+        CU(cudaMemcpyAsync(p->d_ambig, amb.data(), amb.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+        CU(cudaMemcpyAsync(p->d_freq, fr.data(), fr.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+        CU(cudaMemcpyAsync(p->d_child_start, cs.data(), cs.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+        CU(cudaMemcpyAsync(p->d_child_ids, ci.data(), ci.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     }
-    if (Dp == 32) CUP(cudaFuncSetAttribute(hb2::expm_small_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hb2::expm_small_smem_bytes(32)));
+    if (Dp == 32) CU(cudaFuncSetAttribute(hb2::expm_small_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hb2::expm_small_smem_bytes(32)));
     if (Dp == 64) {
         { const char *env = getenv("HB2_EXPM_SHARED"); p->ex_enabled = !(env && env[0] == '0'); }
-        p->ex.G = std::max((int)C + 8, HB2_MAX_TEMPLATES * (int)C); p->ex.cap = (int64_t)(C + 8) * p->B; p->ex.stride = 4096;
-        p->ex.kind.assign(p->ex.G, 0);
-        CUP(cudaMalloc(&p->ex.d_int, (size_t)(2 * p->ex.cap + p->ex.G) * sizeof(int)));
-        CUP(cudaMallocHost(&p->ex.h_int, (size_t)(2 * p->ex.cap + p->ex.G) * sizeof(int)));
-        CUP(cudaMalloc(&p->ex.d_flag, (size_t)p->ex.cap * sizeof(int)));
-        CUP(cudaMalloc(&p->ex.d_weight, (size_t)p->ex.cap * sizeof(double)));
-        CUP(cudaMalloc(&p->ex.d_colsum, (size_t)p->ex.cap * 16 * 64 * sizeof(double)));
-        CUP(cudaMalloc(&p->ex.d_groups, (size_t)p->ex.G * sizeof(hb2::ExpmGroup)));
-        CUP(cudaMemsetAsync(p->ex.d_groups, 0, (size_t)p->ex.G * sizeof(hb2::ExpmGroup), p->stream));
-        CUP(cudaMalloc(&p->ex.d_pow, (size_t)p->ex.G * hb2::EXPM_POW_TERMS * 4096 * sizeof(double)));
-        CUP(cudaMalloc(&p->ex.d_flags, (size_t)p->ex.G * hb2::EXPM_POW_TERMS * sizeof(unsigned long long)));
-        CUP(cudaMemsetAsync(p->ex.d_flags, 0, (size_t)p->ex.G * hb2::EXPM_POW_TERMS * sizeof(unsigned long long), p->stream));
-        CUP(cudaMalloc(&p->ex.d_refvec, (size_t)p->ex.G * p->ex.stride * sizeof(double)));
-        CUP(cudaFuncSetAttribute(hb2::expm_powers_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(3 * 64 * hb2::LD64 * sizeof(double))));
-        CUP(cudaFuncSetAttribute(hb2::expm64_dmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(3 * 64 * hb2::LD64 * sizeof(double))));
-        CUP(cudaFuncSetAttribute(hb2::expm64_dmma_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+        if (p->ex.alloc(std::max((int)C + 8, HB2_MAX_TEMPLATES * (int)C), (int64_t)(C + 8) * p->B, st)) return 1;
+        CU(cudaFuncSetAttribute(hb2::expm_powers_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(3 * 64 * hb2::LD64 * sizeof(double))));
+        CU(cudaFuncSetAttribute(hb2::expm64_dmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(3 * 64 * hb2::LD64 * sizeof(double))));
+        CU(cudaFuncSetAttribute(hb2::expm64_dmma_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     }
-#undef CUP
     if (Dp == 4) {
         if (const char *env = getenv("HB2_SMALL_ILP")) p->small_ilp = atoi(env);
         int b1 = 0, b2 = 0;
@@ -1340,7 +1323,7 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
     p->res_tmpl.assign(C * p->B, 0);
     p->evaluated_cat.assign(C, 0);
     p->own0 = 0; p->ownN = (int)C;
-    *out = p;
+    *out = p.release();
     return 0;
 }
 
@@ -1388,13 +1371,10 @@ int hb2_set_mixture_matrices(hb2_partition *p, int64_t cat, int64_t n, const int
     if (p->mix_busy) { CU(cudaEventSynchronize(p->ev_mix)); p->mix_busy = false; }
     if (nk > p->mix_capacity) {
         CU(cudaStreamSynchronize(p->stream));
-        for (void *d : {(void *)p->d_mix_scratch, (void *)p->d_mix_Q, (void *)p->d_mix_dst}) if (d) cudaFree(d);
-        if (p->h_mix) cudaFreeHost(p->h_mix);
-        p->d_mix_scratch = p->d_mix_Q = nullptr; p->d_mix_dst = nullptr; p->h_mix = nullptr; p->mix_capacity = 0;
-        CU(cudaMalloc(&p->d_mix_scratch, (size_t)nk * dpdp * sizeof(double)));
-        CU(cudaMalloc(&p->d_mix_Q, (size_t)nk * (dd + 1) * sizeof(double)));
-        CU(cudaMalloc(&p->d_mix_dst, (size_t)2 * nk * sizeof(int)));
-        CU(cudaMallocHost(&p->h_mix, (size_t)nk * (dd + 1) * sizeof(double) + (size_t)2 * nk * sizeof(int)));
+        p->mix_capacity = 0;
+        if (p->d_mix_scratch.alloc((size_t)nk * dpdp) || p->d_mix_Q.alloc((size_t)nk * (dd + 1)) || p->d_mix_dst.alloc((size_t)2 * nk) ||
+            p->h_mix.alloc((size_t)nk * (dd + 2)))      // 2 nk ints take nk doubles
+            return 1;
         p->mix_capacity = nk;
     }
     memcpy(p->h_mix, M, (size_t)nk * dd * sizeof(double));
@@ -1419,17 +1399,11 @@ int hb2_set_mixture_matrices(hb2_partition *p, int64_t cat, int64_t n, const int
     }
     if (launch_expm(p, p->d_mix_Q, p->d_mix_dst, (int)nk, 0, nullptr, false, p->d_mix_scratch, &sp)) return 1;
     hb2::mix_reduce_kernel<<<(unsigned)n, 256, 0, p->stream>>>(p->d_mix_scratch, p->d_mix_Q + (size_t)nk * dd, p->d_mix_dst + nk, (int)K, p->Dp,
-                                                              p->d_PT, p->use_tc ? p->d_PB : nullptr, p->d_PTf);
+                                                              p->d_PT, p->use_tc ? p->d_PB : (float *)nullptr, p->d_PTf);
     p->launches++;
     CU(cudaGetLastError());
     for (int64_t i = 0; i < n; i++) { p->have_matrix[cat * p->B + nodeIds[i]] = 1; p->is_rate[cat * p->B + nodeIds[i]] = 0; }
     return 0;
-}
-
-static void free_template(hb2_partition::Tmpl &t) {
-    for (void *d : {(void *)t.d_index, (void *)t.d_formula, (void *)t.d_vdst, (void *)t.d_colfreq, (void *)t.d_V, (void *)t.d_Vres}) if (d) cudaFree(d);
-    for (void *h : {(void *)t.h_vdst, (void *)t.h_colfreq, (void *)t.h_V}) if (h) cudaFreeHost(h);
-    t = hb2_partition::Tmpl();
 }
 
 int hb2_set_rate_template_id(hb2_partition *p, int64_t templateId, int64_t nnz, const int64_t *entryIndex, const int64_t *entryFormula,
@@ -1449,23 +1423,23 @@ int hb2_set_rate_template_id(hb2_partition *p, int64_t templateId, int64_t nnz, 
     }
     if ((int64_t)p->tmpls.size() <= templateId) p->tmpls.resize(templateId + 1);
     hb2_partition::Tmpl &t = p->tmpls[templateId];
-    free_template(t);
-    CU(cudaMalloc(&t.d_index, nnz * sizeof(int)));
-    CU(cudaMalloc(&t.d_formula, nnz * sizeof(int)));
-    CU(cudaMalloc(&t.d_colfreq, p->D * sizeof(double)));
-    CU(cudaMallocHost(&t.h_colfreq, p->D * sizeof(double)));
-    CU(cudaMalloc(&t.d_V, (size_t)p->q_capacity * nFormulas * sizeof(double)));
-    CU(cudaMalloc(&t.d_vdst, p->q_capacity * sizeof(int)));
+    t = hb2_partition::Tmpl();                // undefined until every buffer is in place
+    if (t.d_index.alloc(nnz) || t.d_formula.alloc(nnz) || t.d_colfreq.alloc(p->D) || t.h_colfreq.alloc(p->D) ||
+        t.d_V.alloc((size_t)p->q_capacity * nFormulas) || t.d_vdst.alloc(p->q_capacity))
+        return 1;
     // resident formula values of every slot (replay, shared-powers classification); cached directions of this template's
     // groups are void now
-    CU(cudaMalloc(&t.d_Vres, (size_t)p->C * p->B * nFormulas * sizeof(double)));
-    if (void_template_cache(p, (int)templateId)) return 1;
-    CU(cudaMallocHost(&t.h_V, (size_t)p->q_capacity * nFormulas * sizeof(double)));
-    CU(cudaMallocHost(&t.h_vdst, p->q_capacity * sizeof(int)));
-    CU(cudaMemcpy(t.d_index, idx.data(), nnz * sizeof(int), cudaMemcpyHostToDevice));
-    CU(cudaMemcpy(t.d_formula, frm.data(), nnz * sizeof(int), cudaMemcpyHostToDevice));
+    if (t.d_Vres.alloc((size_t)p->C * p->B * nFormulas) || void_template_cache(p, (int)templateId)) return 1;
+    if (t.h_V.alloc((size_t)p->q_capacity * nFormulas) || t.h_vdst.alloc(p->q_capacity)) return 1;
+    CU(cudaMemcpyAsync(t.d_index, idx.data(), nnz * sizeof(int), cudaMemcpyHostToDevice, p->stream));
+    CU(cudaMemcpyAsync(t.d_formula, frm.data(), nnz * sizeof(int), cudaMemcpyHostToDevice, p->stream));
     t.has_colfreq = colFreq != nullptr;
-    if (colFreq) CU(cudaMemcpy(t.d_colfreq, colFreq, p->D * sizeof(double), cudaMemcpyHostToDevice));
+    if (colFreq) {                            // staged, so that the caller may reuse colFreq at once even if it is pinned
+        memcpy(t.h_colfreq, colFreq, p->D * sizeof(double));
+        CU(cudaMemcpyAsync(t.d_colfreq, t.h_colfreq, p->D * sizeof(double), cudaMemcpyHostToDevice, p->stream));
+        CU(cudaEventRecord(p->ev_staging, p->stream));
+        p->staging_busy = true;
+    }
     t.nnz = nnz; t.nF = nFormulas; t.n_pending = 0;
     return 0;
 }
@@ -1592,38 +1566,12 @@ static int batch_sites(hb2_partition *p, int64_t templateId, int64_t nSets, cons
     // the buffers hold b_cap sets of up to bex.cap / b_cap rows; chunks are b_cap sets wherever they came from
     if (cap > p->b_cap || gk > p->b_groups_per_set || p->b_cap * R > p->bex.cap || p->b_cap * R * nF > p->b_vcap) {
         CU(cudaStreamSynchronize(p->stream));
-        hb2_partition::ExBuf &x = p->bex;
-        for (void *d : {(void *)x.d_int, (void *)x.d_flag, (void *)x.d_weight, (void *)x.d_groups, (void *)x.d_pow, (void *)x.d_refvec, (void *)x.d_flags, (void *)x.d_colsum,
-                        (void *)p->d_bPT, (void *)p->d_bV, (void *)p->d_bcond, (void *)p->d_bout, (void *)p->d_bdst, (void *)p->d_bpat, (void *)p->d_bnodeex,
-                        (void *)p->d_bmixw, (void *)p->d_brow}) if (d) cudaFree(d);
-        if (x.h_int) cudaFreeHost(x.h_int);
-        if (p->h_bdst) cudaFreeHost(p->h_bdst);
-        x = hb2_partition::ExBuf();
-        p->d_bPT = p->d_bV = p->d_bcond = p->d_bout = p->d_bmixw = nullptr; p->d_bdst = p->d_bpat = p->d_bnodeex = p->d_brow = nullptr; p->h_bdst = nullptr;
         p->b_cap = 0; p->b_vcap = 0;
         const int64_t ne = cap * R;
-        x.G = (int)(cap * gk); x.cap = ne; x.stride = 4096; x.kind.assign(x.G, 0);
-        CU(cudaMalloc(&x.d_int, (size_t)(2 * ne + x.G) * sizeof(int)));
-        CU(cudaMallocHost(&x.h_int, (size_t)(2 * ne + x.G) * sizeof(int)));
-        CU(cudaMalloc(&x.d_flag, (size_t)ne * sizeof(int)));
-        CU(cudaMalloc(&x.d_weight, (size_t)ne * sizeof(double)));
-        CU(cudaMalloc(&x.d_colsum, (size_t)ne * 16 * 64 * sizeof(double)));
-        CU(cudaMalloc(&x.d_groups, (size_t)x.G * sizeof(hb2::ExpmGroup)));
-        CU(cudaMemset(x.d_groups, 0, (size_t)x.G * sizeof(hb2::ExpmGroup)));
-        CU(cudaMalloc(&x.d_pow, (size_t)x.G * hb2::EXPM_POW_TERMS * 4096 * sizeof(double)));
-        CU(cudaMalloc(&x.d_flags, (size_t)x.G * hb2::EXPM_POW_TERMS * sizeof(unsigned long long)));
-        CU(cudaMemset(x.d_flags, 0, (size_t)x.G * hb2::EXPM_POW_TERMS * sizeof(unsigned long long)));
-        CU(cudaMalloc(&x.d_refvec, (size_t)x.G * x.stride * sizeof(double)));
-        CU(cudaMalloc(&p->d_bPT, (size_t)ne * 4096 * sizeof(double)));
-        CU(cudaMalloc(&p->d_bV, (size_t)ne * nF * sizeof(double)));
-        CU(cudaMalloc(&p->d_bcond, (size_t)cap * p->I * 64 * sizeof(double)));
-        CU(cudaMalloc(&p->d_bnodeex, (size_t)cap * p->I * sizeof(int)));
-        CU(cudaMalloc(&p->d_bout, (size_t)cap * sizeof(double)));
-        CU(cudaMalloc(&p->d_bdst, (size_t)ne * sizeof(int)));
-        CU(cudaMalloc(&p->d_bpat, (size_t)cap * sizeof(int)));
-        CU(cudaMallocHost(&p->h_bdst, (size_t)(ne + cap) * sizeof(int)));
-        CU(cudaMalloc(&p->d_bmixw, (size_t)ne * sizeof(double)));
-        CU(cudaMalloc(&p->d_brow, (size_t)(B + 1) * sizeof(int)));
+        if (p->bex.alloc((int)(cap * gk), ne, p->stream) || p->d_bPT.alloc((size_t)ne * 4096) || p->d_bV.alloc((size_t)ne * nF) ||
+            p->d_bcond.alloc((size_t)cap * p->I * 64) || p->d_bnodeex.alloc((size_t)cap * p->I) || p->d_bout.alloc(cap) || p->d_bdst.alloc(ne) ||
+            p->d_bpat.alloc(cap) || p->h_bdst.alloc(ne + cap) || p->d_bmixw.alloc(ne) || p->d_brow.alloc(B + 1))
+            return 1;
         p->b_cap = cap; p->b_groups_per_set = gk; p->b_vcap = ne * nF;
     }
     double *hs = p->h_small;
@@ -1734,8 +1682,8 @@ int hb2_read_transition(hb2_partition *p, int64_t cat, int64_t node, double *P) 
 
 static hb2::BranchCacheArgs bc_args(hb2_partition *p, int c0, int nc) {
     hb2::BranchCacheArgs a{};
-    a.cv.c64 = p->use_tc ? nullptr : p->d_cond;
-    a.cv.c32 = p->use_tc ? p->d_condf : nullptr;
+    a.cv.c64 = p->use_tc ? nullptr : (double *)p->d_cond;
+    a.cv.c32 = p->use_tc ? p->d_condf : (float *)nullptr;
     a.cv.scal = p->d_scal; a.cv.I = (int)(p->use_tc ? 2 * p->I : p->I); a.cv.Sp = (int)p->Sp; a.cv.Dp = p->Dp; a.cv.tagged = p->use_tc ? 1 : 0;
     a.PT = p->d_PT; a.leaf = p->d_leaf; a.ambig = p->d_ambig; a.pi = p->d_pi; a.out = p->d_bc_out; a.outE = p->d_bc_outE;
     a.L = (int)p->L; a.B = (int)p->B; a.D = (int)p->D; a.Dp = p->Dp; a.Sp = (int)p->Sp; a.S = (int)p->S; a.cat0 = c0; a.ncls = nc;
@@ -1749,11 +1697,10 @@ int hb2_branch_cache_build(hb2_partition *p, int64_t node, const double *rootFre
     for (int c = p->own0; c < p->own0 + p->ownN; c++)
         if (!p->evaluated_cat[c]) return fail("hb2_branch_cache_build: rate class %d has never been evaluated (no resident conditionals)", c);
     if (flush_matrices(p)) return 1;
-    if (!p->d_bc_out) {
-        CU(cudaMalloc(&p->d_bc_out, (size_t)p->C * p->Sp * p->Dp * sizeof(double)));
-        CU(cudaMalloc(&p->d_bc_outE, (size_t)p->C * p->Sp * sizeof(int)));
-        CU(cudaMalloc(&p->d_bc_sib, (size_t)(3 * (p->L + p->I) + 2) * sizeof(int)));
-    }
+    // keyed on the last of the three: after a failed allocation the next build allocates all of them again
+    if (!p->d_bc_sib && (p->d_bc_out.alloc((size_t)p->C * p->Sp * p->Dp) || p->d_bc_outE.alloc((size_t)p->C * p->Sp) ||
+                         p->d_bc_sib.alloc(3 * (p->L + p->I) + 2)))
+        return 1;
     double *hs = p->h_small;
     for (int k = 0; k < p->Dp; k++) hs[k] = k < p->D ? rootFreqs[k] : 0.0;
     CU(cudaMemcpyAsync(p->d_pi, hs, p->Dp * sizeof(double), cudaMemcpyHostToDevice, p->stream));
@@ -1768,7 +1715,6 @@ int hb2_branch_cache_build(hb2_partition *p, int64_t node, const double *rootFre
         off[i + 1] = (int)sib.size();
         down[i] = (i + 1 < path.size()) ? on_path : -1;
     }
-    CU(cudaStreamSynchronize(p->stream));            // h_small / path upload below are synchronous with respect to earlier work
     // one launch for the whole path: [siblings | sibling offsets (npath+1) | path child below each path node (npath)]
     std::vector<int> pk(sib);
     const int o_off = (int)pk.size();
@@ -1776,7 +1722,7 @@ int hb2_branch_cache_build(hb2_partition *p, int64_t node, const double *rootFre
     const int o_down = (int)pk.size();
     pk.insert(pk.end(), down.begin(), down.end());
     if ((int64_t)pk.size() > 3 * (p->L + p->I) + 2) return fail("branch-cache path does not fit its buffer");
-    CU(cudaMemcpy(p->d_bc_sib, pk.data(), pk.size() * sizeof(int), cudaMemcpyHostToDevice));
+    CU(cudaMemcpyAsync(p->d_bc_sib, pk.data(), pk.size() * sizeof(int), cudaMemcpyHostToDevice, p->stream));
     hb2::BranchCacheArgs a = bc_args(p, p->own0, p->ownN);
     hb2::BranchPathArgs bp;
     bp.sib = p->d_bc_sib; bp.sib_off = p->d_bc_sib + o_off; bp.down = p->d_bc_sib + o_down; bp.npath = (int)path.size();
@@ -1881,15 +1827,15 @@ int hb2_comm_gather_sites(hb2_partition *p, const double *siteL, const int64_t *
     CU(cudaSetDevice(p->device));
     const int R = p->n_ranks, G = std::max(p->cg_G, 1);
     // 1. every rank's pattern count
-    long long mine = (long long)p->S, *d_cnt = nullptr;
+    long long mine = (long long)p->S;
     std::vector<long long> cnt(R);
-    CU(cudaMalloc(&d_cnt, (size_t)(R + 1) * sizeof(long long)));
+    DeviceBuffer<long long> d_cnt;
+    if (d_cnt.alloc(R + 1)) return 1;
     CU(cudaMemcpyAsync(d_cnt + R, &mine, sizeof(long long), cudaMemcpyHostToDevice, p->stream));
     ncclResult_t nr = g_nccl.AllGather(d_cnt + R, d_cnt, sizeof(long long), ncclChar, p->comm, p->stream);
-    if (nr != ncclSuccess) { cudaFree(d_cnt); return fail("ncclAllGather (pattern counts): %s", g_nccl.GetErrorString(nr)); }
+    if (nr != ncclSuccess) return fail("ncclAllGather (pattern counts): %s", g_nccl.GetErrorString(nr));
     CU(cudaMemcpyAsync(cnt.data(), d_cnt, (size_t)R * sizeof(long long), cudaMemcpyDeviceToHost, p->stream));
     CU(cudaStreamSynchronize(p->stream));
-    cudaFree(d_cnt);
     long long mx = 0, tot = 0;
     for (int r = 0; r < R; r++) { mx = std::max(mx, cnt[r]); if (r % G == 0) tot += cnt[r]; }    // ranks of one shard hold the same patterns
     *total = (int64_t)tot;
@@ -1898,15 +1844,13 @@ int hb2_comm_gather_sites(hb2_partition *p, const double *siteL, const int64_t *
     const size_t rec = (size_t)mx * 16;
     std::vector<unsigned char> send(rec, 0), all(rec * R);
     for (long long s = 0; s < mine; s++) { memcpy(&send[(size_t)s * 16], siteL + s, 8); memcpy(&send[(size_t)s * 16 + 8], siteScale + s, 8); }
-    unsigned char *d_send = nullptr, *d_all = nullptr;
-    CU(cudaMalloc(&d_send, std::max<size_t>(rec, 16)));
-    CU(cudaMalloc(&d_all, std::max<size_t>(rec * R, 16)));
+    DeviceBuffer<unsigned char> d_send, d_all;
+    if (d_send.alloc(std::max<size_t>(rec, 16)) || d_all.alloc(std::max<size_t>(rec * R, 16))) return 1;
     CU(cudaMemcpyAsync(d_send, send.data(), rec, cudaMemcpyHostToDevice, p->stream));
     nr = g_nccl.AllGather(d_send, d_all, rec, ncclChar, p->comm, p->stream);
-    if (nr != ncclSuccess) { cudaFree(d_send); cudaFree(d_all); return fail("ncclAllGather (per-pattern outputs): %s", g_nccl.GetErrorString(nr)); }
+    if (nr != ncclSuccess) return fail("ncclAllGather (per-pattern outputs): %s", g_nccl.GetErrorString(nr));
     CU(cudaMemcpyAsync(all.data(), d_all, rec * R, cudaMemcpyDeviceToHost, p->stream));
     CU(cudaStreamSynchronize(p->stream));
-    cudaFree(d_send); cudaFree(d_all);
     // 3. shard order = rank order of the first rank of every shard
     int64_t at = 0;
     for (int r = 0; r < R; r += G)
@@ -1929,22 +1873,19 @@ int hb2_comm_class_groups(hb2_partition *p, int nGroups) {
     p->ownN = (int)(p->C / nGroups); p->own0 = p->cg_g * p->ownN;
     if (nGroups == 1) return 0;
     // exchange length: the longest padded shard among the ranks (shards of the same communicator may differ in size)
-    int *d_len = nullptr;
-    CU(cudaMalloc(&d_len, sizeof(int)));
+    DeviceBuffer<int> d_len;
+    if (d_len.alloc(1)) return 1;
     int len = (int)p->Sp;
     CU(cudaMemcpyAsync(d_len, &len, sizeof(int), cudaMemcpyHostToDevice, p->stream));
     ncclResult_t r = g_nccl.AllReduce(d_len, d_len, 1, ncclInt32, ncclMax, p->comm, p->stream);
-    if (r != ncclSuccess) { cudaFree(d_len); return fail("ncclAllReduce(max): %s", g_nccl.GetErrorString(r)); }
+    if (r != ncclSuccess) return fail("ncclAllReduce(max): %s", g_nccl.GetErrorString(r));
     CU(cudaMemcpyAsync(&len, d_len, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
     CU(cudaStreamSynchronize(p->stream));
-    cudaFree(d_len);
     p->xchg_len = len;
-    for (double **d : {&p->d_xsend, &p->d_xrecv, &p->d_xfreq, &p->d_xpartial}) if (*d) { cudaFree(*d); *d = nullptr; }
     const size_t tot = (size_t)2 * len * p->n_ranks;
-    CU(cudaMalloc(&p->d_xsend, tot * sizeof(double)));
-    CU(cudaMalloc(&p->d_xrecv, tot * sizeof(double)));
-    CU(cudaMalloc(&p->d_xfreq, (size_t)len * p->n_ranks * sizeof(double)));
-    CU(cudaMalloc(&p->d_xpartial, ((size_t)len * p->n_ranks / 256 + 2) * sizeof(double)));
+    if (p->d_xsend.alloc(tot) || p->d_xrecv.alloc(tot) || p->d_xfreq.alloc((size_t)len * p->n_ranks) ||
+        p->d_xpartial.alloc((size_t)len * p->n_ranks / 256 + 2))
+        return 1;
     // pattern frequencies of every rank, gathered once with the same zero-elsewhere sum (d_xsend doubles as scratch)
     CU(cudaMemsetAsync(p->d_xsend, 0, tot * sizeof(double), p->stream));
     CU(cudaMemcpyAsync(p->d_xsend + (size_t)p->rank * len, p->d_freq, (size_t)std::min<int64_t>(p->Sp, len) * sizeof(double), cudaMemcpyDeviceToDevice, p->stream));
@@ -1958,30 +1899,14 @@ int hb2_comm_class_groups(hb2_partition *p, int nGroups) {
 void hb2_destroy(hb2_partition *p) {
     if (!p) return;
     cudaSetDevice(p->device);
-    if (p->stream) cudaStreamSynchronize(p->stream);
+    if (p->stream) cudaStreamSynchronize(p->stream);     // first: the pool may hand the released blocks out at once
     peer_teardown(p);
     if (p->comm) g_nccl.CommDestroy(p->comm);
-    void *dev[] = {p->d_leaf, p->d_scal, p->d_rootE, p->d_child_start, p->d_child_ids, p->d_jobs, p->d_dst, p->d_flag,
-                   p->d_mix_dst, p->d_mix_Q, p->d_ambig, p->d_freq, p->d_cond, p->d_PT, p->d_Q, p->d_pi, p->d_rootL, p->d_weights,
-                   p->d_partial, p->d_lnL, p->d_siteL, p->d_siteScale, p->d_Qres, p->d_condf, p->d_PB, p->d_PTf, p->d_err, p->d_mix_scratch, p->d_xsend, p->d_xrecv, p->d_xfreq, p->d_xpartial, p->d_bc_out, p->d_bc_outE, p->d_bc_sib, p->d_walk, p->d_forced, p->d_cond_side, p->d_lane_flags, p->d_root_counter, p->ex.d_int, p->ex.d_flag, p->ex.d_weight, p->ex.d_groups, p->ex.d_pow, p->ex.d_refvec, p->ex.d_flags, p->ex.d_colsum, p->bex.d_colsum, p->bex.d_int, p->bex.d_flag, p->bex.d_weight, p->bex.d_groups, p->bex.d_pow, p->bex.d_refvec, p->bex.d_flags,
-                   p->d_bPT, p->d_bV, p->d_bcond, p->d_bout, p->d_bdst, p->d_bpat, p->d_bnodeex, p->d_bmixw, p->d_brow};
-    for (void *d : dev) if (d) cudaFree(d);
-    if (p->h_Q) cudaFreeHost(p->h_Q);
-    if (p->h_small) cudaFreeHost(p->h_small);
-    if (p->h_jobs) cudaFreeHost(p->h_jobs);
-    if (p->h_dst) cudaFreeHost(p->h_dst);
-    for (auto &t : p->tmpls) free_template(t);
-    if (p->h_walk) cudaFreeHost(p->h_walk);
-    if (p->h_mix) cudaFreeHost(p->h_mix);
-    if (p->h_forced) cudaFreeHost(p->h_forced);
-    if (p->ex.h_int) cudaFreeHost(p->ex.h_int);
-    if (p->bex.h_int) cudaFreeHost(p->bex.h_int);
-    if (p->h_bdst) cudaFreeHost(p->h_bdst);
-    if (p->ev_mix) cudaEventDestroy(p->ev_mix);
-    for (auto &e : p->ev) if (e) cudaEventDestroy(e);
-    if (p->ev_staging) cudaEventDestroy(p->ev_staging);
-    if (p->stream) cudaStreamDestroy(p->stream);
-    delete p;
+    const cudaStream_t stream = p->stream;
+    const cudaEvent_t events[] = {p->ev_mix, p->ev[0], p->ev[1], p->ev[2], p->ev[3], p->ev_staging};
+    delete p;                                             // releases every buffer
+    for (cudaEvent_t e : events) if (e) cudaEventDestroy(e);
+    if (stream) cudaStreamDestroy(stream);
 }
 
 int64_t hb2_launch_count(const hb2_partition *p) { return p ? p->launches : 0; }
