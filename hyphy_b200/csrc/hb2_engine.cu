@@ -837,6 +837,8 @@ int run_walk(hb2_partition *p, int cat0, int ncls, const std::vector<char> &dirt
 // The pruning kernels, each of which prunes the dirty nodes of a pass in one launch: the tensor walk (33..64 states), the
 // fp64 lanes kernel (33..64 states with HB2_FLAG_FORCE_FP64) and the small-state walks (<= 32 padded states).
 enum PruneKernel { TC_WALK, FP64_LANES, SMALL_DMMA, SMALL_WALK_ILP, SMALL_WALK };
+// SMALL_WALK_ILP and SMALL_WALK are prune_small_walk_kernel with two and one patterns per thread; they keep their own
+// names, which hb2_pruning_kernel reports
 const char *const PRUNE_KERNEL_NAME[] = {"prune64_tc_walk_kernel", "prune64_lanes_kernel", "prune_small_dmma_kernel",
                                          "prune_small_walk_ilp_kernel", "prune_small_walk_kernel"};
 
@@ -880,14 +882,15 @@ int run_small_walk(hb2_partition *p, int cat0, int ncls, const std::vector<char>
             if (p->Dp == 16) hb2::prune_small_dmma_kernel<16, 4><<<g, 128, 0, p->stream>>>(a, p->d_jobs, n);
             else hb2::prune_small_dmma_kernel<24, 4><<<g, 128, 0, p->stream>>>(a, p->d_jobs, n);
         }
-    } else if (kernel == SMALL_WALK_ILP) {
-        dim3 g2((unsigned)((p->Sp + 255) / 256), (unsigned)ncls);
-        hb2::prune_small_walk_ilp_kernel<4, 2><<<g2, 128, 0, p->stream>>>(a, p->d_jobs, n);
-    } else {
-        dim3 grid((unsigned)(p->Sp / 128), (unsigned)ncls);   // 4 / 8 padded states: one thread per pattern
+    } else {                                     // 4 / 8 padded states: PP patterns per thread (two only for 4 states)
+        const int PP = kernel == SMALL_WALK_ILP ? 2 : 1;
+        dim3 grid((unsigned)((p->Sp + 128 * PP - 1) / (128 * PP)), (unsigned)ncls);
         switch (p->Dp) {
-            case 4: hb2::prune_small_walk_kernel<4><<<grid, 128, 0, p->stream>>>(a, p->d_jobs, n); break;
-            case 8: hb2::prune_small_walk_kernel<8><<<grid, 128, 0, p->stream>>>(a, p->d_jobs, n); break;
+            case 4:
+                if (PP == 2) hb2::prune_small_walk_kernel<4, 2><<<grid, 128, 0, p->stream>>>(a, p->d_jobs, n);
+                else hb2::prune_small_walk_kernel<4, 1><<<grid, 128, 0, p->stream>>>(a, p->d_jobs, n);
+                break;
+            case 8: hb2::prune_small_walk_kernel<8, 1><<<grid, 128, 0, p->stream>>>(a, p->d_jobs, n); break;
             default: return fail("unsupported padded state count %d", p->Dp);
         }
     }
@@ -1311,8 +1314,8 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
     if (Dp == 4) {
         if (const char *env = getenv("HB2_SMALL_ILP")) p->small_ilp = atoi(env);
         int b1 = 0, b2 = 0;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b1, hb2::prune_small_walk_kernel<4>, 128, 0);
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b2, hb2::prune_small_walk_ilp_kernel<4, 2>, 128, 0);
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b1, hb2::prune_small_walk_kernel<4, 1>, 128, 0);
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b2, hb2::prune_small_walk_kernel<4, 2>, 128, 0);
         p->small_resident[0] = std::max(b1, 1) * p->sm_count;
         p->small_resident[1] = std::max(b2, 1) * p->sm_count;
     }

@@ -2,7 +2,7 @@
 //
 //   expm64_dmma_kernel / expm_small_kernel  P = exp(Q t) per (branch, rate class), one CTA per matrix
 //                                           (replaces _Matrix::Exponentiate, reference matrix.cpp:5537-5951)
-//   prune_small_walk_kernel                 Felsenstein pruning pass for 4 / 8 padded states, one thread per pattern:
+//   prune_small_walk_kernel<Dp, PP>         Felsenstein pruning pass for 4 / 8 padded states, PP patterns per thread:
 //                                           all children folded (leaf column gather, ambiguity mat-vec, internal
 //                                           contraction), per-pattern renormalisation, root pi-dot
 //                                           (replaces ComputeTreeBlockByBranch, reference tree_evaluator.cpp:3556-4171)
@@ -817,133 +817,35 @@ __global__ void __launch_bounds__(128) expm_small_kernel(ExpmArgs a) {
 }
 
 
+// A pinned node (PruneArgs::forced_node) keeps only the pattern's forced state f.
+template <int N>
+__device__ __forceinline__ void keep_state(double (&v)[N], int f) {
+#pragma unroll
+    for (int k = 0; k < N; k++) if (k != f) v[k] = 0.0;
+}
+
 // ------------------------------------------------------------------------------------------------
-// 4 / 8 padded states, whole pruning pass in ONE launch: thread s owns pattern s and walks the dirty internal nodes in
+// 4 / 8 padded states, whole pruning pass in ONE launch: each thread owns PP patterns and walks the dirty internal nodes in
 // post-order.  Every dependency is thread-local (a child's conditionals were written by the same thread earlier in the
 // same launch, or are a valid cache from an earlier evaluation), so there is no synchronisation of any kind; P^T of a
 // branch is read by all threads at the same address (L1 broadcast).  HBM traffic per evaluation is the algorithmic
 // minimum: one coalesced write and (at most) one read of Dp*8+4 bytes per (node, pattern) plus 4 B per leaf state.
-// grid = (Sp/128, classes), block = 128.  jobs = dirty internal indices, ascending (= post-order).
+// The node computed by the previous job is, in post-order, very often a child of the current one (every node follows its
+// last child): its vectors are handed over in registers instead of being re-read from L2 (the thread would wait a full L2
+// round trip for data it wrote a moment ago).
+// PP = 1 (4 and 8 states) is bound by the latency of each thread's serial node chain, and -- every CTA walking the whole
+// tree -- by wave quantisation (256 x 200 k nucleotides: 1563 CTAs on 1332 resident = 1.17 waves, i.e. two passes).  With
+// PP = 2 (4 states) the loads and the arithmetic of both patterns are in flight together (the pass gets 1.55x longer, not
+// 2x) and half as many CTAs cover the alignment; the host picks the variant with the cheaper (passes x pass cost).
+// Thread t of CTA b owns patterns (b*PP + u)*128 + t: coalesced for every u.
+// grid = (ceil(Sp / (128*PP)), classes), block = 128.  jobs = dirty internal indices, ascending (= post-order).
 // ------------------------------------------------------------------------------------------------
-// (Forcing 16 CTAs/SM for 4 states -- 32 registers, spills -- was slower.)
-template <int DP>
-__global__ void __launch_bounds__(128) prune_small_walk_kernel(PruneArgs a, const int *__restrict__ jobs, int njobs) {
-    // P^T of a branch (16 / 64 doubles) is read straight through L1; 16..32 states run prune_small_dmma_kernel.
-    static_assert(DP <= 8, "one thread per pattern is used for 4 and 8 padded states only");
-    // The node computed by the previous job is, in post-order, very often a child of the current one (every node follows
-    // its last child): its vector is handed over in registers instead of being re-read from L2 (the thread would wait a
-    // full L2 round trip for data it wrote a moment ago).
-    const int tid = threadIdx.x;
-    const int cat = a.cat0 + blockIdx.y;
-    const size_t Sp = a.Sp;
-    const size_t s = (size_t)blockIdx.x * 128 + tid;
-    double pv[DP];
-    int prev = -1, pex = 0;
-    for (int jb = 0; jb < njobs; jb++) {
-        const int par = __ldg(jobs + jb);
-        double v[DP];
-#pragma unroll
-        for (int k = 0; k < DP; k++) v[k] = 1.0;
-        int ex = 0;
-        const int c_begin = __ldg(a.tree.child_start + par), c_end = __ldg(a.tree.child_start + par + 1);
-        for (int ci = c_begin; ci < c_end; ci++) {
-            const int child = __ldg(a.tree.child_ids + ci);
-            const double *PT = a.PT + ((size_t)cat * a.B + child) * DP * DP;
-            if (child < a.L) {
-                const int code = (child == a.forced_node) ? __ldg(a.forced + s) : __ldg(a.leaf + (size_t)child * Sp + s);
-                if (code >= 0) {
-                    const double2 *row = reinterpret_cast<const double2 *>(PT + (size_t)code * DP);
-#pragma unroll
-                    for (int k = 0; k < DP; k += 2) { const double2 r = __ldg(row + k / 2); v[k] *= r.x; v[k + 1] *= r.y; }
-                } else {
-                    const double *amb = a.ambig + (size_t)(-code - 1) * DP;
-                    double acc[DP];
-#pragma unroll
-                    for (int k = 0; k < DP; k++) acc[k] = 0.0;
-                    for (int j = 0; j < a.D; j++) {
-                        const double wgt = __ldg(amb + j);
-                        const double2 *row = reinterpret_cast<const double2 *>(PT + (size_t)j * DP);
-#pragma unroll
-                        for (int k = 0; k < DP; k += 2) { const double2 r = __ldg(row + k / 2); acc[k] = fma(wgt, r.x, acc[k]); acc[k + 1] = fma(wgt, r.y, acc[k + 1]); }
-                    }
-#pragma unroll
-                    for (int k = 0; k < DP; k++) v[k] *= acc[k];
-                }
-            } else {
-                const int cin = child - a.L;
-                double x[DP];
-                if (cin == prev) {
-#pragma unroll
-                    for (int j = 0; j < DP; j++) x[j] = pv[j];
-                    ex += pex;
-                } else {
-                    const double2 *X = reinterpret_cast<const double2 *>(a.cond + (((size_t)cat * a.I + cin) * Sp + s) * DP);
-#pragma unroll
-                    for (int j = 0; j < DP; j += 2) { const double2 t = X[j / 2]; x[j] = t.x; x[j + 1] = t.y; }
-                    ex += a.scal[((size_t)cat * a.I + cin) * Sp + s];
-                }
-                double acc[DP];
-#pragma unroll
-                for (int k = 0; k < DP; k++) acc[k] = 0.0;
-#pragma unroll
-                for (int j = 0; j < DP; j++) {
-                    const double2 *row = reinterpret_cast<const double2 *>(PT + (size_t)j * DP);
-#pragma unroll
-                    for (int k = 0; k < DP; k += 2) { const double2 r = __ldg(row + k / 2); acc[k] = fma(x[j], r.x, acc[k]); acc[k + 1] = fma(x[j], r.y, acc[k + 1]); }
-                }
-#pragma unroll
-                for (int k = 0; k < DP; k++) v[k] *= acc[k];
-            }
-            if (ci - c_begin >= 1 && ci + 1 < c_end) {       // wide node: before its third and later children
-                if (a.L + par == a.forced_node) {           // pinned: rescale by the forced state, the only one that survives
-                    const int f = __ldg(a.forced + s);
-#pragma unroll
-                    for (int k = 0; k < DP; k++) if (k != f) v[k] = 0.0;
-                }
-                rescale_running(v, ex);
-            }
-        }
-        if (a.L + par == a.forced_node) {
-            const int f = __ldg(a.forced + s);
-#pragma unroll
-            for (int k = 0; k < DP; k++) if (k != f) v[k] = 0.0;
-        }
-        double m = 0.0;
-#pragma unroll
-        for (int k = 0; k < DP; k++) m = fmax(m, v[k]);
-        if (m > 0.0 && m < INFINITY) {
-            const int e = ilogb(m) + 1;
-            const double s1 = exp2i(-(e / 2)), s2 = exp2i(-(e - e / 2));
-#pragma unroll
-            for (int k = 0; k < DP; k++) v[k] = v[k] * s1 * s2;
-            ex += e;
-        }
-        double2 *outp = reinterpret_cast<double2 *>(a.cond + (((size_t)cat * a.I + par) * Sp + s) * DP);
-#pragma unroll
-        for (int k = 0; k < DP; k += 2) outp[k / 2] = make_double2(v[k], v[k + 1]);
-        a.scal[((size_t)cat * a.I + par) * Sp + s] = ex;
-#pragma unroll
-        for (int k = 0; k < DP; k++) pv[k] = v[k];
-        prev = par; pex = ex;
-        if (par == a.I - 1) {
-            double r = 0.0;
-#pragma unroll
-            for (int k = 0; k < DP; k++) r = fma(v[k], a.pi[k], r);
-            a.rootL[(size_t)cat * Sp + s] = r;
-            a.rootE[(size_t)cat * Sp + s] = ex;
-        }
-    }
-}
-
-// ------------------------------------------------------------------------------------------------
-// 4 / 8 padded states, PP patterns per thread: the one-pattern kernel above is bound by the latency of each thread's serial
-// node chain, and -- every CTA walking the whole tree -- by wave quantisation (256 x 200 k nucleotides: 1563 CTAs on 1332
-// resident = 1.17 waves, i.e. two passes).  With two patterns per thread the loads and the arithmetic of both are in flight
-// together (the pass gets 1.55x longer, not 2x) and half as many CTAs cover the alignment; the host picks the variant
-// with the cheaper (passes x pass cost).  Thread t of CTA b owns patterns (b*PP + u)*128 + t: coalesced for every u.
-// ------------------------------------------------------------------------------------------------
+// (Forcing 16 CTAs/SM for 4 states -- 32 registers, spills -- was slower.  PP = 1 takes no minimum: a minimum of 1 CTA/SM
+// lets ptxas spend up to 216 registers.)
 template <int DP, int PP>
-__global__ void __launch_bounds__(128, 6) prune_small_walk_ilp_kernel(PruneArgs a, const int *__restrict__ jobs, int njobs) {
+__global__ void __launch_bounds__(128, PP == 1 ? 0 : 6) prune_small_walk_kernel(PruneArgs a, const int *__restrict__ jobs, int njobs) {
+    // P^T of a branch (16 / 64 doubles) is read straight through L1; 16..32 states run prune_small_dmma_kernel.
+    static_assert(DP <= 8, "patterns in registers are used for 4 and 8 padded states only");
     const int tid = threadIdx.x;
     const int cat = a.cat0 + blockIdx.y;
     const size_t Sp = a.Sp;
@@ -952,7 +854,7 @@ __global__ void __launch_bounds__(128, 6) prune_small_walk_ilp_kernel(PruneArgs 
 #pragma unroll
     for (int u = 0; u < PP; u++) {
         s[u] = ((size_t)blockIdx.x * PP + u) * 128 + tid;
-        live[u] = s[u] < Sp;
+        live[u] = PP == 1 || s[u] < Sp;       // Sp is a multiple of 128: with one pattern per thread every slot is live
         if (!live[u]) s[u] = Sp - 1;          // loads stay in range; nothing is stored for a dead slot
     }
     double pv[PP][DP];
@@ -1041,11 +943,8 @@ __global__ void __launch_bounds__(128, 6) prune_small_walk_ilp_kernel(PruneArgs 
             if (ci - c_begin >= 1 && ci + 1 < c_end) {       // wide node: before its third and later children
 #pragma unroll
                 for (int u = 0; u < PP; u++) {
-                    if (a.L + par == a.forced_node) {       // pinned: rescale by the forced state, the only one that survives
-                        const int f = __ldg(a.forced + s[u]);
-#pragma unroll
-                        for (int k = 0; k < DP; k++) if (k != f) v[u][k] = 0.0;
-                    }
+                    // pinned: rescale by the forced state, the only one that survives
+                    if (a.L + par == a.forced_node) keep_state(v[u], __ldg(a.forced + s[u]));
                     rescale_running(v[u], ex[u]);
                 }
             }
@@ -1053,11 +952,7 @@ __global__ void __launch_bounds__(128, 6) prune_small_walk_ilp_kernel(PruneArgs 
         const bool pinned = a.L + par == a.forced_node;
 #pragma unroll
         for (int u = 0; u < PP; u++) {
-            if (pinned) {
-                const int f = __ldg(a.forced + s[u]);
-#pragma unroll
-                for (int k = 0; k < DP; k++) if (k != f) v[u][k] = 0.0;
-            }
+            if (pinned) keep_state(v[u], __ldg(a.forced + s[u]));
             double m = 0.0;
 #pragma unroll
             for (int k = 0; k < DP; k++) m = fmax(m, v[u][k]);
@@ -1167,6 +1062,43 @@ __device__ __forceinline__ double merge_classes(int n, Term term, int &emax_out)
     return sum;
 }
 
+// log L of a pattern with L = sum * 2^emax: NaN stays NaN, and a sum that is neither positive nor NaN gives -inf after
+// impossible() has run (the caller's flag).
+template <class Impossible>
+__device__ __forceinline__ double pattern_lnl(double sum, int emax, Impossible impossible) {
+    if (sum > 0.0) return log(sum) + (double)emax * 0.693147180559945309417232121458;
+    if (sum != sum) return sum;
+    impossible();
+    return -INFINITY;
+}
+
+// The reference's per-pattern output convention for L = sum * 2^emax: L = siteL * 2^(-64*siteScale) with siteL = sum * 2^r,
+// r in (-64, 0] (DESIGN §4.5).  A sum that is 0 or NaN goes out as it is, with siteScale 0.
+struct SiteOut {
+    double L;
+    long long scale;
+};
+__device__ __forceinline__ SiteOut site_output(double sum, int emax) {
+    long long cnt = 0; double outL = sum;
+    if (sum > 0.0) {
+        cnt = (emax < 0) ? (long long)((-emax) / 64) : -(long long)((emax + 63) / 64);
+        const int rem = emax + (int)(64 * cnt);    // in (-64, 0]
+        outL = sum * exp2i(rem);
+    }
+    return {outL, cnt};
+}
+
+// red[0] = the sum of v over the 256 threads of the block, added in a fixed order: the same bits on every run.  Called by
+// every thread; ends with a barrier.
+__device__ __forceinline__ void block_sum256(double *red, double v) {
+    red[threadIdx.x] = v;
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+        if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
+        __syncthreads();
+    }
+}
+
 struct CombineArgs {
     const double *rootL; const int *rootE; const double *weights; const double *freq;
     double *partial; int *flag; double *siteL; long long *siteScale;
@@ -1188,29 +1120,14 @@ __global__ void __launch_bounds__(256) combine_kernel(CombineArgs a) {
         }, emax);
         if (emax == INT_MIN) emax = 0;
         const double f = a.freq[s];
-        double lnl;
-        if (sum > 0.0) lnl = log(sum) + (double)emax * 0.693147180559945309417232121458;
-        else if (sum != sum) lnl = sum;
-        else { lnl = -INFINITY; if (f > 0.0) atomicOr(a.flag, 1); }
+        const double lnl = pattern_lnl(sum, emax, [&] { if (f > 0.0) atomicOr(a.flag, 1); });
         term = (f > 0.0) ? f * lnl : 0.0;
         if (a.siteL) {
-            // reference convention: L_true = siteL * 2^(-64*count); keep siteL in (2^-64, 1]
-            long long cnt = 0; double outL = sum;
-            if (sum > 0.0) {
-                int e2 = emax;                       // L_true = sum * 2^e2
-                cnt = (e2 < 0) ? (long long)((-e2) / 64) : -(long long)((e2 + 63) / 64);
-                const int rem = e2 + (int)(64 * cnt);    // in (-64, 0]
-                outL = sum * exp2i(rem);
-            }
-            a.siteL[s] = outL; a.siteScale[s] = cnt;
+            const SiteOut o = site_output(sum, emax);
+            a.siteL[s] = o.L; a.siteScale[s] = o.scale;
         }
     }
-    red[threadIdx.x] = term;
-    __syncthreads();
-    for (int o = 128; o > 0; o >>= 1) {
-        if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
-        __syncthreads();
-    }
+    block_sum256(red, term);
     if (threadIdx.x == 0) a.partial[blockIdx.x] = red[0];
     if (a.counter) {
         __shared__ int s_last;
@@ -1223,12 +1140,7 @@ __global__ void __launch_bounds__(256) combine_kernel(CombineArgs a) {
         __threadfence();
         double s = 0.0;
         for (int i = threadIdx.x; i < (int)gridDim.x; i += 256) s += __ldcg(a.partial + i);
-        red[threadIdx.x] = s;
-        __syncthreads();
-        for (int o = 128; o > 0; o >>= 1) {
-            if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
-            __syncthreads();
-        }
+        block_sum256(red, s);
         if (threadIdx.x == 0) {
             a.out[0] = __ldcg(a.flag) ? -INFINITY : red[0];
             *a.flag = 0;
@@ -1447,28 +1359,14 @@ __global__ void __launch_bounds__(256) class_merge_kernel(const double *gath, co
             w = 1.0; m = q[s]; e = (int)q[xs + s];
         }, emax);
         if (emax == INT_MIN) emax = 0;
-        double lnl;
-        if (sum > 0.0) lnl = log(sum) + (double)emax * 0.693147180559945309417232121458;
-        else if (sum != sum) lnl = sum;
-        else { lnl = -INFINITY; if (f > 0.0) atomicOr(flag, 1); }
+        const double lnl = pattern_lnl(sum, emax, [&] { if (f > 0.0) atomicOr(flag, 1); });
         term = (f > 0.0) ? f * lnl : 0.0;
         if (siteL && j == myShard && s < S) {
-            long long cnt = 0; double outL = sum;
-            if (sum > 0.0) {
-                const int e2 = emax;
-                cnt = (e2 < 0) ? (long long)((-e2) / 64) : -(long long)((e2 + 63) / 64);
-                const int rem = e2 + (int)(64 * cnt);
-                outL = sum * exp2i(rem);
-            }
-            siteL[s] = outL; siteScale[s] = cnt;
+            const SiteOut o = site_output(sum, emax);
+            siteL[s] = o.L; siteScale[s] = o.scale;
         }
     }
-    red[threadIdx.x] = term;
-    __syncthreads();
-    for (int o = 128; o > 0; o >>= 1) {
-        if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
-        __syncthreads();
-    }
+    block_sum256(red, term);
     if (threadIdx.x == 0) partial[blockIdx.x] = red[0];
 }
 
@@ -1581,10 +1479,7 @@ __global__ void __launch_bounds__(64) prune_batch_kernel(BatchPruneArgs a) {
             for (int o = 16; o > 0; o >>= 1) r += __shfl_xor_sync(0xffffffffu, r, o);
             if ((k & 31) == 0) red[k >> 5] = r;
             __syncthreads();
-            if (k == 0) {
-                const double L = red[0] + red[1];
-                a.out[s] = L > 0.0 ? log(L) + (double)ex * 0.693147180559945309417232121458 : (L != L ? L : -INFINITY);
-            }
+            if (k == 0) a.out[s] = pattern_lnl(red[0] + red[1], ex, [] {});
         }
     }
 }
@@ -1701,20 +1596,11 @@ __global__ void __launch_bounds__(256) class_exchange_kernel(ClassXchgArgs a) {
             w = 1.0; m = __ldcg(q + s); e = (int)__ldcg(q + xs + s);
         }, emax);
         if (emax == INT_MIN) emax = 0;
-        double lnl;
-        if (sum > 0.0) lnl = log(sum) + (double)emax * 0.693147180559945309417232121458;
-        else if (sum != sum) lnl = sum;
-        else { lnl = -INFINITY; if (f > 0.0) s_bad = 1; }
+        const double lnl = pattern_lnl(sum, emax, [&] { if (f > 0.0) s_bad = 1; });
         if (f > 0.0) term += f * lnl;
         if (a.siteL && j == a.myShard && s < a.S) {
-            long long cnt = 0; double outL = sum;
-            if (sum > 0.0) {
-                const int e2 = emax;
-                cnt = (e2 < 0) ? (long long)((-e2) / 64) : -(long long)((e2 + 63) / 64);
-                const int rem = e2 + (int)(64 * cnt);
-                outL = sum * exp2i(rem);
-            }
-            a.siteL[s] = outL; a.siteScale[s] = cnt;
+            const SiteOut o = site_output(sum, emax);
+            a.siteL[s] = o.L; a.siteScale[s] = o.scale;
         }
     }
     red[tid] = term;
@@ -1730,12 +1616,7 @@ __global__ void __launch_bounds__(256) final_sum_kernel(const double *partial, i
     __shared__ double red[256];
     double s = 0.0;
     for (int i = threadIdx.x; i < n; i += 256) s += partial[i];
-    red[threadIdx.x] = s;
-    __syncthreads();
-    for (int o = 128; o > 0; o >>= 1) {
-        if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
-        __syncthreads();
-    }
+    block_sum256(red, s);
     if (threadIdx.x == 0) out[0] = (*flag) ? -INFINITY : red[0];
 }
 
