@@ -177,6 +177,51 @@ int pad_states(int64_t D) {
     return -1;
 }
 
+// What a hand-over entry holds: a rate or a transition matrix (the ABI's HB2_MATRIX_* values), or a compiled template's
+// formula values.
+enum class Kind : signed char { Rate = HB2_MATRIX_RATE, Trans = HB2_MATRIX_TRANS, Compiled = 2 };
+
+// Input of one expm launch: its kind and, for compiled input, the template.
+struct Source {
+    Kind kind;
+    int tmpl = 0;
+};
+
+// Matrices handed over since the last flush: entries [0, n) are rows of `row` doubles (D*D matrix entries, or a template's
+// formula values), each with its destination slot (-1: retired) and kind.  The pinned rows and slots are uploaded at the
+// flush.
+struct HandoverQueue {
+    int64_t n = 0, cap = 0, row = 0;
+    PinnedBuffer<double> h_rows;
+    PinnedBuffer<int> h_dst;
+    DeviceBuffer<double> d_rows;
+    DeviceBuffer<int> d_dst;
+    std::vector<Kind> kind;
+    int alloc(int64_t cap_, int64_t row_) {
+        n = 0; cap = 0; row = row_;
+        kind.assign(cap_, Kind::Rate);
+        if (h_rows.alloc(cap_ * row_) || h_dst.alloc(cap_) || d_rows.alloc(cap_ * row_) || d_dst.alloc(cap_)) return 1;
+        cap = cap_;
+        return 0;
+    }
+};
+constexpr int DENSE_QUEUE = -1;               // queue id of the dense queue; a template's compiled queue has the template id
+
+// Where the resident copy of a slot's last matrix is kept (hb2_time_resident replays from it; the classification of the
+// shared-powers path compares against it).
+enum class Resident : signed char { None, DenseQ, Formula };   // none, dense Q in d_Qres, formula values in a template's d_Vres
+
+// One (class, branch) slot.  A slot handed over again before a flush overwrites its pending entry in place when the new one
+// joins the same queue and retires it otherwise (last one wins, like the reference's SetCompExp, calcnode.cpp:714), so one
+// expm launch never holds two CTAs with the same destination and the flush order of the queues cannot matter.
+struct Slot {
+    bool have = false;                        // a matrix was staged or launched (another class group's: handed over)
+    Resident res = Resident::None;
+    signed char res_tmpl = 0;                 // template whose d_Vres holds the formula values (res == Formula)
+    signed char queue = DENSE_QUEUE;          // queue of the pending entry
+    int entry = -1;                           // index of the pending entry in that queue, -1 none
+};
+
 }  // namespace
 
 struct hb2_partition {
@@ -189,31 +234,20 @@ struct hb2_partition {
     std::vector<std::vector<int>> children;   // per internal node, flat ids
     std::vector<int> height;                  // per internal node: 0 = only leaf children
     // device
-    DeviceBuffer<int> d_leaf, d_scal, d_rootE, d_child_start, d_child_ids, d_jobs, d_dst, d_flag;
-    DeviceBuffer<double> d_ambig, d_freq, d_cond, d_PT, d_Q, d_pi, d_rootL, d_weights, d_partial, d_lnL, d_siteL;
+    DeviceBuffer<int> d_leaf, d_scal, d_rootE, d_child_start, d_child_ids, d_jobs, d_flag;
+    DeviceBuffer<double> d_ambig, d_freq, d_cond, d_PT, d_pi, d_rootL, d_weights, d_partial, d_lnL, d_siteL;
     DeviceBuffer<long long> d_siteScale;
     // pinned host staging
-    PinnedBuffer<double> h_Q, h_small;        // h_small: pi (Dp) + weights (C) + lnL (1)
-    PinnedBuffer<int> h_jobs, h_dst;
-    // pending matrices: entries [0, n_pending) of h_Q / h_dst, with kinds
-    int64_t n_pending = 0;
-    std::vector<int> pending_kind;
-    // one pending entry per (class, node) slot across BOTH queues: >= 0 index into the dense queue, <= -2 -> index
-    // -(v+2) into the compiled queue, -1 none.  A slot handed over twice before an evaluation overwrites / retires its
-    // earlier entry (last one wins, like the reference's SetCompExp, calcnode.cpp:714), so one expm launch never holds
-    // two CTAs with the same destination and the flush order of the two queues cannot matter.
-    std::vector<int> pend_pos;
-    int64_t q_capacity = 0;                   // in matrices
-    std::vector<char> have_matrix;            // [C*B]
-    std::vector<char> is_rate;                // [C*B] slot holds a rate matrix resident in d_Qres (for hb2_time_resident)
+    PinnedBuffer<double> h_small;             // pi (Dp) + weights (C) + lnL (1)
+    PinnedBuffer<int> h_jobs;
+    HandoverQueue dense;                      // dense matrices, one per slot (its d_dst also carries hb2_time_resident's slots)
+    std::vector<Slot> slots;                  // [C*B]
     DeviceBuffer<double> d_Qres;              // [C][B][D*D] last rate matrices, resident copy
     // explicit-form mixtures (hb2_set_mixture_matrices): own staging so that nothing is shared with the plain queues
     DeviceBuffer<double> d_mix_scratch, d_mix_Q;   // [cap][Dp*Dp], [cap][D*D] | [cap] weights
     PinnedBuffer<double> h_mix;                    // as d_mix_Q, then 2 cap ints
     DeviceBuffer<int> d_mix_dst;
     int64_t mix_capacity = 0;
-    cudaEvent_t ev_mix = nullptr;
-    bool mix_busy = false;
     // shared-powers expm (64 padded states, hb2_kernels_fp64.cuh "Shared powers"): group = rate class (plain batches) or
     // C + mixture component; per-entry arrays are indexed like the batch
     struct ExBuf {
@@ -252,16 +286,14 @@ struct hb2_partition {
     // values.  A tree may carry several models (foreground / background branches, per-branch models of aBSREL): one
     // template each, up to HB2_MAX_TEMPLATES.
     struct Tmpl {
-        int64_t nnz = 0, nF = 0, n_pending = 0;
+        int64_t nnz = 0, nF = 0;
         bool has_colfreq = false;
-        DeviceBuffer<int> d_index, d_formula, d_vdst;
-        PinnedBuffer<int> h_vdst;
-        DeviceBuffer<double> d_colfreq, d_V, d_Vres;
-        PinnedBuffer<double> h_colfreq, h_V;
+        DeviceBuffer<int> d_index, d_formula;
+        DeviceBuffer<double> d_colfreq, d_Vres;
+        PinnedBuffer<double> h_colfreq;
+        HandoverQueue queue;
     };
     std::vector<Tmpl> tmpls;
-    std::vector<signed char> pend_tmpl;       // [C*B] template of the slot's pending compiled entry
-    std::vector<signed char> res_tmpl;        // [C*B] template of the slot's resident formula values (is_rate == 2)
     // tensor-core path (33..64 states unless HB2_FLAG_FORCE_FP64): fp32 conditionals + split/tiled P operands
     bool use_tc = false;
     DeviceBuffer<float> d_condf, d_PB, d_PTf;
@@ -308,13 +340,15 @@ struct hb2_partition {
     DeviceBuffer<double *> d_px_peer;
     DeviceBuffer<unsigned> d_px_counter;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
+    // recorded after uploads from pinned staging (the queues, ExBuf::h_int, column frequencies, mixtures, the replay's
+    // slots): every writer of those buffers waits for it first
     cudaEvent_t ev_staging = nullptr;
     bool staging_busy = false;
 };
 
 namespace {
 
-// The pinned staging buffers (both queues, h_dst/h_vdst included) may still be read by the H2D copies of the last flush.
+// The pinned staging buffers may still be read by the H2D copies enqueued before the last staged_uploads.
 int wait_staging(hb2_partition *p) {
     if (p->staging_busy) {
         CU(cudaEventSynchronize(p->ev_staging));
@@ -323,13 +357,22 @@ int wait_staging(hb2_partition *p) {
     return 0;
 }
 
+// Called after enqueueing uploads from pinned staging: the next writer waits for them.
+int staged_uploads(hb2_partition *p) {
+    CU(cudaEventRecord(p->ev_staging, p->stream));
+    p->staging_busy = true;
+    return 0;
+}
+
+HandoverQueue &queue_of(hb2_partition *p, int queue) { return queue == DENSE_QUEUE ? p->dense : p->tmpls[queue].queue; }
+
 // Host half of the shared-powers path for one batch: groups and references of the n entries (h_dst = their slots, < 0
 // retired; kind 1 = compiled hand-over, 2 = dense).  A group whose batch holds at least EX_MIN_GROUP live entries gets its
 // power table rebuilt from the first of them; smaller groups are compared with the direction the table was last built
-// from.  Fills the pinned arrays and enqueues their upload: call BEFORE ev_staging is recorded.
+// from.  Fills the pinned arrays and enqueues their upload: call BEFORE staged_uploads.
 struct SharedPlan {
     bool use = false;
-    int kind = 0, n_refs = 0, tmpl = 0;
+    int kind = 0, n_refs = 0;
     hb2_partition::ExBuf *x = nullptr;
 };
 constexpr int EX_MIN_GROUP = 24;
@@ -361,7 +404,7 @@ int plan_shared(hb2_partition *p, const int *h_dst, int64_t n, int kind, const i
     for (int64_t k = 0; k < n; k++) ref[k] = grp[k] >= 0 ? first[grp[k]] : -1;
     for (int r = 0; r < nr; r++) x.kind[grp[refs[r]]] = kind;
     CU(cudaMemcpyAsync(x.d_int, x.h_int, (size_t)(2 * x.cap + x.G) * sizeof(int), cudaMemcpyHostToDevice, p->stream));
-    sp.use = true; sp.kind = kind; sp.n_refs = nr; sp.tmpl = tmpl;
+    sp.use = true; sp.kind = kind; sp.n_refs = nr;
     return 0;
 }
 
@@ -376,52 +419,53 @@ int void_template_cache(hb2_partition *p, int tmpl) {
         CU(cudaMemsetAsync(p->ex.d_groups + g, 0, sizeof(hb2::ExpmGroup), p->stream));
         p->ex.kind[g] = 0;
     }
-    for (size_t k = 0; k < p->is_rate.size(); k++) if (p->is_rate[k] == 2 && p->res_tmpl[k] == tmpl) p->is_rate[k] = 0;
+    for (Slot &s : p->slots) if (s.res == Resident::Formula && s.res_tmpl == tmpl) s.res = Resident::None;
     return 0;
 }
 
-// One CTA per listed matrix.  is_trans: 0 rate matrices (exponentiated), 1 transition matrices (transposed/padded only),
-// 2 compiled template (dQ = formula values).  pt_override: write the results there instead of the P cache (mixture
-// components go to a scratch area first); pack_tc: also emit the tensor-path operands of the slot.  sp: shared-powers plan
-// of the WHOLE batch this run [off, off + n) belongs to (dQ / d_dst already point at the run).
-int launch_expm(hb2_partition *p, const double *dQ, const int *d_dst, int n, int is_trans, double *qres, bool pack_tc = true,
-                double *pt_override = nullptr, const SharedPlan *sp = nullptr, int64_t off = 0, int tmpl = 0) {
+// One CTA per listed matrix of `in` (rows of D*D matrix entries, or of the template's formula values).  The results go to
+// the P cache, with the tensor-path operands when use_tc, or, when scratch is given, to scratch alone (mixture components
+// and batched site sets).  keep_resident: leave the resident copy of each entry's rate matrix (dense Q, or formula values
+// on the shared-powers path), as a flushed hand-over does.  sp: shared-powers plan of the WHOLE batch this run
+// [off, off + n) belongs to (in / d_dst already point at the run).
+int launch_expm(hb2_partition *p, Source src, const double *in, const int *d_dst, int n, bool keep_resident, const SharedPlan &sp,
+                int64_t off = 0, double *scratch = nullptr) {
     if (n <= 0) return 0;
     hb2::ExpmArgs a{};
-    a.Q = dQ; a.dst = d_dst; a.PT = pt_override ? pt_override : p->d_PT; a.Qres = qres; a.D = (int)p->D;
-    a.is_trans = is_trans;
-    if (is_trans == 2) {                       // compiled template: dQ points at the formula values [n][nF]
-        const hb2_partition::Tmpl &t = p->tmpls[tmpl];
-        a.is_trans = 0; a.Q = nullptr; a.V = dQ; a.tmpl_index = t.d_index; a.tmpl_formula = t.d_formula;
-        a.tmpl_colfreq = t.has_colfreq ? t.d_colfreq : (double *)nullptr; a.tmpl_nnz = (int)t.nnz; a.nF = (int)t.nF;
+    a.Q = in; a.dst = d_dst; a.PT = scratch ? scratch : p->d_PT; a.D = (int)p->D;
+    a.Qres = keep_resident && src.kind != Kind::Trans ? (double *)p->d_Qres : nullptr;
+    a.is_trans = src.kind == Kind::Trans;
+    const hb2_partition::Tmpl *t = src.kind == Kind::Compiled ? &p->tmpls[src.tmpl] : nullptr;
+    if (t) {
+        a.Q = nullptr; a.V = in; a.tmpl_index = t->d_index; a.tmpl_formula = t->d_formula;
+        a.tmpl_colfreq = t->has_colfreq ? t->d_colfreq : (double *)nullptr; a.tmpl_nnz = (int)t->nnz; a.nF = (int)t->nF;
     }
-    pack_tc = pack_tc && p->use_tc && !pt_override;
     switch (p->Dp) {
         case 64: {
             const size_t smem = 3 * 64 * hb2::LD64 * sizeof(double);
             hb2::ExpmTcOut tc{nullptr, nullptr};
-            if (pack_tc) { tc.PB = p->d_PB; tc.PTf = p->d_PTf; }
-            if (sp && sp->use && is_trans != 1) {
-                hb2_partition::ExBuf &x = *sp->x;
-                const int nV = sp->kind == 1 ? (int)p->tmpls[tmpl].nF : (int)(p->D * p->D);
+            if (p->use_tc && !scratch) { tc.PB = p->d_PB; tc.PTf = p->d_PTf; }
+            if (sp.use && src.kind != Kind::Trans) {
+                hb2_partition::ExBuf &x = *sp.x;
+                const int nV = t ? (int)t->nF : (int)(p->D * p->D);
                 const hb2::ExpmGroup *groups = x.d_groups;
                 hb2::ExpmClassifyArgs ca{};
-                ca.V = dQ; ca.nV = nV; ca.kind = sp->kind; ca.dst = d_dst; ca.group = x.d_int + off;
+                ca.V = in; ca.nV = nV; ca.kind = sp.kind; ca.dst = d_dst; ca.group = x.d_int + off;
                 ca.ref = x.d_int + x.cap + off; ca.groups = groups; ca.refvec = x.d_refvec; ca.refvec_stride = x.stride;
                 ca.weight = x.d_weight + off; ca.flag = x.d_flag + off;
-                ca.res = pt_override ? nullptr : (sp->kind == 1 ? p->tmpls[tmpl].d_Vres : qres);   // scratch targets keep no resident copy
+                ca.res = !keep_resident ? nullptr : t ? (double *)t->d_Vres : (double *)p->d_Qres;
                 // references index the whole batch: classification has to see it in one piece (off == 0 for compiled batches
                 // and for dense batches that consist of a single run; mixed dense batches fall back below)
                 if (nV <= 256) hb2::expm_classify_warp_kernel<<<(n + 7) / 8, 256, 0, p->stream>>>(ca, n);
                 else hb2::expm_classify_kernel<<<n, 128, 0, p->stream>>>(ca);
                 a.group = ca.group; a.flag = ca.flag; a.weight = ca.weight; a.groups = groups; a.pow = x.d_pow;
                 a.Qres = nullptr;                    // the classification stage keeps the resident copy
-                if (sp->n_refs > 0) {
+                if (sp.n_refs > 0) {
                     hb2::ExpmPowersArgs pa{};
                     pa.a = a; pa.refs = x.d_int + 2 * x.cap; pa.groups = x.d_groups;
-                    pa.pow = x.d_pow; pa.refvec = x.d_refvec; pa.refvec_stride = x.stride; pa.nV = nV; pa.kind = sp->kind; pa.Vin = dQ;
+                    pa.pow = x.d_pow; pa.refvec = x.d_refvec; pa.refvec_stride = x.stride; pa.nV = nV; pa.kind = sp.kind; pa.Vin = in;
                     pa.flags = x.d_flags; pa.gen = ++x.gen; pa.err = p->d_err;
-                    hb2::expm_powers_kernel<<<dim3(hb2::EXPM_POW_TERMS - 1, (unsigned)sp->n_refs), 256, smem, p->stream>>>(pa);
+                    hb2::expm_powers_kernel<<<dim3(hb2::EXPM_POW_TERMS - 1, (unsigned)sp.n_refs), 256, smem, p->stream>>>(pa);
                     p->launches++;
                 }
                 double *colsum = x.d_colsum + (size_t)off * 16 * 64;
@@ -444,108 +488,117 @@ int launch_expm(hb2_partition *p, const double *dQ, const int *d_dst, int n, int
     return 0;
 }
 
-// Flush matrices handed over since the last evaluation: one H2D copy + one (or two) expm launches per queue.  Retired
-// entries (destination -1: the slot was handed over again later) are skipped by the kernels.
-int flush_compiled(hb2_partition *p) {
-    for (size_t ti = 0; ti < p->tmpls.size(); ti++) {
-        hb2_partition::Tmpl &t = p->tmpls[ti];
-        const int64_t n = t.n_pending;
-        if (n == 0) continue;
-        CU(cudaMemcpyAsync(t.d_V, t.h_V, n * t.nF * sizeof(double), cudaMemcpyHostToDevice, p->stream));
-        CU(cudaMemcpyAsync(t.d_vdst, t.h_vdst, n * sizeof(int), cudaMemcpyHostToDevice, p->stream));
-        SharedPlan sp;
-        if (plan_shared(p, t.h_vdst, n, 1, nullptr, sp, (int)ti)) return 1;
-        CU(cudaEventRecord(p->ev_staging, p->stream));
-        p->staging_busy = true;
-        if (launch_expm(p, t.d_V, t.d_vdst, (int)n, 2, sp.use ? nullptr : (double *)p->d_Qres, true, nullptr, &sp, 0, (int)ti)) return 1;
-        for (int64_t k = 0; k < n; k++)
-            if (t.h_vdst[k] >= 0) { p->is_rate[t.h_vdst[k]] = sp.use ? 2 : 1; p->res_tmpl[t.h_vdst[k]] = (signed char)ti; p->pend_pos[t.h_vdst[k]] = -1; }
-        t.n_pending = 0;
-    }
-    return 0;
-}
-
-int flush_matrices(hb2_partition *p) {
-    if (flush_compiled(p)) return 1;
-    const int64_t n = p->n_pending;
+// Uploads a queue and exponentiates its entries, one launch per run of equal kind.  Retired entries (destination -1) are
+// skipped by the kernels.  Shared powers apply only when the queue holds no transition matrix.  Each entry leaves its
+// slot's resident copy: formula values for a compiled entry on shared powers, none for a transition matrix, dense Q
+// otherwise.
+int flush_queue(hb2_partition *p, int queue) {
+    HandoverQueue &q = queue_of(p, queue);
+    const int64_t n = q.n;
     if (n == 0) return 0;
-    const size_t dd = (size_t)p->D * p->D;
-    CU(cudaMemcpyAsync(p->d_Q, p->h_Q, n * dd * sizeof(double), cudaMemcpyHostToDevice, p->stream));
-    CU(cudaMemcpyAsync(p->d_dst, p->h_dst, n * sizeof(int), cudaMemcpyHostToDevice, p->stream));
-    SharedPlan sp;                           // shared powers only for batches that are one run of rate matrices
-    {
-        bool all_rate = true;
-        for (int64_t k = 0; k < n; k++) all_rate = all_rate && p->pending_kind[k] == HB2_MATRIX_RATE;
-        if (all_rate && plan_shared(p, p->h_dst, n, 2, nullptr, sp)) return 1;
+    const int tmpl = std::max(queue, 0);
+    CU(cudaMemcpyAsync(q.d_rows, q.h_rows, n * q.row * sizeof(double), cudaMemcpyHostToDevice, p->stream));
+    CU(cudaMemcpyAsync(q.d_dst, q.h_dst, n * sizeof(int), cudaMemcpyHostToDevice, p->stream));
+    SharedPlan sp;
+    const bool any_trans = std::find(q.kind.begin(), q.kind.begin() + n, Kind::Trans) != q.kind.begin() + n;
+    if (!any_trans && plan_shared(p, q.h_dst, n, queue == DENSE_QUEUE ? 2 : 1, nullptr, sp, tmpl)) return 1;
+    if (staged_uploads(p)) return 1;
+    for (int64_t i = 0, j; i < n; i = j) {
+        for (j = i + 1; j < n && q.kind[j] == q.kind[i]; j++) {}
+        if (launch_expm(p, {q.kind[i], tmpl}, q.d_rows + i * q.row, q.d_dst + i, (int)(j - i), true, sp, i)) return 1;
     }
-    // the pinned staging buffers are reused by the next hb2_set_matrices: it waits on this event (copies only)
-    CU(cudaEventRecord(p->ev_staging, p->stream));
-    p->staging_busy = true;
-    // pending entries are grouped by kind in runs; one launch per run.  Rate matrices also leave a resident copy
-    // in d_Qres (written by the kernel while it loads them) so a whole evaluation can be replayed on device.
-    int64_t i = 0;
-    while (i < n) {
-        int64_t j = i;
-        while (j < n && p->pending_kind[j] == p->pending_kind[i]) j++;
-        const int is_trans = p->pending_kind[i] == HB2_MATRIX_TRANS;
-        if (launch_expm(p, p->d_Q + i * dd, p->d_dst + i, (int)(j - i), is_trans, is_trans ? nullptr : (double *)p->d_Qres, true, nullptr, &sp, i)) return 1;
-        i = j;
+    for (int64_t k = 0; k < n; k++) {
+        if (q.h_dst[k] < 0) continue;
+        Slot &s = p->slots[q.h_dst[k]];
+        s.entry = -1;
+        s.res = q.kind[k] == Kind::Trans ? Resident::None : q.kind[k] == Kind::Compiled && sp.use ? Resident::Formula : Resident::DenseQ;
+        s.res_tmpl = (signed char)tmpl;
     }
-    for (int64_t k = 0; k < n; k++)
-        if (p->h_dst[k] >= 0) { p->is_rate[p->h_dst[k]] = (p->pending_kind[k] == HB2_MATRIX_RATE); p->pend_pos[p->h_dst[k]] = -1; }
-    p->n_pending = 0;
-    p->pending_kind.clear();
+    q.n = 0;
     return 0;
 }
 
-// A matrix of `node` is about to change: the single-branch cache (if any) only survives changes of ITS branch.
-inline void note_matrix_change(hb2_partition *p, int64_t node) {
-    if (p->bc_node >= 0 && node != p->bc_node && p->bc_dirty_node < 0) p->bc_dirty_node = node;
+// Flush the compiled queues in ascending template id: one H2D copy and one expm launch sequence each.
+int flush_compiled(hb2_partition *p) {
+    for (size_t t = 0; t < p->tmpls.size(); t++)
+        if (flush_queue(p, (int)t)) return 1;
+    return 0;
 }
 
-// Retire the pending entry of `slot` if it sits in ANOTHER queue than the one it is about to join (tmpl < 0: the dense
-// queue; >= 0: that template's compiled queue).  Returns the index of an entry of the SAME queue that can be overwritten
-// in place, or -1.
-int64_t claim_slot(hb2_partition *p, int64_t slot, int tmpl) {
-    const int pos = p->pend_pos[slot];
-    if (pos == -1) return -1;
-    if (pos >= 0) {                            // pending in the dense queue
-        if (tmpl < 0) return pos;
-        p->h_dst[pos] = -1;
-    } else {                                   // pending in a compiled queue
-        const int pt = p->pend_tmpl[slot];
-        if (pt == tmpl) return -(int64_t)pos - 2;
-        p->tmpls[pt].h_vdst[-(int64_t)pos - 2] = -1;
-    }
-    p->pend_pos[slot] = -1;
-    return -1;
+// Flush everything handed over since the last evaluation: the compiled queues, then the dense queue.
+int flush_matrices(hb2_partition *p) {
+    return flush_compiled(p) || flush_queue(p, DENSE_QUEUE);
 }
 
-int stage_matrix(hb2_partition *p, int64_t cat, int64_t node, const double *M, int kind) {
+// Checks a hand-over of n matrices of class `cat` (-1 means 0) as a whole before anything changes: the class, every node
+// id and, where the entry point has them, the kind and the matrix pointers.  A refused hand-over changes nothing.  An
+// accepted one is noted for the branch cache; `stage` is false for another class group's class, whose slots are marked
+// here since nothing is staged for them.
+int accept_handover(hb2_partition *p, int64_t &cat, int64_t n, const int64_t *nodeIds, bool &stage, int kind = HB2_MATRIX_RATE,
+                    const double *const *M = nullptr) {
     if (cat < 0) cat = 0;
     if (cat >= p->C) return fail("rate class %lld out of range (C=%lld)", (long long)cat, (long long)p->C);
-    if (node < 0 || node >= p->B) return fail("node id %lld has no branch (valid 0..%lld)", (long long)node, (long long)p->B - 1);
+    for (int64_t k = 0; k < n; k++)
+        if (nodeIds[k] < 0 || nodeIds[k] >= p->B)
+            return fail("node id %lld has no branch (valid 0..%lld)", (long long)nodeIds[k], (long long)p->B - 1);
     if (kind != HB2_MATRIX_RATE && kind != HB2_MATRIX_TRANS) return fail("unknown matrix kind %d", kind);
-    note_matrix_change(p, node);
-    if (cat < p->own0 || cat >= p->own0 + p->ownN) { p->have_matrix[cat * p->B + node] = 1; return 0; }   // another class group's
-    if (wait_staging(p)) return 1;            // previous flush's H2D copies must have left the pinned buffers
-    const int64_t slot = cat * p->B + node;
-    int64_t at = claim_slot(p, slot, -1);
-    if (at < 0) {
-        if (p->n_pending == p->q_capacity) {
-            cudaSetDevice(p->device);
-            if (flush_matrices(p) || wait_staging(p)) return 1;
-        }
-        at = p->n_pending++;
-        p->pending_kind.push_back(kind);
-        p->pend_pos[slot] = (int)at;
-    }
-    const size_t dd = (size_t)p->D * p->D;
-    memcpy(p->h_Q + at * dd, M, dd * sizeof(double));
-    p->h_dst[at] = (int)slot;
-    p->pending_kind[at] = kind;
-    p->have_matrix[slot] = 1;
+    for (int64_t k = 0; M && k < n; k++)
+        if (!M[k]) return fail("matrix %lld is null", (long long)k);
+    // the single-branch cache (if any) only survives changes of ITS branch
+    for (int64_t k = 0; k < n && p->bc_node >= 0 && p->bc_dirty_node < 0; k++)
+        if (nodeIds[k] != p->bc_node) p->bc_dirty_node = nodeIds[k];
+    stage = cat >= p->own0 && cat < p->own0 + p->ownN;
+    if (!stage) for (int64_t k = 0; k < n; k++) p->slots[cat * p->B + nodeIds[k]].have = true;
     return 0;
+}
+
+// Stages one row for `slot` in a queue (DENSE_QUEUE or a template id).  The slot's pending entry is overwritten when it
+// sits in the same queue and retired otherwise.  A full compiled queue flushes the compiled queues; a full dense queue
+// flushes everything.
+int enqueue(hb2_partition *p, int queue, int64_t slot, const double *row, Kind kind) {
+    if (wait_staging(p)) return 1;            // the last flush's H2D copies must have left the pinned buffers
+    HandoverQueue &q = queue_of(p, queue);
+    Slot &s = p->slots[slot];
+    if (s.entry >= 0 && s.queue != queue) {
+        queue_of(p, s.queue).h_dst[s.entry] = -1;
+        s.entry = -1;
+    }
+    if (s.entry < 0) {
+        if (q.n == q.cap) {
+            cudaSetDevice(p->device);
+            if ((queue == DENSE_QUEUE ? flush_matrices(p) : flush_compiled(p)) || wait_staging(p)) return 1;
+        }
+        s.queue = (signed char)queue;
+        s.entry = (int)q.n++;
+    }
+    memcpy(q.h_rows + s.entry * q.row, row, q.row * sizeof(double));
+    q.h_dst[s.entry] = (int)slot;
+    q.kind[s.entry] = kind;
+    s.have = true;
+    return 0;
+}
+
+// Stages the root vector, zero-padded to Dp (unless null), and the first nw class weights (when given).  Every caller
+// synchronises the stream before it returns, so h_small is free again at the next call.
+int stage_root(hb2_partition *p, const double *rootFreqs, const double *weights = nullptr, int nw = 0) {
+    double *hs = p->h_small;
+    if (rootFreqs) {
+        for (int k = 0; k < p->Dp; k++) hs[k] = k < p->D ? rootFreqs[k] : 0.0;
+        CU(cudaMemcpyAsync(p->d_pi, hs, p->Dp * sizeof(double), cudaMemcpyHostToDevice, p->stream));
+    }
+    if (weights) {
+        for (int c = 0; c < nw; c++) hs[p->Dp + c] = weights[c];
+        CU(cudaMemcpyAsync(p->d_weights, hs + p->Dp, nw * sizeof(double), cudaMemcpyHostToDevice, p->stream));
+    }
+    return 0;
+}
+
+// Stages a template's column frequencies through its pinned buffer, so that the caller may reuse colFreq at once.
+int stage_colfreq(hb2_partition *p, hb2_partition::Tmpl &t, const double *colFreq) {
+    if (wait_staging(p)) return 1;
+    memcpy(t.h_colfreq, colFreq, p->D * sizeof(double));
+    CU(cudaMemcpyAsync(t.d_colfreq, t.h_colfreq, p->D * sizeof(double), cudaMemcpyHostToDevice, p->stream));
+    return staged_uploads(p);
 }
 
 // Checks a flat parent list (leaves 0..L-1, then the internal nodes in post-order, the root last with parent -1) and
@@ -1090,7 +1143,7 @@ int run_root(hb2_partition *p, int c0, int nc, bool use_weights, bool want_sites
 int check_ready(hb2_partition *p, int c0, int nc) {
     for (int c = c0; c < c0 + nc; c++)
         for (int64_t b = 0; b < p->B; b++)
-            if (!p->have_matrix[c * p->B + b])
+            if (!p->slots[c * p->B + b].have)
                 return fail("no matrix was ever set for rate class %d, node %lld", c, (long long)b);
     return 0;
 }
@@ -1131,12 +1184,8 @@ int evaluate_impl(hb2_partition *p, int c0, int nc, const double *weights, int64
         std::fill(p->evaluated_cat.begin(), p->evaluated_cat.end(), 0);
         p->walk_reset = false;
     }
-    // small inputs: pi (padded) and class weights
+    if (stage_root(p, rootFreqs, weights, nw)) return 1;
     double *hs = p->h_small;
-    for (int k = 0; k < p->Dp; k++) hs[k] = k < p->D ? rootFreqs[k] : 0.0;
-    if (weights) for (int c = 0; c < nw; c++) hs[p->Dp + c] = weights[c];
-    CU(cudaMemcpyAsync(p->d_pi, hs, p->Dp * sizeof(double), cudaMemcpyHostToDevice, p->stream));
-    if (weights) CU(cudaMemcpyAsync(p->d_weights, hs + p->Dp, nw * sizeof(double), cudaMemcpyHostToDevice, p->stream));
     // classes never pruned before need the whole tree regardless of updateNodes (likefunc.cpp:10965-10967)
     bool all = (updateNodes == nullptr || nUpdate < 0);
     for (int c = c0; c < c0 + nc; c++) if (!p->evaluated_cat[c]) all = true;
@@ -1239,7 +1288,6 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
     CU(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
     for (auto &e : p->ev) CU(cudaEventCreate(&e));
     CU(cudaEventCreateWithFlags(&p->ev_staging, cudaEventDisableTiming));
-    CU(cudaEventCreateWithFlags(&p->ev_mix, cudaEventDisableTiming));
     const size_t Sp = p->Sp, dpdp = (size_t)Dp * Dp, dd = (size_t)D * D;
     cudaStream_t st = p->stream;
     if (p->d_leaf.alloc(L * Sp) || p->d_ambig.alloc(std::max<int64_t>(nAmb, 1) * Dp) || p->d_freq.alloc(Sp)) return 1;
@@ -1274,16 +1322,15 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
     }
     if (p->d_err.alloc(1) || p->d_err.zero(st)) return 1;
     if (p->d_scal.alloc((size_t)C * 2 * I * Sp) || p->d_PT.alloc((size_t)C * p->B * dpdp) || p->d_Qres.alloc((size_t)C * p->B * dd)) return 1;   // 2I: see d_condf
-    p->q_capacity = C * p->B;
-    if (p->d_Q.alloc((size_t)p->q_capacity * dd) || p->d_dst.alloc(p->q_capacity) || p->d_pi.alloc(Dp) || p->d_rootL.alloc((size_t)C * Sp) ||
-        p->d_rootE.alloc((size_t)C * Sp) || p->d_weights.alloc(C))
+    if (p->dense.alloc(C * p->B, dd) || p->d_pi.alloc(Dp) || p->d_rootL.alloc((size_t)C * Sp) || p->d_rootE.alloc((size_t)C * Sp) ||
+        p->d_weights.alloc(C))
         return 1;
     p->n_partial_blocks = (int)((S + 255) / 256);
     if (p->d_partial.alloc(p->n_partial_blocks) || p->d_lnL.alloc(1) || p->d_flag.alloc(1) || p->d_flag.zero(st) || p->d_root_counter.alloc(1) ||
         p->d_root_counter.zero(st))
         return 1;
     if (p->d_siteL.alloc(Sp) || p->d_siteScale.alloc(Sp) || p->d_jobs.alloc(I) || p->d_child_start.alloc(I + 1) || p->d_child_ids.alloc(L + I)) return 1;
-    if (p->h_Q.alloc((size_t)p->q_capacity * dd) || p->h_dst.alloc(p->q_capacity) || p->h_small.alloc(Dp + C + 8) || p->h_jobs.alloc(I)) return 1;
+    if (p->h_small.alloc(Dp + C + 8) || p->h_jobs.alloc(I)) return 1;
     if (p->d_scal.zero(st) || p->d_PT.zero(st) || p->d_rootL.zero(st) || p->d_rootE.zero(st)) return 1;
     {   // static uploads (pageable host vectors: released once the copies are enqueued)
         std::vector<int> leaf((size_t)L * Sp, 0);          // padding patterns: state 0 everywhere, frequency 0
@@ -1319,51 +1366,40 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
         p->small_resident[0] = std::max(b1, 1) * p->sm_count;
         p->small_resident[1] = std::max(b2, 1) * p->sm_count;
     }
-    p->have_matrix.assign(C * p->B, 0);
-    p->is_rate.assign(C * p->B, 0);
-    p->pend_pos.assign(C * p->B, -1);
-    p->pend_tmpl.assign(C * p->B, 0);
-    p->res_tmpl.assign(C * p->B, 0);
+    p->slots.assign(C * p->B, Slot());
     p->evaluated_cat.assign(C, 0);
     p->own0 = 0; p->ownN = (int)C;
     *out = p.release();
     return 0;
 }
 
-int hb2_set_matrices(hb2_partition *p, int64_t cat, int64_t n, const int64_t *nodeIds, const double *const *M, int kind) {
+// Body of both dense entry points: matrix k is at M[k] (pointer array) or at packed + k*D*D.
+static int set_dense(hb2_partition *p, int64_t cat, int64_t n, const int64_t *nodeIds, const double *const *M, const double *packed, int kind) {
     if (!p) return fail("null partition");
-    if (n < 0 || (n > 0 && (!nodeIds || !M))) return fail("bad matrix list");
-    for (int64_t k = 0; k < n; k++) {
-        if (!M[k]) return fail("matrix %lld is null", (long long)k);
-        if (stage_matrix(p, cat, nodeIds[k], M[k], kind)) return 1;
-    }
+    if (n < 0 || (n > 0 && (!nodeIds || !(M || packed)))) return fail("bad matrix list");
+    bool stage;
+    if (accept_handover(p, cat, n, nodeIds, stage, kind, M)) return 1;
+    const size_t dd = (size_t)p->D * p->D;
+    for (int64_t k = 0; stage && k < n; k++)
+        if (enqueue(p, DENSE_QUEUE, cat * p->B + nodeIds[k], M ? M[k] : packed + k * dd, (Kind)kind)) return 1;
     return 0;
 }
 
+int hb2_set_matrices(hb2_partition *p, int64_t cat, int64_t n, const int64_t *nodeIds, const double *const *M, int kind) {
+    return set_dense(p, cat, n, nodeIds, M, nullptr, kind);
+}
+
 int hb2_set_matrices_packed(hb2_partition *p, int64_t cat, int64_t n, const int64_t *nodeIds, const double *M, int kind) {
-    if (!p) return fail("null partition");
-    if (n < 0 || (n > 0 && (!nodeIds || !M))) return fail("bad matrix list");
-    const size_t dd = (size_t)p->D * p->D;
-    for (int64_t k = 0; k < n; k++)
-        if (stage_matrix(p, cat, nodeIds[k], M + k * dd, kind)) return 1;
-    return 0;
+    return set_dense(p, cat, n, nodeIds, nullptr, M, kind);
 }
 
 int hb2_set_mixture_matrices(hb2_partition *p, int64_t cat, int64_t n, const int64_t *nodeIds, int64_t K, const double *M,
                              const double *w) {
     if (!p) return fail("null partition");
     if (n < 0 || K < 1 || (n > 0 && (!nodeIds || !M || !w))) return fail("bad mixture arguments");
-    if (cat < 0) cat = 0;
-    if (cat >= p->C) return fail("rate class %lld out of range", (long long)cat);
-    for (int64_t i = 0; i < n; i++) {
-        if (nodeIds[i] < 0 || nodeIds[i] >= p->B) return fail("node id %lld has no branch", (long long)nodeIds[i]);
-        note_matrix_change(p, nodeIds[i]);
-    }
-    if (cat < p->own0 || cat >= p->own0 + p->ownN) {       // another class group's
-        for (int64_t i = 0; i < n; i++) p->have_matrix[cat * p->B + nodeIds[i]] = 1;
-        return 0;
-    }
-    if (n == 0) return 0;
+    bool stage;
+    if (accept_handover(p, cat, n, nodeIds, stage)) return 1;
+    if (!stage || n == 0) return 0;
     CU(cudaSetDevice(p->device));
     if (flush_matrices(p)) return 1;         // keep ordering with plain matrices staged earlier (same stream)
     // Two launches, no host synchronisation: all n*K components are exponentiated side by side into a scratch area
@@ -1371,7 +1407,7 @@ int hb2_set_mixture_matrices(hb2_partition *p, int64_t cat, int64_t n, const int
     // tensor-path operands.  Own pinned staging: [n*K matrices | n*K weights], then the n destination slots as ints.
     const size_t dd = (size_t)p->D * p->D, dpdp = (size_t)p->Dp * p->Dp;
     const int64_t nk = n * K;
-    if (p->mix_busy) { CU(cudaEventSynchronize(p->ev_mix)); p->mix_busy = false; }
+    if (wait_staging(p)) return 1;
     if (nk > p->mix_capacity) {
         CU(cudaStreamSynchronize(p->stream));
         p->mix_capacity = 0;
@@ -1387,25 +1423,25 @@ int hb2_set_mixture_matrices(hb2_partition *p, int64_t cat, int64_t n, const int
     for (int64_t i = 0; i < n; i++) h_idx[nk + i] = (int)(cat * p->B + nodeIds[i]);
     CU(cudaMemcpyAsync(p->d_mix_Q, p->h_mix, (size_t)nk * (dd + 1) * sizeof(double), cudaMemcpyHostToDevice, p->stream));
     CU(cudaMemcpyAsync(p->d_mix_dst, h_idx, (size_t)(nk + n) * sizeof(int), cudaMemcpyHostToDevice, p->stream));
-    CU(cudaEventRecord(p->ev_mix, p->stream));
-    p->mix_busy = true;
     // component k of every node is (in BS-REL / BUSTED models) the same rate matrix up to the branch length: the components
     // form shared-powers groups C + k
     SharedPlan sp;
     if (K <= 8) {
-        if (wait_staging(p)) return 1;
         std::vector<int> grp(nk);
         for (int64_t k = 0; k < nk; k++) grp[k] = (int)(p->C + k % K);
         if (plan_shared(p, h_idx, nk, 2, grp.data(), sp)) return 1;
-        CU(cudaEventRecord(p->ev_staging, p->stream));
-        p->staging_busy = true;
     }
-    if (launch_expm(p, p->d_mix_Q, p->d_mix_dst, (int)nk, 0, nullptr, false, p->d_mix_scratch, &sp)) return 1;
+    if (staged_uploads(p)) return 1;
+    if (launch_expm(p, {Kind::Rate}, p->d_mix_Q, p->d_mix_dst, (int)nk, false, sp, 0, p->d_mix_scratch)) return 1;
     hb2::mix_reduce_kernel<<<(unsigned)n, 256, 0, p->stream>>>(p->d_mix_scratch, p->d_mix_Q + (size_t)nk * dd, p->d_mix_dst + nk, (int)K, p->Dp,
                                                               p->d_PT, p->use_tc ? p->d_PB : (float *)nullptr, p->d_PTf);
     p->launches++;
     CU(cudaGetLastError());
-    for (int64_t i = 0; i < n; i++) { p->have_matrix[cat * p->B + nodeIds[i]] = 1; p->is_rate[cat * p->B + nodeIds[i]] = 0; }
+    for (int64_t i = 0; i < n; i++) {
+        Slot &s = p->slots[cat * p->B + nodeIds[i]];
+        s.have = true;
+        s.res = Resident::None;
+    }
     return 0;
 }
 
@@ -1416,8 +1452,7 @@ int hb2_set_rate_template_id(hb2_partition *p, int64_t templateId, int64_t nnz, 
     if (nnz < 1 || nFormulas < 1 || !entryIndex || !entryFormula) return fail("bad template arguments");
     CU(cudaSetDevice(p->device));
     if (flush_matrices(p)) return 1;
-    CU(cudaStreamSynchronize(p->stream));
-    p->staging_busy = false;
+    CU(cudaStreamSynchronize(p->stream));     // the template's buffers are about to be re-allocated
     std::vector<int> idx(nnz), frm(nnz);
     for (int64_t e = 0; e < nnz; e++) {
         if (entryIndex[e] < 0 || entryIndex[e] >= p->D * p->D) return fail("template entry %lld: index %lld out of range", (long long)e, (long long)entryIndex[e]);
@@ -1428,22 +1463,16 @@ int hb2_set_rate_template_id(hb2_partition *p, int64_t templateId, int64_t nnz, 
     hb2_partition::Tmpl &t = p->tmpls[templateId];
     t = hb2_partition::Tmpl();                // undefined until every buffer is in place
     if (t.d_index.alloc(nnz) || t.d_formula.alloc(nnz) || t.d_colfreq.alloc(p->D) || t.h_colfreq.alloc(p->D) ||
-        t.d_V.alloc((size_t)p->q_capacity * nFormulas) || t.d_vdst.alloc(p->q_capacity))
+        t.queue.alloc(p->C * p->B, nFormulas))
         return 1;
     // resident formula values of every slot (replay, shared-powers classification); cached directions of this template's
     // groups are void now
     if (t.d_Vres.alloc((size_t)p->C * p->B * nFormulas) || void_template_cache(p, (int)templateId)) return 1;
-    if (t.h_V.alloc((size_t)p->q_capacity * nFormulas) || t.h_vdst.alloc(p->q_capacity)) return 1;
     CU(cudaMemcpyAsync(t.d_index, idx.data(), nnz * sizeof(int), cudaMemcpyHostToDevice, p->stream));
     CU(cudaMemcpyAsync(t.d_formula, frm.data(), nnz * sizeof(int), cudaMemcpyHostToDevice, p->stream));
     t.has_colfreq = colFreq != nullptr;
-    if (colFreq) {                            // staged, so that the caller may reuse colFreq at once even if it is pinned
-        memcpy(t.h_colfreq, colFreq, p->D * sizeof(double));
-        CU(cudaMemcpyAsync(t.d_colfreq, t.h_colfreq, p->D * sizeof(double), cudaMemcpyHostToDevice, p->stream));
-        CU(cudaEventRecord(p->ev_staging, p->stream));
-        p->staging_busy = true;
-    }
-    t.nnz = nnz; t.nF = nFormulas; t.n_pending = 0;
+    if (colFreq && stage_colfreq(p, t, colFreq)) return 1;
+    t.nnz = nnz; t.nF = nFormulas;
     return 0;
 }
 
@@ -1459,11 +1488,7 @@ int hb2_set_template_frequencies(hb2_partition *p, int64_t templateId, const dou
     if (!t.has_colfreq) return fail("template %lld was defined without column frequencies", (long long)templateId);
     CU(cudaSetDevice(p->device));
     if (flush_matrices(p)) return 1;          // matrices handed over so far were assembled with the old frequencies
-    if (wait_staging(p)) return 1;
-    memcpy(t.h_colfreq, colFreq, p->D * sizeof(double));
-    CU(cudaMemcpyAsync(t.d_colfreq, t.h_colfreq, p->D * sizeof(double), cudaMemcpyHostToDevice, p->stream));
-    CU(cudaEventRecord(p->ev_staging, p->stream));
-    p->staging_busy = true;
+    if (stage_colfreq(p, t, colFreq)) return 1;
     return void_template_cache(p, (int)templateId);
 }
 
@@ -1471,30 +1496,11 @@ int hb2_set_matrices_compiled_id(hb2_partition *p, int64_t templateId, int64_t c
     if (!p) return fail("null partition");
     if (templateId < 0 || templateId >= (int64_t)p->tmpls.size() || p->tmpls[templateId].nnz == 0) return fail("hb2_set_rate_template has not been called (template %lld)", (long long)templateId);
     if (n < 0 || (n > 0 && (!nodeIds || !formulaValues))) return fail("bad compiled matrix list");
-    if (cat < 0) cat = 0;
-    if (cat >= p->C) return fail("rate class %lld out of range (C=%lld)", (long long)cat, (long long)p->C);
-    hb2_partition::Tmpl &t = p->tmpls[templateId];
-    const bool owned = cat >= p->own0 && cat < p->own0 + p->ownN;
-    for (int64_t k = 0; k < n; k++) {
-        if (nodeIds[k] < 0 || nodeIds[k] >= p->B) return fail("node id %lld has no branch", (long long)nodeIds[k]);
-        p->have_matrix[cat * p->B + nodeIds[k]] = 1;
-        note_matrix_change(p, nodeIds[k]);
-    }
-    if (!owned) return 0;                                   // another class group's matrices
-    if (wait_staging(p)) return 1;
-    const size_t row = (size_t)t.nF * sizeof(double);
-    for (int64_t k = 0; k < n; k++) {
-        const int64_t slot = cat * p->B + nodeIds[k];
-        int64_t at = claim_slot(p, slot, (int)templateId);
-        if (at < 0) {
-            if (t.n_pending == p->q_capacity) { cudaSetDevice(p->device); if (flush_compiled(p) || wait_staging(p)) return 1; }
-            at = t.n_pending++;
-            p->pend_pos[slot] = (int)(-at - 2);
-            p->pend_tmpl[slot] = (signed char)templateId;
-        }
-        memcpy(t.h_V + at * t.nF, formulaValues + k * t.nF, row);
-        t.h_vdst[at] = (int)slot;
-    }
+    bool stage;
+    if (accept_handover(p, cat, n, nodeIds, stage)) return 1;
+    const int64_t nF = p->tmpls[templateId].nF;
+    for (int64_t k = 0; stage && k < n; k++)
+        if (enqueue(p, (int)templateId, cat * p->B + nodeIds[k], formulaValues + k * nF, Kind::Compiled)) return 1;
     return 0;
 }
 
@@ -1577,10 +1583,8 @@ static int batch_sites(hb2_partition *p, int64_t templateId, int64_t nSets, cons
             return 1;
         p->b_cap = cap; p->b_groups_per_set = gk; p->b_vcap = ne * nF;
     }
-    double *hs = p->h_small;
     CU(cudaStreamSynchronize(p->stream));
-    for (int k = 0; k < p->Dp; k++) hs[k] = k < p->D ? rootFreqs[k] : 0.0;
-    CU(cudaMemcpyAsync(p->d_pi, hs, p->Dp * sizeof(double), cudaMemcpyHostToDevice, p->stream));
+    if (stage_root(p, rootFreqs)) return 1;
     if (mix) CU(cudaMemcpyAsync(p->d_brow, row_off.data(), (size_t)(B + 1) * sizeof(int), cudaMemcpyHostToDevice, p->stream));
     std::vector<int> grp;
     for (int64_t s0 = 0; s0 < nSets; s0 += p->b_cap) {
@@ -1602,11 +1606,9 @@ static int batch_sites(hb2_partition *p, int64_t templateId, int64_t nSets, cons
         // an earlier chunk or call, whose table may come from another template or other column frequencies
         std::fill(p->bex.kind.begin(), p->bex.kind.end(), 0);
         CU(cudaMemsetAsync(p->bex.d_groups, 0, (size_t)p->bex.G * sizeof(hb2::ExpmGroup), p->stream));
-        if (plan_shared(p, p->h_bdst, ne, 1, grp.data(), sp, (int)templateId, &p->bex, 4)) return 1;
-        CU(cudaEventRecord(p->ev_staging, p->stream));
-        p->staging_busy = true;
-        // classification writes its "resident copy" of the formula values in place (res = input) -- harmless
-        if (launch_expm(p, p->d_bV, p->d_bdst, (int)ne, 2, nullptr, false, p->d_bPT, &sp, 0, (int)templateId)) return 1;
+        if (plan_shared(p, p->h_bdst, ne, 1, grp.data(), sp, (int)templateId, &p->bex, 4) || staged_uploads(p)) return 1;
+        // the chunk's P area is scratch: no resident copy is kept
+        if (launch_expm(p, {Kind::Compiled, (int)templateId}, p->d_bV, p->d_bdst, (int)ne, false, sp, 0, p->d_bPT)) return 1;
         hb2::BatchPruneArgs ba;
         ba.PT = p->d_bPT; ba.cond = p->d_bcond; ba.node_ex = p->d_bnodeex; ba.pat = p->d_bpat; ba.leaf = p->d_leaf; ba.ambig = p->d_ambig; ba.pi = p->d_pi;
         ba.tree.child_start = p->d_child_start; ba.tree.child_ids = p->d_child_ids; ba.out = p->d_bout;
@@ -1704,9 +1706,7 @@ int hb2_branch_cache_build(hb2_partition *p, int64_t node, const double *rootFre
     if (!p->d_bc_sib && (p->d_bc_out.alloc((size_t)p->C * p->Sp * p->Dp) || p->d_bc_outE.alloc((size_t)p->C * p->Sp) ||
                          p->d_bc_sib.alloc(3 * (p->L + p->I) + 2)))
         return 1;
-    double *hs = p->h_small;
-    for (int k = 0; k < p->Dp; k++) hs[k] = k < p->D ? rootFreqs[k] : 0.0;
-    CU(cudaMemcpyAsync(p->d_pi, hs, p->Dp * sizeof(double), cudaMemcpyHostToDevice, p->stream));
+    if (stage_root(p, rootFreqs)) return 1;
     // root -> parent(node) path (internal indices) and, per path node, its children that are NOT on the path
     std::vector<int> path;
     for (int64_t u = p->parents[node]; u >= 0; u = p->parents[p->L + u]) path.push_back((int)u);
@@ -1757,11 +1757,8 @@ int hb2_branch_cache_evaluate(hb2_partition *p, int64_t cat, const double *weigh
         if (cat >= p->C) return fail("rate class %lld out of range", (long long)cat);
         c0 = (int)cat; nc = 1;
     }
+    if (stage_root(p, nullptr, weights, (int)p->C)) return 1;    // the root vector of the build stays
     double *hs = p->h_small;
-    if (weights) {
-        for (int c = 0; c < p->C; c++) hs[p->Dp + c] = weights[c];
-        CU(cudaMemcpyAsync(p->d_weights, hs + p->Dp, p->C * sizeof(double), cudaMemcpyHostToDevice, p->stream));
-    }
     hb2::BranchCacheArgs a = bc_args(p, c0, nc);
     dim3 grid((unsigned)((p->S + 127) / 128), (unsigned)nc);
     hb2::bc_eval_kernel<<<grid, 128, 0, p->stream>>>(a, (int)p->bc_node, p->d_rootL, p->d_rootE);
@@ -1869,8 +1866,7 @@ int hb2_comm_class_groups(hb2_partition *p, int nGroups) {
     if (!p->comm) return fail("hb2_comm_class_groups needs hb2_comm_init first");
     if (nGroups < 1 || p->C % nGroups != 0 || p->n_ranks % nGroups != 0)
         return fail("class groups: %d must divide both the %lld rate classes and the %d ranks", nGroups, (long long)p->C, p->n_ranks);
-    if (p->n_pending) return fail("hb2_comm_class_groups must be called before matrices are set");
-    for (char h : p->have_matrix) if (h) return fail("hb2_comm_class_groups must be called before matrices are set");
+    for (const Slot &s : p->slots) if (s.have) return fail("hb2_comm_class_groups must be called before matrices are set");
     CU(cudaSetDevice(p->device));
     p->cg_G = nGroups; p->cg_g = p->rank % nGroups;
     p->ownN = (int)(p->C / nGroups); p->own0 = p->cg_g * p->ownN;
@@ -1906,7 +1902,7 @@ void hb2_destroy(hb2_partition *p) {
     peer_teardown(p);
     if (p->comm) g_nccl.CommDestroy(p->comm);
     const cudaStream_t stream = p->stream;
-    const cudaEvent_t events[] = {p->ev_mix, p->ev[0], p->ev[1], p->ev[2], p->ev[3], p->ev_staging};
+    const cudaEvent_t events[] = {p->ev[0], p->ev[1], p->ev[2], p->ev[3], p->ev_staging};
     delete p;                                             // releases every buffer
     for (cudaEvent_t e : events) if (e) cudaEventDestroy(e);
     if (stream) cudaStreamDestroy(stream);
@@ -1932,38 +1928,34 @@ int hb2_time_resident(hb2_partition *p, const double *weights, const double *roo
     // every slot must hold a resident copy of its rate matrix (dense, or the formula values of a compiled hand-over) so
     // that the expm stage can be replayed
     std::vector<int> dst;
-    int res_kind = 0;
+    Resident res = Resident::None;
     for (int64_t k = (int64_t)p->own0 * p->B; k < (int64_t)(p->own0 + p->ownN) * p->B; k++) {
-        if (!p->is_rate[k])
+        const Slot &s = p->slots[k];
+        if (s.res == Resident::None)
             return fail("hb2_time_resident needs a rate matrix (dense or compiled) in every slot, handed over after its template last "
                         "changed: class %lld, branch %lld has none", (long long)(k / p->B), (long long)(k % p->B));
-        if (res_kind && res_kind != p->is_rate[k]) return fail("hb2_time_resident: hand all matrices over the same way (dense or compiled) before timing");
-        if (p->is_rate[k] == 2 && p->res_tmpl[k] != 0) return fail("hb2_time_resident replays template 0 only");
-        res_kind = p->is_rate[k];
+        if (res != Resident::None && res != s.res) return fail("hb2_time_resident: hand all matrices over the same way (dense or compiled) before timing");
+        if (s.res == Resident::Formula && s.res_tmpl != 0) return fail("hb2_time_resident replays template 0 only");
+        res = s.res;
         dst.push_back((int)k);
     }
+    const bool compiled = res == Resident::Formula;
     if (wait_staging(p)) return 1;           // the flush above may still be reading the pinned queues
-    memcpy(p->h_dst, dst.data(), dst.size() * sizeof(int));
-    CU(cudaMemcpyAsync(p->d_dst, p->h_dst, dst.size() * sizeof(int), cudaMemcpyHostToDevice, p->stream));
+    HandoverQueue &q = p->dense;             // empty after the flush: its destination slots carry the replay's
+    memcpy(q.h_dst, dst.data(), dst.size() * sizeof(int));
+    CU(cudaMemcpyAsync(q.d_dst, q.h_dst, dst.size() * sizeof(int), cudaMemcpyHostToDevice, p->stream));
     SharedPlan sp;
-    if (plan_shared(p, p->h_dst, (int64_t)dst.size(), res_kind == 2 ? 1 : 2, nullptr, sp)) return 1;
-    if (res_kind == 2 && !sp.use) return fail("hb2_time_resident: compiled resident copies need the shared-powers path");
-    CU(cudaEventRecord(p->ev_staging, p->stream));
-    p->staging_busy = true;
-    double *hs = p->h_small;
-    for (int k = 0; k < p->Dp; k++) hs[k] = k < p->D ? rootFreqs[k] : 0.0;
-    for (int c = 0; c < p->C; c++) hs[p->Dp + c] = weights[c];
-    CU(cudaMemcpyAsync(p->d_pi, hs, p->Dp * sizeof(double), cudaMemcpyHostToDevice, p->stream));
-    CU(cudaMemcpyAsync(p->d_weights, hs + p->Dp, p->C * sizeof(double), cudaMemcpyHostToDevice, p->stream));
+    if (plan_shared(p, q.h_dst, (int64_t)dst.size(), compiled ? 1 : 2, nullptr, sp)) return 1;
+    if (compiled && !sp.use) return fail("hb2_time_resident: compiled resident copies need the shared-powers path");
+    if (staged_uploads(p) || stage_root(p, rootFreqs, weights, (int)p->C)) return 1;
     std::vector<char> dirty;
     if (dirty_nodes(p->parents.data(), p->L, p->I, -1, nullptr, dirty)) return 1;
+    const double *in = compiled ? p->tmpls[0].d_Vres + (size_t)p->own0 * p->B * p->tmpls[0].nF : p->d_Qres + (size_t)p->own0 * p->B * p->D * p->D;
     double tot = 0, st[3] = {0, 0, 0};
     for (int it = 0; it < iters; it++) {
         CU(cudaEventRecord(p->ev[0], p->stream));
         const int64_t l0 = p->launches;
-        if (res_kind == 2) {
-            if (launch_expm(p, p->tmpls[0].d_Vres + (size_t)p->own0 * p->B * p->tmpls[0].nF, p->d_dst, (int)dst.size(), 2, nullptr, true, nullptr, &sp)) return 1;
-        } else if (launch_expm(p, p->d_Qres + (size_t)p->own0 * p->B * p->D * p->D, p->d_dst, (int)dst.size(), 0, nullptr, true, nullptr, &sp)) return 1;
+        if (launch_expm(p, {compiled ? Kind::Compiled : Kind::Rate}, in, q.d_dst, (int)dst.size(), false, sp)) return 1;
         const int64_t l1 = p->launches;
         CU(cudaEventRecord(p->ev[1], p->stream));
         if (run_pruning(p, p->own0, p->ownN, dirty)) return 1;

@@ -60,7 +60,9 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
 /* Replaces ExponentiateMatrices (tree.cpp:2932-3113) + _CalcNode::SetCompExp (calcnode.cpp:714): hands the engine
  * the matrices of the nodes in `*matrices` (DetermineNodesForUpdate, tree.cpp:3117) for rate class `cat`
  * (0..C-1; -1 is accepted as 0 for partitions without category variables, likefunc.cpp:10843).
- * nodeIds[k] in 0..L+I-2; M[k] -> D*D doubles.  kind = HB2_MATRIX_RATE | HB2_MATRIX_TRANS. */
+ * nodeIds[k] in 0..L+I-2; M[k] -> D*D doubles.  kind = HB2_MATRIX_RATE | HB2_MATRIX_TRANS.
+ * Every hand-over (hb2_set_matrices*, hb2_set_mixture_matrices) checks its whole list first: a refused call (bad class,
+ * node id, kind or matrix pointer anywhere in the list) changes nothing -- no slot, no pending matrix, no branch cache. */
 int hb2_set_matrices(hb2_partition *p, int64_t cat, int64_t n, const int64_t *nodeIds,
                      const double *const *M, int kind);
 /* same, matrices packed back to back (n*D*D doubles) */

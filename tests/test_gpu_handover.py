@@ -508,3 +508,61 @@ def test_batched_site_likelihoods_follow_template_and_frequencies():
     call(0, small, "template 0 after a frequency change, groups of 1-3")
     call(0, big, "template 0 after a frequency change, groups of 4+")
     lf.close()
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# 10. refused hand-overs
+# ---------------------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("form", ["dense", "compiled template 0", "compiled template 1", "mixture"])
+def test_refused_handovers_change_nothing(form):
+    """A hand-over whose last node id is B (no such branch) is refused as a whole.  (a) On a fresh partition in which every
+    other slot holds a matrix, the listed slots still hold none: compute() fails with "no matrix was ever set".  (b) On an
+    evaluated partition, the listed valid slots keep their matrices bit for bit, a branch cache built before the call still
+    evaluates, and a re-evaluation gives the same lnL bit for bit."""
+    w = hc.workload(61, 12, 40, 2, mean_t=0.1)
+    t = w.tree.t
+    tm = hc.gy94_template()
+    base = hc.unit_rate(tm, hc.gy94_rates(2.0, 0.5))
+    c, listed = 1, np.array([2, 7])
+    refused = np.r_[listed, w.tree.n_branches]
+
+    def fresh():
+        lf = LF(w, "fp64")
+        tm.define(lf.part, 0)
+        tm.with_freqs(hc.codon_pi(71)).define(lf.part, 1)
+        return lf
+
+    def refuse(part):
+        v = values(base, t, refused % w.tree.n_branches, 1.3)
+        with pytest.raises(engine.EngineError, match="has no branch"):
+            if form == "dense":
+                part.set_matrices(c, refused, np.stack([tm.Q(x) for x in v]), engine.MATRIX_RATE)
+            elif form == "mixture":
+                part.set_mixture_matrices(c, refused, *mixture_inputs(tm, t, refused % w.tree.n_branches, 1.3))
+            else:
+                part.set_matrices_compiled(c, refused, v, template=int(form[-1]))
+
+    lf = fresh()                                                                         # (a)
+    nodes = lf.all_nodes
+    for cc in range(w.C):
+        rest = nodes if cc != c else np.setdiff1d(nodes, listed)
+        lf.part.set_matrices_compiled(cc, rest, values(base, t, rest))
+    refuse(lf.part)
+    with pytest.raises(engine.EngineError, match="no matrix was ever set"):
+        lf.compute()
+    lf.close()
+
+    lf = fresh()                                                                         # (b)
+    for cc in range(w.C):
+        lf.part.set_matrices_compiled(cc, nodes, values(base, t, nodes))
+    before = lf.compute()
+    P = [lf.part.read_transition(c, b) for b in listed]
+    lf.part.branch_cache_build(int(listed[0]), w.pi)
+    refuse(lf.part)
+    cached = lf.part.branch_cache_evaluate(w.class_weights)
+    assert abs(cached - before) <= 1e-10 * abs(before), f"branch cache {cached!r}, full {before!r}"
+    for b, Pb in zip(listed, P):
+        assert np.array_equal(lf.part.read_transition(c, b), Pb), f"{form}: the matrix of branch {b} changed"
+    after = lf.compute()
+    assert after == before, f"{form}: lnL {before!r} -> {after!r}"
+    lf.close()
