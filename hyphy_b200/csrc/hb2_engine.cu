@@ -254,7 +254,7 @@ struct hb2_partition {
         int G = 0, stride = 0;                // groups, doubles per cached reference direction
         DeviceBuffer<int> d_int, d_flag;      // d_int: [group cap | ref cap | refs G]
         PinnedBuffer<int> h_int;
-        DeviceBuffer<double> d_weight, d_pow, d_refvec, d_colsum;   // colsum [cap][16][64]
+        DeviceBuffer<double> d_weight, d_pow, d_refvec;
         DeviceBuffer<hb2::ExpmGroup> d_groups;
         DeviceBuffer<unsigned long long> d_flags;   // generation flags of the coefficient matrices [G][EXPM_POW_TERMS]
         unsigned long long gen = 0;
@@ -265,7 +265,7 @@ struct hb2_partition {
             G = G_; cap = cap_; stride = 4096; gen = 0;
             kind.assign(G, 0);
             return d_int.alloc(2 * cap + G) || h_int.alloc(2 * cap + G) || d_flag.alloc(cap) || d_weight.alloc(cap) ||
-                   d_colsum.alloc(cap * 16 * 64) || d_groups.alloc(G) || d_groups.zero(stream) ||
+                   d_groups.alloc(G) || d_groups.zero(stream) ||
                    d_pow.alloc((size_t)G * hb2::EXPM_POW_TERMS * 4096) || d_flags.alloc((size_t)G * hb2::EXPM_POW_TERMS) ||
                    d_flags.zero(stream) || d_refvec.alloc((size_t)G * stride);
         }
@@ -468,12 +468,18 @@ int launch_expm(hb2_partition *p, Source src, const double *in, const int *d_dst
                     hb2::expm_powers_kernel<<<dim3(hb2::EXPM_POW_TERMS - 1, (unsigned)sp.n_refs), 256, smem, p->stream>>>(pa);
                     p->launches++;
                 }
-                double *colsum = x.d_colsum + (size_t)off * 16 * 64;
-                hb2::expm_poly_kernel<<<dim3(16, (unsigned)((n + hb2::EXPM_POLY_CHUNK - 1) / hb2::EXPM_POLY_CHUNK)), 256, 0, p->stream>>>(a, tc, colsum, n);
-                a.colsum = colsum;                   // the finishing kernel below repairs the rows of the entries finished here
+                cudaLaunchConfig_t cfg{};
+                cfg.gridDim = dim3(hb2::EXPM_POLY_CLUSTER, (unsigned)((n + hb2::EXPM_POLY_CHUNK - 1) / hb2::EXPM_POLY_CHUNK));
+                cfg.blockDim = dim3(256);
+                cfg.stream = p->stream;
+                cudaLaunchAttribute attr{};
+                attr.id = cudaLaunchAttributeClusterDimension;
+                attr.val.clusterDim.x = hb2::EXPM_POLY_CLUSTER; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+                cfg.attrs = &attr; cfg.numAttrs = 1;
+                CU(cudaLaunchKernelEx(&cfg, hb2::expm_poly_kernel, a, tc, n));
                 p->launches += 2;
             }
-            hb2::expm64_dmma_kernel<<<n, 256, smem, p->stream>>>(a, tc);
+            hb2::expm64_dmma_kernel<<<std::min(n, 2 * p->sm_count), 256, smem, p->stream>>>(a, tc, n);
             break;
         }
         case 4: hb2::expm_small_kernel<4><<<n, 128, hb2::expm_small_smem_bytes(4), p->stream>>>(a); break;
@@ -1357,6 +1363,19 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
         CU(cudaFuncSetAttribute(hb2::expm_powers_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(3 * 64 * hb2::LD64 * sizeof(double))));
         CU(cudaFuncSetAttribute(hb2::expm64_dmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(3 * 64 * hb2::LD64 * sizeof(double))));
         CU(cudaFuncSetAttribute(hb2::expm64_dmma_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+        // the polynomial kernel's 16 row slices of a chunk share their column sums as one cluster (a non-portable size)
+        CU(cudaFuncSetAttribute(hb2::expm_poly_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+        cudaLaunchConfig_t cfg{};
+        cfg.gridDim = dim3(hb2::EXPM_POLY_CLUSTER);
+        cfg.blockDim = dim3(256);
+        cudaLaunchAttribute attr{};
+        attr.id = cudaLaunchAttributeClusterDimension;
+        attr.val.clusterDim.x = hb2::EXPM_POLY_CLUSTER; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+        cfg.attrs = &attr; cfg.numAttrs = 1;
+        int clusters = 0;
+        CU(cudaOccupancyMaxActiveClusters(&clusters, hb2::expm_poly_kernel, &cfg));
+        if (clusters < 1)
+            return fail("expm_poly_kernel: no cluster of %d CTAs can be resident on device %d", hb2::EXPM_POLY_CLUSTER, device);
     }
     if (Dp == 4) {
         if (const char *env = getenv("HB2_SMALL_ILP")) p->small_ilp = atoi(env);
@@ -1566,9 +1585,9 @@ static int batch_sites(hb2_partition *p, int64_t templateId, int64_t nSets, cons
     int64_t cap;
     if (!mix)                                   // P matrices of `cap` sets (32 KB per branch)
         cap = std::min<int64_t>(nSets, std::max<int64_t>(1, (int64_t)(8.0e9 / ((double)B * (4096 + 1024 + (double)nF) * 8))));
-    else {                                      // a set's R component matrices, formula values, weights and colsum scratch,
+    else {                                      // a set's R component matrices, formula values and weights,
                                                 // the power tables of its groups and its node vectors
-        const double per_set = (double)R * (4096 + 16 * 64 + (double)nF + 1) * 8 + (double)gk * hb2::EXPM_POW_TERMS * 4096 * 8 + (double)p->I * 64 * 8;
+        const double per_set = (double)R * (4096 + (double)nF + 1) * 8 + (double)gk * hb2::EXPM_POW_TERMS * 4096 * 8 + (double)p->I * 64 * 8;
         cap = std::min<int64_t>(nSets, std::max<int64_t>(1, (int64_t)(8.0e9 / per_set)));
     }
     cap = std::min<int64_t>(cap, 1024);

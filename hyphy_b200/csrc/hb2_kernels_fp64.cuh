@@ -1,6 +1,6 @@
 // hb2_kernels_fp64.cuh -- fp64 CUDA kernels of the likelihood hot path (sm_90a).
 //
-//   expm64_dmma_kernel / expm_small_kernel  P = exp(Q t) per (branch, rate class), one CTA per matrix
+//   expm64_dmma_kernel / expm_small_kernel  P = exp(Q t) per (branch, rate class)
 //                                           (replaces _Matrix::Exponentiate, reference matrix.cpp:5537-5951)
 //   prune_small_walk_kernel<Dp, PP>         Felsenstein pruning pass for 4 / 8 padded states, PP patterns per thread:
 //                                           all children folded (leaf column gather, ambiguity mat-vec, internal
@@ -21,6 +21,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <math.h>
+#include <cooperative_groups.h>
 
 namespace hb2 {
 
@@ -94,7 +95,8 @@ __device__ __forceinline__ void rescale_running_quad(double (&v)[NT][2], int &ex
 }
 
 // ------------------------------------------------------------------------------------------------
-// Matrix exponential.  One CTA per matrix (expm64_dmma_kernel, expm_small_kernel), or the shared-powers path below.
+// Matrix exponential.  One wave of CTAs over the batch (expm64_dmma_kernel), one CTA per matrix (expm_small_kernel), or
+// the shared-powers path below.
 //   in : Q [n][D*D] row-major rate matrices (Q*t, diagonal = -rowsum), dst[n] = slot index into PT
 //   out: PT[slot] = exp(Q)^T with padding rows/cols zeroed, negatives clamped, columns repaired to sum to 1
 // Algorithm (engine's own, same result as the reference's Taylor+squaring to ~1e-15): scale by 2^-s, Taylor polynomial
@@ -104,8 +106,6 @@ struct ExpmArgs {
     const double *Q;        // [n][D*D]
     const int *dst;         // [n] destination slot; < 0: retired entry (the slot was handed over again), skipped
     double *PT;
-    const double *colsum;   // nullable [n][16][64]: column-sum partials of expm_poly_kernel; non-null = expm64_dmma_kernel also
-                            // does the row repair of the entries that kernel finished
     double *Qres;           // nullable [slots][D*D]: resident copy of the rate matrices, written while loading
     int D;
     int is_trans;           // 1: input already a transition matrix -> just transpose/pad
@@ -335,50 +335,42 @@ __global__ void __launch_bounds__(256) expm_classify_warp_kernel(ExpmClassifyArg
     if (lane == 0) { a.flag[k] = ok; a.weight[k] = wk; }
 }
 
-__global__ void __launch_bounds__(256, 2) expm64_dmma_kernel(ExpmArgs a, ExpmTcOut tc) {
-    // Three shared 64x64 fp64 buffers (101 KB) so that TWO CTAs share an SM and one CTA's load/norm/epilogue phases
-    // overlap the other's DMMA products:  X0 = A -> later R,  X1 = A^2,  X2 = A^3.  The polynomial blocks need A at the
-    // thread's own output positions after X0 has become R: those values are parked in the (not yet written) output
-    // slot PT[slot] in global memory (L2 resident, same [row][col] layout) and re-read per Horner step.
-    extern __shared__ __align__(16) double sm[];
+// Shared-powers entry k: rho = ||A_k||_inf estimated from its weight, and the squarings expm_poly_kernel chose for it.
+// shift == 0 with rho not NaN: that kernel has finished the entry.
+__device__ __forceinline__ int expm_poly_shift(const ExpmArgs &a, int k, double &rho) {
+    const ExpmGroup gi = a.groups[a.group[k]];
+    rho = gi.nu * (a.weight[k] / gi.weight);
+    int shift = 0;
+    if (rho > EXPM_POLY_THETA) { int e = 0; frexp(rho / EXPM_POLY_THETA, &e); shift = max(e, 0); }
+    return shift;
+}
+
+// One entry of expm64_dmma_kernel.  Three shared 64x64 fp64 buffers (101 KB) so that TWO CTAs share an SM and one CTA's
+// load/norm/epilogue phases overlap the other's DMMA products:  X0 = A -> later R,  X1 = A^2,  X2 = A^3.  The polynomial
+// blocks need A at the thread's own output positions after X0 has become R: those values are parked in the (not yet
+// written) output slot PT[slot] in global memory (L2 resident, same [row][col] layout) and re-read per Horner step.
+// Every exit is CTA-uniform; the caller separates entries with a barrier.  Kept out of line: inlined into the kernel's
+// entry loop, the body no longer fits the 128 registers of two CTAs per SM and spills.
+__device__ __noinline__ void expm64_dmma_entry(const ExpmArgs a, const ExpmTcOut tc, int entry, double *sm) {
     double *X0 = sm, *X1 = X0 + 64 * LD64, *X2 = X1 + 64 * LD64;
     __shared__ double red[64];
     __shared__ int s_shift, s_Q;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int wr = warp >> 1, wc = warp & 1, g = lane >> 2, q4 = lane & 3;
     const int D = a.D;
-    if (a.dst[blockIdx.x] < 0) return;
-    const size_t slot = a.dst[blockIdx.x];
+    if (a.dst[entry] < 0) return;
+    const size_t slot = a.dst[entry];
     double *out = a.PT + slot * 4096;
     double *park = out;
     double *R = X0;
 
-    const bool shared_powers = a.flag && a.flag[blockIdx.x];
+    const bool shared_powers = a.flag && a.flag[entry];
     if (shared_powers) {
         // expm_poly_kernel has left the Taylor polynomial of A / 2^shift in the output slot; squarings and the epilogue
         // (clamp, row repair, tensor-path operands) remain.  shift is recomputed exactly as the polynomial stage chose it.
-        const ExpmGroup gi = a.groups[a.group[blockIdx.x]];
-        const double rho = gi.nu * (a.weight[blockIdx.x] / gi.weight);
-        int shift = 0;
-        if (rho > EXPM_POLY_THETA) { int e = 0; frexp(rho / EXPM_POLY_THETA, &e); shift = max(e, 0); }
-        if (shift == 0 && rho == rho) {          // finished by expm_poly_kernel up to the row repair
-            if (a.colsum && tid < 64) {
-                const int col = tid;
-                double s = 0.0;
-#pragma unroll
-                for (int sl = 0; sl < 16; sl++) s += a.colsum[((size_t)blockIdx.x * 16 + sl) * 64 + col];
-                const double d = col < a.D ? fmax(1.0 - s, 0.0) : 0.0;
-                out[col * 64 + col] = d;
-                if (tc.PB) {
-                    tc.PTf[slot * 4352 + col * 68 + col] = (float)d;
-                    const float hi = tf32_rn_dev((float)d);
-                    float *pb = tc.PB + slot * 8192 + (col >> 2) * 256 + col * 4 + (col & 3);
-                    pb[0] = hi;
-                    pb[4096] = tf32_rn_dev((float)(d - (double)hi));
-                }
-            }
-            return;
-        }
+        double rho;
+        const int shift = expm_poly_shift(a, entry, rho);
+        if (shift == 0 && rho == rho) return;    // finished by expm_poly_kernel
         if (!(rho == rho) || shift > 900) {
             for (int idx = tid; idx < 4096; idx += 256) out[idx] = __longlong_as_double(0x7ff8000000000000LL);
             if (tc.PB) {
@@ -391,7 +383,7 @@ __global__ void __launch_bounds__(256, 2) expm64_dmma_kernel(ExpmArgs a, ExpmTcO
         if (tid == 0) s_shift = shift;
         __syncthreads();
     } else
-    load_rate_matrix<64, LD64, 256>(a, X0, tid);
+    load_rate_matrix<64, LD64, 256>(a, X0, tid, entry);
     if (shared_powers || !a.is_trans) {
       double acc[2][4][2];
       auto zero = [&]() {
@@ -528,6 +520,31 @@ __global__ void __launch_bounds__(256, 2) expm64_dmma_kernel(ExpmArgs a, ExpmTcO
     }
 }
 
+// One wave of CTAs (gridDim.x <= 2 per SM) striding over the n entries of a batch.  Per round of up to 256 entries of
+// its share, the CTA first lists the entries with work left, one thread per entry (on the shared-powers path
+// expm_poly_kernel has finished most of them), then processes the listed ones in turn.
+__global__ void __launch_bounds__(256, 2) expm64_dmma_kernel(ExpmArgs a, ExpmTcOut tc, int n) {
+    extern __shared__ __align__(16) double sm[];
+    __shared__ int s_list[256], s_count;
+    for (int base = blockIdx.x; base < n; base += 256 * gridDim.x) {
+        if (threadIdx.x == 0) s_count = 0;
+        __syncthreads();
+        const int k = base + threadIdx.x * gridDim.x;
+        if (k < n && a.dst[k] >= 0) {
+            double rho;
+            const bool finished = a.flag && a.flag[k] && expm_poly_shift(a, k, rho) == 0 && rho == rho;
+            if (!finished) s_list[atomicAdd(&s_count, 1)] = k;
+        }
+        __syncthreads();
+        const int count = s_count;
+        for (int j = 0; j < count; j++) {
+            expm64_dmma_entry(a, tc, s_list[j], sm);
+            __syncthreads();                     // the next entry overwrites the shared buffers
+        }
+        __syncthreads();                         // every thread has read s_count
+    }
+}
+
 // ------------------------------------------------------------------------------------------------
 // Shared-powers path, stage 2: S_m = R^m / m! (PT layout, i.e. powers of the TRANSPOSED reference matrix), m = 1..24, for
 // every group whose reference is (re)established in this batch.  grid = (24, number of such groups); CTA (j, g) produces
@@ -644,20 +661,25 @@ __global__ void __launch_bounds__(256, 1) expm_powers_kernel(ExpmPowersArgs pa) 
 // ------------------------------------------------------------------------------------------------
 // Shared-powers path, stage 3: P = sum_m S_m x^m with x = rho / 2^shift <= EXPM_POLY_THETA for every flagged entry, fused
 // with the epilogue for the (common) entries that need no squaring.
-// grid = (16 row slices, chunks of EXPM_POLY_CHUNK entries).  Thread t of slice sl owns element (row 4 sl + t%4,
-// column t/4) of the PT layout (row = child state, column = parent state) and keeps that element's 24 coefficients in
-// registers while it walks its chunk (reloaded only when the group changes: batches are class-major); the chunk's
-// metadata is fetched up front so that the loop carries no dependent global loads.
+// grid = (16 row slices, chunks of EXPM_POLY_CHUNK entries); the 16 slices of a chunk form one thread-block cluster
+// (EXPM_POLY_CLUSTER, a non-portable size).  Thread t of slice sl owns element (row 4 sl + t%4, column t/4) of the PT
+// layout (row = child state, column = parent state) and keeps that element's 24 coefficients in registers while it walks
+// its chunk (reloaded only when the group changes: batches are class-major); the chunk's metadata is fetched up front so
+// that the loop carries no dependent global loads.
 //   shift == 0: the value is final up to the row repair.  It is clamped at 0, padding is zeroed, and PT (fp64), PTf (fp32
 //               table) and PB (tf32 hi/lo tiles; chunk sl of the canonical layout is exactly this slice, offset t) are
-//               written directly; the partial column sums of the slice (4 rows, diagonal excluded; 4 adjacent lanes) go to
-//               colsum[entry][sl][column] for expm64_dmma_kernel, which sets the diagonal to 1 - (sum of the rest of P's row).
+//               written directly; the partial column sums of the slice (4 rows, diagonal excluded; 4 adjacent lanes) stay
+//               in shared memory.  After a cluster barrier the slice that holds diagonal (c, c) adds the 16 slices'
+//               partials of column c through distributed shared memory, in slice order, and writes 1 - sum (clamped at 0):
+//               rows of P sum to 1.  The entry is then final.
 //   shift  > 0: the raw polynomial value goes to PT; expm64_dmma_kernel squares and finishes the entry.
 // ------------------------------------------------------------------------------------------------
-constexpr int EXPM_POLY_CHUNK = 8;
-__global__ void __launch_bounds__(256, 3) expm_poly_kernel(ExpmArgs a, ExpmTcOut tc, double *__restrict__ colsum, int n) {
-    __shared__ int s_slot[EXPM_POLY_CHUNK], s_grp[EXPM_POLY_CHUNK];
+constexpr int EXPM_POLY_CHUNK = 16;
+constexpr int EXPM_POLY_CLUSTER = 16;
+__global__ void __launch_bounds__(256, 3) expm_poly_kernel(ExpmArgs a, ExpmTcOut tc, int n) {
+    __shared__ int s_slot[EXPM_POLY_CHUNK], s_grp[EXPM_POLY_CHUNK], s_fin[EXPM_POLY_CHUNK];
     __shared__ double s_wgt[EXPM_POLY_CHUNK];
+    __shared__ double s_part[EXPM_POLY_CHUNK][64];                  // this slice's column partials of the finished entries
     const int tid = threadIdx.x, sl = blockIdx.x;
     const int row = 4 * sl + (tid & 3), col = tid >> 2;
     const int e = row * 64 + col;                                     // element index in the 64x64 PT layout
@@ -674,7 +696,7 @@ __global__ void __launch_bounds__(256, 3) expm_poly_kernel(ExpmArgs a, ExpmTcOut
             gv = a.group[k];
             wv = a.weight[k];
         }
-        s_slot[tid] = sv; s_grp[tid] = gv; s_wgt[tid] = wv;
+        s_slot[tid] = sv; s_grp[tid] = gv; s_wgt[tid] = wv; s_fin[tid] = 0;
     }
     __syncthreads();
     double c[EXPM_POW_TERMS];
@@ -710,13 +732,15 @@ __global__ void __launch_bounds__(256, 3) expm_poly_kernel(ExpmArgs a, ExpmTcOut
         double v = fma(vo, x, fma(ve, x2, unit));
         const size_t sidx = (size_t)slot;
         if (shift > 0) { __stcg(a.PT + sidx * 4096 + out_pt, v); continue; }
+        if (!(rho == rho)) continue;                                  // NaN input: the finishing kernel writes NaN
         v = (pad || v < 0.0) ? 0.0 : v;
         // column sums over this slice's 4 rows (lanes t, t^1, t^2, t^3 share a column), diagonal element excluded
         double part = (row == col) ? 0.0 : v;
         part += __shfl_xor_sync(0xffffffffu, part, 1);
         part += __shfl_xor_sync(0xffffffffu, part, 2);
-        if ((tid & 3) == 0) colsum[((size_t)(k0 + i) * 16 + sl) * 64 + col] = part;
-        if (row != col) {                                             // expm64_dmma_kernel owns the diagonal
+        if ((tid & 3) == 0) s_part[i][col] = part;
+        if (tid == 0) s_fin[i] = 1;
+        if (row != col) {                                             // the diagonal is written after the cluster barrier
             __stcg(a.PT + sidx * 4096 + out_pt, v);
             if (tc.PB) {
                 const float vf = (float)v;
@@ -728,6 +752,27 @@ __global__ void __launch_bounds__(256, 3) expm_poly_kernel(ExpmArgs a, ExpmTcOut
             }
         }
     }
+    // row repair: thread t handles entry t/4 and diagonal column 4 sl + t%4
+    static_assert(4 * EXPM_POLY_CHUNK <= 256, "one thread per (entry, diagonal column) of the slice");
+    cooperative_groups::cluster_group cluster = cooperative_groups::this_cluster();
+    cluster.sync();                                                   // every slice's partials are in its shared memory
+    if (tid < 4 * EXPM_POLY_CHUNK && s_fin[tid >> 2]) {
+        const int i = tid >> 2, c = 4 * sl + (tid & 3);
+        double s = 0.0;
+#pragma unroll
+        for (int r = 0; r < EXPM_POLY_CLUSTER; r++) s += cluster.map_shared_rank(&s_part[i][0], r)[c];
+        const double d = c < a.D ? fmax(1.0 - s, 0.0) : 0.0;
+        const size_t sidx = (size_t)s_slot[i];
+        a.PT[sidx * 4096 + c * 64 + c] = d;
+        if (tc.PB) {
+            tc.PTf[sidx * 4352 + c * 68 + c] = (float)d;
+            const float hi = tf32_rn_dev((float)d);
+            float *pb = tc.PB + sidx * 8192 + (c >> 2) * 256 + c * 4 + (c & 3);
+            pb[0] = hi;
+            pb[4096] = tf32_rn_dev((float)(d - (double)hi));
+        }
+    }
+    cluster.sync();                                                   // peers may still be reading this slice's partials
 }
 
 // Small state spaces (Dp <= 32): one CTA of 128 threads per matrix, plain shared-memory products.
