@@ -339,6 +339,15 @@ struct hb2_partition {
     std::vector<double *> px_peer;            // host copy of the mapped pointers (entry rank = px_local)
     DeviceBuffer<double *> d_px_peer;
     DeviceBuffer<unsigned> d_px_counter;
+    // simulation scratch (hb2_simulate), grown on demand and used by nothing else: the prefix-sum table, the call's small
+    // vectors, and one chunk of leaf / node / class outputs and internal states
+    struct SimBuf {
+        DeviceBuffer<double> cdf, vec;
+        DeviceBuffer<int> ints, cls;
+        DeviceBuffer<long long> leaf, node;
+        DeviceBuffer<unsigned char> states;
+        size_t cap[7] = {0, 0, 0, 0, 0, 0, 0};
+    } sim;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
     // recorded after uploads from pinned staging (the queues, ExBuf::h_int, column frequencies, mixtures, the replay's
     // slots): every writer of those buffers waits for it first
@@ -1244,6 +1253,35 @@ int lane_ctas_per_sm(const char *name, const void *fn, int threads, int smem, in
     return 0;
 }
 
+// ---- Simulation (hb2_simulate) --------------------------------------------------------------------------------------------
+constexpr int64_t SIM_CHUNK = (int64_t)1 << 18;    // sites per simulate_kernel launch
+constexpr int SIM_THREADS = 128;
+constexpr size_t SIM_SMEM_MAX = 48 << 10;          // internal states of a CTA's sites in shared memory up to this size
+
+// Prefix sums of a weight vector by the draw rule and its last positive index.  False when an entry is negative or NaN or
+// the total is not finite and > 0.
+bool sim_prefix(const double *v, int64_t m, double *c, int *last) {
+    double s = 0.0;
+    *last = -1;
+    for (int64_t j = 0; j < m; j++) {
+        if (!(v[j] >= 0.0)) return false;
+        if (v[j] > 0.0) { s += v[j]; *last = (int)j; }
+        c[j] = s;
+    }
+    return s > 0.0 && std::isfinite(s);
+}
+
+// Grows a simulation buffer to n elements (its contents are not kept).
+template <typename T>
+int sim_reserve(hb2_partition *p, DeviceBuffer<T> &b, size_t &cap, size_t n) {
+    if (n <= cap) return 0;
+    CU(cudaStreamSynchronize(p->stream));
+    cap = 0;
+    if (b.alloc(std::max<size_t>(n, 1))) return 1;
+    cap = n;
+    return 0;
+}
+
 }  // namespace
 
 // =================================================================================================
@@ -1701,6 +1739,86 @@ int hb2_read_transition(hb2_partition *p, int64_t cat, int64_t node, double *P) 
     CU(cudaMemcpy(tmp.data(), p->d_PT + ((size_t)cat * p->B + node) * p->Dp * p->Dp, tmp.size() * sizeof(double), cudaMemcpyDeviceToHost));
     for (int64_t i = 0; i < p->D; i++)
         for (int64_t j = 0; j < p->D; j++) P[i * p->D + j] = tmp[j * p->Dp + i];   // stored transposed
+    return 0;
+}
+
+int hb2_simulate(hb2_partition *p, const double *weights, const double *rootFreqs, int64_t nSites, uint64_t seed, int64_t firstSite,
+                 int64_t *leafStates, int64_t *nodeStates, int32_t *siteClass) {
+    if (!p) return fail("null partition");
+    if (nSites < 0) return fail("hb2_simulate: nSites=%lld is negative", (long long)nSites);
+    if (firstSite < 0 || firstSite > INT64_MAX - nSites) return fail("hb2_simulate: firstSite=%lld out of range", (long long)firstSite);
+    if (!rootFreqs) return fail("hb2_simulate: rootFreqs must not be null");
+    if (nSites > 0 && !leafStates) return fail("hb2_simulate: leafStates must not be null");
+    if (p->cg_G > 1) return fail("hb2_simulate is not available with class groups: a rank does not hold the other groups' matrices");
+    if (!weights && p->C > 1) return fail("hb2_simulate: weights may be null only with one rate class (C=%lld)", (long long)p->C);
+    const int64_t C = p->C, D = p->D, B = p->B, L = p->L, I = p->I;
+    std::vector<double> vec(C + D);                 // prefix sums: classes | root states
+    std::vector<int> ints(C + 3);                   // active classes [C] | last class | last root state | first bad row
+    if (weights) {
+        if (!sim_prefix(weights, C, vec.data(), &ints[C]))
+            return fail("hb2_simulate: class weights must be >= 0 and not NaN, with a finite positive total");
+    } else {
+        vec[0] = 1.0; ints[C] = 0;
+    }
+    if (!sim_prefix(rootFreqs, D, vec.data() + C, &ints[C + 1]))
+        return fail("hb2_simulate: root frequencies must be >= 0 and not NaN, with a finite positive total");
+    ints[C + 2] = INT_MAX;
+    for (int64_t c = 0; c < C; c++) {
+        ints[c] = !weights || weights[c] > 0.0;
+        for (int64_t b = 0; ints[c] && b < B; b++)
+            if (!p->slots[c * B + b].have)
+                return fail("hb2_simulate: no matrix was ever set for rate class %lld, node %lld", (long long)c, (long long)b);
+    }
+    if (nSites == 0) return 0;
+    CU(cudaSetDevice(p->device));
+    if (flush_matrices(p)) return 1;
+    const int64_t chunk = std::min(nSites, SIM_CHUNK);
+    const bool smem_states = (size_t)I * SIM_THREADS <= SIM_SMEM_MAX;
+    hb2_partition::SimBuf &sb = p->sim;
+    if (sim_reserve(p, sb.cdf, sb.cap[0], (size_t)C * B * D * p->Dp) || sim_reserve(p, sb.vec, sb.cap[1], vec.size()) ||
+        sim_reserve(p, sb.ints, sb.cap[2], (size_t)C * B * D + ints.size()) || sim_reserve(p, sb.leaf, sb.cap[3], (size_t)L * chunk) ||
+        (nodeStates && sim_reserve(p, sb.node, sb.cap[4], (size_t)I * chunk)) ||
+        (siteClass && sim_reserve(p, sb.cls, sb.cap[5], (size_t)chunk)) ||
+        (!smem_states && sim_reserve(p, sb.states, sb.cap[6], (size_t)I * chunk)))
+        return 1;
+    int *d_last = sb.ints, *d_ints = sb.ints + C * B * D;
+    CU(cudaMemcpyAsync(sb.vec, vec.data(), vec.size() * sizeof(double), cudaMemcpyHostToDevice, p->stream));
+    CU(cudaMemcpyAsync(d_ints, ints.data(), ints.size() * sizeof(int), cudaMemcpyHostToDevice, p->stream));
+    hb2::SimArgs a{};
+    a.PT = p->d_PT; a.cdf = sb.cdf; a.last = d_last; a.active = d_ints; a.bad = d_ints + C + 2;
+    a.class_cdf = sb.vec; a.root_cdf = sb.vec + C; a.class_last = d_ints + C; a.root_last = d_ints + C + 1;
+    a.tree.child_start = p->d_child_start; a.tree.child_ids = p->d_child_ids;
+    a.leaf_out = sb.leaf; a.node_out = nodeStates ? (long long *)sb.node : nullptr; a.class_out = siteClass ? (int *)sb.cls : nullptr;
+    a.states = smem_states ? nullptr : (unsigned char *)sb.states;
+    a.L = (int)L; a.I = (int)I; a.B = (int)B; a.C = (int)C; a.D = (int)D; a.Dp = p->Dp; a.chunk = (int)chunk;
+    a.key = make_uint2((unsigned)seed, (unsigned)(seed >> 32));
+    // the table of every drawn class, and its check: a refused call writes nothing
+    hb2::sim_cdf_kernel<<<(unsigned)(C * B), 64, 0, p->stream>>>(a);
+    p->launches++;
+    CU(cudaGetLastError());
+    int bad = INT_MAX;
+    CU(cudaMemcpyAsync(&bad, a.bad, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
+    CU(cudaStreamSynchronize(p->stream));
+    if (bad != INT_MAX) {
+        const long long row = bad % D, cb = bad / D;
+        return fail("hb2_simulate: row %lld of the transition matrix of rate class %lld, node %lld does not have a finite positive total",
+                    row, cb / B, cb % B);
+    }
+    const size_t smem = smem_states ? (size_t)I * SIM_THREADS : 0;
+    for (int64_t s0 = 0; s0 < nSites; s0 += chunk) {
+        const int64_t n = std::min(chunk, nSites - s0);
+        a.n = (int)n; a.g0 = (unsigned long long)(firstSite + s0);
+        hb2::simulate_kernel<<<(unsigned)((n + SIM_THREADS - 1) / SIM_THREADS), SIM_THREADS, smem, p->stream>>>(a);
+        p->launches++;
+        CU(cudaGetLastError());
+        CU(cudaMemcpy2DAsync(leafStates + s0, nSites * sizeof(int64_t), sb.leaf, chunk * sizeof(long long), n * sizeof(int64_t), L,
+                             cudaMemcpyDeviceToHost, p->stream));
+        if (nodeStates)
+            CU(cudaMemcpy2DAsync(nodeStates + s0, nSites * sizeof(int64_t), sb.node, chunk * sizeof(long long), n * sizeof(int64_t), I,
+                                 cudaMemcpyDeviceToHost, p->stream));
+        if (siteClass) CU(cudaMemcpyAsync(siteClass + s0, sb.cls, n * sizeof(int32_t), cudaMemcpyDeviceToHost, p->stream));
+    }
+    CU(cudaStreamSynchronize(p->stream));
     return 0;
 }
 

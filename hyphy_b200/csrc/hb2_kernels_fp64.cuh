@@ -1530,6 +1530,146 @@ __global__ void __launch_bounds__(64) prune_batch_kernel(BatchPruneArgs a) {
 }
 
 // ------------------------------------------------------------------------------------------------
+// Simulated alignments (hb2_simulate; SimulateDataSet, likefunc.cpp:12584, discrete-category mode).  Every draw is one
+// Philox4x32-10 call on the counter (lo32(g), hi32(g), slot, 0) with key (lo32(seed), hi32(seed)), g = global site,
+// turned into u = (x0 * 2^21 + (x1 >> 11)) * 2^-53, and resolved against the sequential fp64 prefix sums c of the
+// weights (entries that are not > 0 count as 0): the smallest j with fl(u * c_last) < c_j, else the last positive j.
+// sim_cdf_kernel builds the prefix sums of every matrix row of the drawn classes once per call; simulate_kernel walks
+// the tree from the root, one thread per site.
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
+#pragma unroll
+    for (int r = 0; r < 10; r++) {
+        if (r > 0) { k.x += 0x9E3779B9u; k.y += 0xBB67AE85u; }
+        const unsigned lo0 = 0xD2511F53u * c.x, hi0 = __umulhi(0xD2511F53u, c.x);
+        const unsigned lo1 = 0xCD9E8D57u * c.z, hi1 = __umulhi(0xCD9E8D57u, c.z);
+        c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
+    }
+    return c;
+}
+
+// Uniform in [0, 1) of draw `slot` of global site g.
+__device__ __forceinline__ double sim_uniform(unsigned long long g, unsigned slot, uint2 key) {
+    const uint4 x = philox4x32_10(make_uint4((unsigned)g, (unsigned)(g >> 32), slot, 0u), key);
+    return (double)(((unsigned long long)x.x << 21) + (x.y >> 11)) * 0x1p-53;
+}
+
+// The draw rule on prefix sums c[0..m-1]; *last = the last index of positive weight, read only when u * total rounds up
+// to the total.
+// Vectors of 17..64 entries (matrix rows and root frequencies; the class vector when C <= 64) first load the total and the
+// last entry of each 16-entry segment (one 128-byte line of a 64-padded row) together, so that a draw waits for memory
+// about once instead of once per probe; the segment they select holds the result (c is non-decreasing), and the search
+// inside it reads a line that is already in L1.  Longer vectors (C > 64 classes) take a plain binary search.
+__device__ __forceinline__ int sim_draw(const double *__restrict__ c, int m, const int *last, double u) {
+    int lo = 0, hi = m;
+    double t;
+    if (m > 16 && m <= 64) {
+        double b[3];
+#pragma unroll
+        for (int k = 0; k < 3; k++) b[k] = 16 * k + 15 < m ? __ldg(c + 16 * k + 15) : 0.0;
+        t = __dmul_rn(u, __ldg(c + m - 1));
+        int s = 0;
+#pragma unroll
+        for (int k = 0; k < 3; k++) s += (16 * k + 15 < m && b[k] <= t) ? 1 : 0;
+        lo = 16 * s;
+        hi = min(lo + 16, m);
+    } else {
+        t = __dmul_rn(u, __ldg(c + m - 1));
+    }
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (t < c[mid]) hi = mid; else lo = mid + 1;
+    }
+    return lo < m ? lo : *last;
+}
+
+struct SimArgs {
+    const double *PT;          // [C][B][Dp*Dp] transposed transition matrices
+    double *cdf;               // [C][B][D][Dp] prefix sums of each row (columns 0..D-1)
+    int *last;                 // [C][B][D] last column of positive weight of each row
+    const int *active;         // [C] 1 = the class has positive weight (its rows are built and checked)
+    int *bad;                  // first bad row ((c * B + b) * D + row), INT_MAX when none
+    const double *class_cdf;   // [C] prefix sums of the class weights
+    const double *root_cdf;    // [D] prefix sums of the root frequencies
+    const int *class_last;     // last class of positive weight
+    const int *root_last;      // last state of positive root frequency
+    TreeDev tree;
+    long long *leaf_out;       // [L][chunk]
+    long long *node_out;       // [I][chunk] or null
+    int *class_out;            // [chunk] or null
+    unsigned char *states;     // [I][chunk] internal states, used when they do not fit in shared memory (else null)
+    int L, I, B, C, D, Dp, chunk, n;
+    unsigned long long g0;     // global site of the chunk's first site
+    uint2 key;
+};
+
+// One CTA of 64 threads per (class, branch) of a drawn class; thread `row` forms the sequential prefix sums of its row
+// (PT column `row`: adjacent threads read adjacent doubles) in shared memory, padded to 65 doubles per row against bank
+// conflicts, and the CTA then stores the matrix's D x Dp block of the table with consecutive threads on consecutive
+// doubles.  A row whose total is not finite and > 0 is reported through atomicMin.
+constexpr int SIM_CDF_LD = 65;
+__global__ void __launch_bounds__(64) sim_cdf_kernel(SimArgs a) {
+    __shared__ double rows[64 * SIM_CDF_LD];
+    const long long cb = blockIdx.x;                       // class * B + branch
+    if (!a.active[cb / a.B]) return;                       // uniform over the CTA
+    const int row = threadIdx.x;
+    if (row < a.D) {
+        const double *P = a.PT + (size_t)cb * a.Dp * a.Dp + row;
+        double *c = rows + row * SIM_CDF_LD;
+        double s = 0.0;
+        int last = -1;
+#pragma unroll 4
+        for (int j = 0; j < a.D; j++) {
+            const double v = P[(size_t)j * a.Dp];
+            if (v > 0.0) { s = __dadd_rn(s, v); last = j; }
+            c[j] = s;
+        }
+        const long long r = cb * a.D + row;
+        a.last[r] = last;
+        if (!(s > 0.0 && s <= 1.7976931348623157e308)) atomicMin(a.bad, (int)r);
+    }
+    __syncthreads();
+    double *out = a.cdf + (size_t)cb * a.D * a.Dp;
+    for (int k = threadIdx.x; k < a.D * a.Dp; k += blockDim.x) {
+        const int rr = k / a.Dp, j = k - rr * a.Dp;
+        if (j < a.D) out[k] = rows[rr * SIM_CDF_LD + j];   // padded columns are never read
+    }
+}
+
+// One thread per site of the chunk: class, root state, then every internal node from the root down (flat post-order puts
+// a parent after its children), each child's state drawn from the row of its parent's state.  Internal states are bytes
+// in shared memory ([I][blockDim]) or, for trees with too many internal nodes, in global scratch ([I][chunk]).
+__global__ void __launch_bounds__(128) simulate_kernel(SimArgs a) {
+    extern __shared__ unsigned char sim_smem[];
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= a.n) return;
+    const unsigned long long g = a.g0 + (unsigned long long)i;
+    const int L = a.L, I = a.I;
+    unsigned char *st = a.states ? a.states + i : sim_smem + threadIdx.x;
+    const size_t stride = a.states ? (size_t)a.chunk : (size_t)blockDim.x;
+    const int cls = a.C == 1 ? 0 : sim_draw(a.class_cdf, a.C, a.class_last, sim_uniform(g, (unsigned)(L + I), a.key));
+    if (a.class_out) a.class_out[i] = cls;
+    int s = sim_draw(a.root_cdf, a.D, a.root_last, sim_uniform(g, (unsigned)(L + I - 1), a.key));
+    if (a.node_out) a.node_out[(size_t)(I - 1) * a.chunk + i] = s;
+    const size_t cls_rows = (size_t)cls * a.B;
+    for (int n = I - 1; n >= 0; n--) {
+        if (n < I - 1) s = st[(size_t)n * stride];
+        const int c_end = a.tree.child_start[n + 1];
+        for (int ci = a.tree.child_start[n]; ci < c_end; ci++) {
+            const int ch = a.tree.child_ids[ci];
+            const size_t r = (cls_rows + ch) * a.D + s;
+            const int x = sim_draw(a.cdf + r * a.Dp, a.D, a.last + r, sim_uniform(g, (unsigned)ch, a.key));
+            if (ch < L) {
+                a.leaf_out[(size_t)ch * a.chunk + i] = x;
+            } else {
+                st[(size_t)(ch - L) * stride] = (unsigned char)x;
+                if (a.node_out) a.node_out[(size_t)(ch - L) * a.chunk + i] = x;
+            }
+        }
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // Peer exchange over NVLink (one process per GPU; every rank maps every other rank's exchange buffer through CUDA IPC).
 // Buffer of a rank:  data[2 parities][R source ranks][payload doubles]  followed by  flags[2][R] (uint64 generation).
 // A writer stores its payload into slot `rank` of EVERY rank's buffer (its own included), fences system-wide and then

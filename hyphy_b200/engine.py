@@ -46,6 +46,7 @@ ABI = [
     ("hb2_batch_site_mixture_likelihoods", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, C.c_int64, _ip, _dp, _dp, _ip, _dp, _dp]),
     ("hb2_read_conditionals", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _dp, _i32p]),
     ("hb2_read_transition", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _dp]),
+    ("hb2_simulate", C.c_int, [C.c_void_p, _dp, _dp, C.c_int64, C.c_uint64, C.c_int64, _ip, _ip, _i32p]),
     ("hb2_comm_unique_id", C.c_int, [C.c_void_p]),
     ("hb2_branch_cache_build", C.c_int, [C.c_void_p, C.c_int64, _dp]),
     ("hb2_branch_cache_evaluate", C.c_int, [C.c_void_p, C.c_int64, _dp, C.POINTER(C.c_double), _dp, _ip]),
@@ -309,6 +310,25 @@ class Partition:
         _check(self._lib.hb2_read_transition(self._h, int(cat), int(node), P.ctypes.data_as(_dp)))
         return P
 
+    # -- SimulateDataSet ---------------------------------------------------------------------------
+    def simulate(self, n_sites, root_freqs, weights=None, seed=0, first_site=0, want_nodes=False, want_classes=False):
+        """Sites first_site .. first_site + n_sites - 1 of the simulation stream `seed` (hb2_simulate) from the current
+        matrices.  Returns (leaf states [L, n] int64, internal-node states [I, n] int64 or None, classes [n] int32 or None)."""
+        n = int(n_sites)
+        pi, ppi = _d(root_freqs)
+        assert pi.shape == (self.D,)
+        pw = None
+        if weights is not None:
+            w, pw = _d(weights)
+            assert w.shape == (self.C,)
+        leaf = np.empty((self.L, max(n, 0)), dtype=np.int64)
+        nodes = np.empty((self.I, max(n, 0)), dtype=np.int64) if want_nodes else None
+        classes = np.empty(max(n, 0), dtype=np.int32) if want_classes else None
+        _check(self._lib.hb2_simulate(self._h, pw, ppi, n, int(seed) & 0xFFFFFFFFFFFFFFFF, int(first_site), leaf.ctypes.data_as(_ip),
+                                      nodes.ctypes.data_as(_ip) if want_nodes else None,
+                                      classes.ctypes.data_as(_i32p) if want_classes else None))
+        return leaf, nodes, classes
+
     # -- multi-GPU ---------------------------------------------------------------------------------
     @staticmethod
     def comm_unique_id() -> bytes:
@@ -383,6 +403,7 @@ class LikelihoodFunction:
       set_all_matrices   ExponentiateMatrices tree.cpp:2932 (every branch, every rate class)
       compute_block      ComputeBlock         likefunc.cpp:10783 (one rate class; optional per-pattern outputs)
       compute            Compute              likefunc.cpp:2421 (category path fused on device)
+      simulate           SimulateDataSet      likefunc.cpp:12584 (discrete-category mode)
       close              DeleteCaches         likefunc.cpp:10556
     """
 
@@ -417,6 +438,11 @@ class LikelihoodFunction:
     def compute(self, update_nodes=None, want_sites=False, weights=None):
         wts = self.w.class_weights if weights is None else weights
         return self.part.evaluate_classes(wts, self.w.pi, update_nodes, want_sites)
+
+    def simulate(self, n_sites, seed=0, first_site=0, want_nodes=False, want_classes=False):
+        """SimulateDataSet from the current matrices with the workload's root frequencies and class weights:
+        (leaf states [L, n], internal-node states [I, n] | None, classes [n] | None); see Partition.simulate."""
+        return self.part.simulate(n_sites, self.w.pi, self.w.class_weights, seed, first_site, want_nodes, want_classes)
 
     def close(self):
         self.part.close()

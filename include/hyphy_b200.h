@@ -179,6 +179,35 @@ int hb2_read_conditionals(hb2_partition *p, int64_t cat, int64_t inode, double *
 /* Read back the transition matrix currently cached for (cat, node): D*D doubles, row = parent state. */
 int hb2_read_transition(hb2_partition *p, int64_t cat, int64_t node, double *P);
 
+/* Simulated alignment columns from the partition's current transition matrices (SimulateDataSet, likefunc.cpp:12584,
+ * discrete-category mode: every site draws one rate class and evolves down the tree with that class's matrices).  Site i
+ * of the call is global site g = firstSite + i of the stream `seed`, so a replicate may be produced in any number of calls.
+ *   weights    C class weights, not necessarily normalised; NULL only when C == 1.  A class of weight 0 is never drawn and
+ *              its matrices need not exist.
+ *   rootFreqs  D root-state weights.
+ *   leafStates [L][nSites]: leafStates[l*nSites + i], hb2_create's leafState layout (a block can be handed to hb2_create as
+ *              nSites patterns of frequency 1).
+ *   nodeStates nullable [I][nSites]: internal-node states, root at I-1 (the reference's storeIntermediates).
+ *   siteClass  nullable [nSites]: the drawn class of every site.
+ * The matrices are those hb2_read_transition returns (pending hand-overs are flushed first): dense, compiled and mixture
+ * hand-overs alike, on every kernel family.
+ * The stream (results depend on matrices, weights, rootFreqs, seed and g only -- not on chunking or launch shape):
+ *   - one Philox4x32-10 call per draw: counter = (lo32(g), hi32(g), slot, 0), key = (lo32(seed), hi32(seed));
+ *   - slot n in 0..L+I-2: flat node n's state drawn from its parent's row; slot L+I-1: the root state; slot L+I: the class;
+ *   - uniform u = (x0 * 2^21 + (x1 >> 11)) * 2^-53 from the first two output words.
+ * The draw rule for a weight vector v[0..m-1] (a matrix row: row = parent state, columns 0..D-1):
+ *   - entries that are not > 0 (negative, zero, NaN) count as 0;
+ *   - c_j = sequential fp64 prefix sum over j = 0..m-1, T = c_{m-1};
+ *   - the result is the smallest j with fl(u*T) < c_j, or, when there is none, the largest j with v_j > 0.
+ * Refusals (a refused call writes no output): nSites < 0; firstSite < 0; negative or NaN weights or rootFreqs, or a total
+ * that is not finite and > 0; NULL weights with C > 1; a class of positive weight with a branch that never received a
+ * matrix; a matrix row of such a class whose total is not finite and > 0 (checked on the device, reported with class,
+ * node and row); class-group mode (hb2_comm_class_groups: a rank does not hold the other groups' matrices).  Pattern-sharded
+ * ranks simulate from their own copy of the matrices.  nSites == 0 after these checks does nothing.
+ * Nothing an evaluation reads is touched: conditionals, scalers, walk plans and tags, the branch cache, the root vector. */
+int hb2_simulate(hb2_partition *p, const double *weights, const double *rootFreqs, int64_t nSites, uint64_t seed,
+                 int64_t firstSite, int64_t *leafStates, int64_t *nodeStates, int32_t *siteClass);
+
 /* Multi-GPU (one process per GPU, patterns sharded by the caller: each rank creates its partition with its own
  * pattern shard).  After hb2_comm_init every hb2_evaluate* returns the SUM over ranks of the partial lnL
  * (a single fp64 ncclAllReduce on the partition's stream; per-pattern outputs stay local to the shard).
