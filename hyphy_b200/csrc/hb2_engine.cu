@@ -349,6 +349,10 @@ struct hb2_partition {
         size_t cap[7] = {0, 0, 0, 0, 0, 0, 0};
     } sim;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
+    // side stream of the expm stage: the power tables are built on it while the classification runs on `stream`
+    // (launch_expm forks at ev_fork and joins at ev_join)
+    cudaStream_t side = nullptr;
+    cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     // recorded after uploads from pinned staging (the queues, ExBuf::h_int, column frequencies, mixtures, the replay's
     // slots): every writer of those buffers waits for it first
     cudaEvent_t ev_staging = nullptr;
@@ -411,6 +415,12 @@ int plan_shared(hb2_partition *p, const int *h_dst, int64_t n, int kind, const i
     }
     if (!any) return 0;
     for (int64_t k = 0; k < n; k++) ref[k] = grp[k] >= 0 ? first[grp[k]] : -1;
+    // launch_expm rebuilds the power tables beside the classification, and expm_powers_kernel rewrites the cached
+    // direction and record of every group it rebuilds, which the classification reads for entries without a reference in
+    // the batch: no group may have both in one batch.
+    for (int64_t k = 0; k < n; k++)
+        if (grp[k] >= 0 && ref[k] < 0 && first[grp[k]] >= 0)
+            return fail("plan_shared: entry %lld of group %d has no reference although the group's table is rebuilt", (long long)k, grp[k]);
     for (int r = 0; r < nr; r++) x.kind[grp[refs[r]]] = kind;
     CU(cudaMemcpyAsync(x.d_int, x.h_int, (size_t)(2 * x.cap + x.G) * sizeof(int), cudaMemcpyHostToDevice, p->stream));
     sp.use = true; sp.kind = kind; sp.n_refs = nr;
@@ -457,26 +467,32 @@ int launch_expm(hb2_partition *p, Source src, const double *in, const int *d_dst
             if (sp.use && src.kind != Kind::Trans) {
                 hb2_partition::ExBuf &x = *sp.x;
                 const int nV = t ? (int)t->nF : (int)(p->D * p->D);
-                const hb2::ExpmGroup *groups = x.d_groups;
-                hb2::ExpmClassifyArgs ca{};
-                ca.V = in; ca.nV = nV; ca.kind = sp.kind; ca.dst = d_dst; ca.group = x.d_int + off;
-                ca.ref = x.d_int + x.cap + off; ca.groups = groups; ca.refvec = x.d_refvec; ca.refvec_stride = x.stride;
-                ca.weight = x.d_weight + off; ca.flag = x.d_flag + off;
-                ca.res = !keep_resident ? nullptr : t ? (double *)t->d_Vres : (double *)p->d_Qres;
                 // references index the whole batch: classification has to see it in one piece (off == 0 for compiled batches
                 // and for dense batches that consist of a single run; mixed dense batches fall back below)
-                if (nV <= 256) hb2::expm_classify_warp_kernel<<<(n + 7) / 8, 256, 0, p->stream>>>(ca, n);
-                else hb2::expm_classify_kernel<<<n, 128, 0, p->stream>>>(ca);
-                a.group = ca.group; a.flag = ca.flag; a.weight = ca.weight; a.groups = groups; a.pow = x.d_pow;
+                a.group = x.d_int + off; a.flag = x.d_flag + off; a.weight = x.d_weight + off; a.groups = x.d_groups;
+                a.pow = x.d_pow;
                 a.Qres = nullptr;                    // the classification stage keeps the resident copy
+                // the power tables are built on the side stream while the classification runs (plan_shared keeps the two
+                // from touching the same group)
                 if (sp.n_refs > 0) {
                     hb2::ExpmPowersArgs pa{};
                     pa.a = a; pa.refs = x.d_int + 2 * x.cap; pa.groups = x.d_groups;
                     pa.pow = x.d_pow; pa.refvec = x.d_refvec; pa.refvec_stride = x.stride; pa.nV = nV; pa.kind = sp.kind; pa.Vin = in;
                     pa.flags = x.d_flags; pa.gen = ++x.gen; pa.err = p->d_err;
-                    hb2::expm_powers_kernel<<<dim3(hb2::EXPM_POW_TERMS - 1, (unsigned)sp.n_refs), 256, smem, p->stream>>>(pa);
+                    CU(cudaEventRecord(p->ev_fork, p->stream));
+                    CU(cudaStreamWaitEvent(p->side, p->ev_fork, 0));
+                    hb2::expm_powers_kernel<<<dim3(hb2::EXPM_POW_TERMS - 1, (unsigned)sp.n_refs), 256, smem, p->side>>>(pa);
                     p->launches++;
+                    CU(cudaEventRecord(p->ev_join, p->side));
                 }
+                hb2::ExpmClassifyArgs ca{};
+                ca.V = in; ca.nV = nV; ca.kind = sp.kind; ca.dst = d_dst; ca.group = x.d_int + off;
+                ca.ref = x.d_int + x.cap + off; ca.groups = x.d_groups; ca.refvec = x.d_refvec; ca.refvec_stride = x.stride;
+                ca.weight = x.d_weight + off; ca.flag = x.d_flag + off;
+                ca.res = !keep_resident ? nullptr : t ? (double *)t->d_Vres : (double *)p->d_Qres;
+                if (nV <= 256) hb2::expm_classify_warp_kernel<<<(n + 7) / 8, 256, 0, p->stream>>>(ca, n);
+                else hb2::expm_classify_kernel<<<n, 128, 0, p->stream>>>(ca);
+                if (sp.n_refs > 0) CU(cudaStreamWaitEvent(p->stream, p->ev_join, 0));
                 cudaLaunchConfig_t cfg{};
                 cfg.gridDim = dim3(hb2::EXPM_POLY_CLUSTER, (unsigned)((n + hb2::EXPM_POLY_CHUNK - 1) / hb2::EXPM_POLY_CHUNK));
                 cfg.blockDim = dim3(256);
@@ -1332,6 +1348,9 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
     CU(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
     for (auto &e : p->ev) CU(cudaEventCreate(&e));
     CU(cudaEventCreateWithFlags(&p->ev_staging, cudaEventDisableTiming));
+    CU(cudaStreamCreateWithFlags(&p->side, cudaStreamNonBlocking));
+    CU(cudaEventCreateWithFlags(&p->ev_fork, cudaEventDisableTiming));
+    CU(cudaEventCreateWithFlags(&p->ev_join, cudaEventDisableTiming));
     const size_t Sp = p->Sp, dpdp = (size_t)Dp * Dp, dd = (size_t)D * D;
     cudaStream_t st = p->stream;
     if (p->d_leaf.alloc(L * Sp) || p->d_ambig.alloc(std::max<int64_t>(nAmb, 1) * Dp) || p->d_freq.alloc(Sp)) return 1;
@@ -2036,13 +2055,14 @@ void hb2_destroy(hb2_partition *p) {
     if (!p) return;
     cudaSetDevice(p->device);
     if (p->stream) cudaStreamSynchronize(p->stream);     // first: the pool may hand the released blocks out at once
+    if (p->side) cudaStreamSynchronize(p->side);
     peer_teardown(p);
     if (p->comm) g_nccl.CommDestroy(p->comm);
-    const cudaStream_t stream = p->stream;
-    const cudaEvent_t events[] = {p->ev[0], p->ev[1], p->ev[2], p->ev[3], p->ev_staging};
+    const cudaStream_t streams[] = {p->stream, p->side};
+    const cudaEvent_t events[] = {p->ev[0], p->ev[1], p->ev[2], p->ev[3], p->ev_staging, p->ev_fork, p->ev_join};
     delete p;                                             // releases every buffer
     for (cudaEvent_t e : events) if (e) cudaEventDestroy(e);
-    if (stream) cudaStreamDestroy(stream);
+    for (cudaStream_t s : streams) if (s) cudaStreamDestroy(s);
 }
 
 int64_t hb2_launch_count(const hb2_partition *p) { return p ? p->launches : 0; }

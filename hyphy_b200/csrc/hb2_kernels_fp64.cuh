@@ -171,8 +171,10 @@ __device__ __forceinline__ void load_rate_matrix(const ExpmArgs &a, double *A1, 
             for (int idx = tid; idx < D * D; idx += NT) { const int i = idx / D, j = idx - i * D; a.Qres[slot * D * D + idx] = A1[j * LD + i]; }
     } else {
         const double *Q = a.Q + (size_t)entry * D * D;
-        for (int idx = tid; idx < DP * DP; idx += NT) {
-            const int i = idx / DP, j = idx - i * DP;
+#pragma unroll                                    // every load of the thread in flight at once
+        for (int it = 0; it < (DP * DP + NT - 1) / NT; it++) {
+            const int idx = tid + it * NT, i = idx / DP, j = idx - i * DP;
+            if (idx >= DP * DP) break;
             const double v = (i < D && j < D) ? Q[(size_t)i * D + j] : 0.0;
             A1[j * LD + i] = v;
             if (a.Qres && i < D && j < D) a.Qres[slot * D * D + (size_t)i * D + j] = v;
@@ -248,7 +250,7 @@ struct ExpmClassifyArgs {
     const int *dst;           // [n]
     const int *group;         // [n]
     const int *ref;           // [n] batch index of the group's reference entry, or -1: use the cached direction
-    const ExpmGroup *groups;  // [G]
+    ExpmGroup *groups;        // [G]; the weight of a group whose reference entry is in the batch is written here
     const double *refvec;     // [G][nVmax] cached reference directions
     int refvec_stride;
     double *weight;           // out [n]
@@ -256,26 +258,56 @@ struct ExpmClassifyArgs {
     double *res;              // nullable: resident copy [slots][nV]
 };
 
+// What both classification kernels do once an entry's sums and flag are known.  The weight of a group's reference entry
+// (k == ref[k]) goes to the group's record here rather than in expm_powers_kernel, which runs at the same time on the
+// partition's side stream and writes only the other fields (nu, kind).
+__device__ __forceinline__ void expm_classify_result(const ExpmClassifyArgs &a, int k, int g, int r, int ok, double wk) {
+    a.flag[k] = ok;
+    a.weight[k] = wk;
+    if (g >= 0 && r == k) a.groups[g].weight = wk;
+}
+
+// Inputs of more than 256 values (dense: nV = D*D <= 4096): each thread holds its up to EXPM_CLASSIFY_REGS values of the
+// entry and of the reference in registers, all loads issued before any sum, so the entry is read from memory once and the
+// proportionality check runs from registers.  Values f = tid + 128 i are summed in increasing i, as a plain strided loop
+// would; the loop past the register tile only serves longer compiled inputs.
+constexpr int EXPM_CLASSIFY_REGS = 32;
 __global__ void __launch_bounds__(128) expm_classify_kernel(ExpmClassifyArgs a) {
     __shared__ double red[2][4];
     __shared__ int bad[4];
-    const int k = blockIdx.x, tid = threadIdx.x;
+    const int k = blockIdx.x, tid = threadIdx.x, nV = a.nV;
     const int slot = a.dst[k];
     if (slot < 0) { if (tid == 0) { a.flag[k] = 0; a.weight[k] = 0.0; } return; }
-    const double *v = a.V + (size_t)k * a.nV;
+    const double *v = a.V + (size_t)k * nV;
     const int g = a.group[k], r = a.ref[k];
     const double *vr = nullptr;
     double wr_cached = -1.0;
     if (g >= 0) {
-        if (r >= 0) vr = a.V + (size_t)r * a.nV;
+        if (r >= 0) vr = a.V + (size_t)r * nV;
         else if (a.groups[g].kind == a.kind) { vr = a.refvec + (size_t)g * a.refvec_stride; wr_cached = a.groups[g].weight; }
     }
+    double xv[EXPM_CLASSIFY_REGS], xr[EXPM_CLASSIFY_REGS];
+#pragma unroll
+    for (int i = 0; i < EXPM_CLASSIFY_REGS; i++) {
+        const int f = tid + 128 * i;
+        xv[i] = f < nV ? v[f] : 0.0;
+        xr[i] = vr && f < nV ? vr[f] : 0.0;
+    }
     double wk = 0.0, wr = 0.0;
-    for (int f = tid; f < a.nV; f += 128) {
-        const double x = v[f];
-        wk += fabs(x);
+#pragma unroll
+    for (int i = 0; i < EXPM_CLASSIFY_REGS; i++) {       // the zeros past nV leave the (non-negative) sums unchanged
+        wk += fabs(xv[i]);
+        wr += fabs(xr[i]);
+    }
+    for (int f = tid + 128 * EXPM_CLASSIFY_REGS; f < nV; f += 128) {
+        wk += fabs(v[f]);
         if (vr) wr += fabs(vr[f]);
-        if (a.res) a.res[(size_t)slot * a.nV + f] = x;
+    }
+    if (a.res) {
+        double *res = a.res + (size_t)slot * nV;
+#pragma unroll
+        for (int i = 0; i < EXPM_CLASSIFY_REGS; i++) if (tid + 128 * i < nV) res[tid + 128 * i] = xv[i];
+        for (int f = tid + 128 * EXPM_CLASSIFY_REGS; f < nV; f += 128) res[f] = v[f];
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) { wk += __shfl_xor_sync(0xffffffffu, wk, o); wr += __shfl_xor_sync(0xffffffffu, wr, o); }
@@ -287,16 +319,16 @@ __global__ void __launch_bounds__(128) expm_classify_kernel(ExpmClassifyArgs a) 
     int ok = (vr != nullptr) && (wr > 0.0) && (wk >= 0.0) && (wk < INFINITY) && (wr < INFINITY);   // NaN fails every comparison
     if (ok) {
         const double tol = 1e-13 * wk * wr;
-        for (int f = tid; f < a.nV; f += 128)
+#pragma unroll
+        for (int i = 0; i < EXPM_CLASSIFY_REGS; i++)
+            if (tid + 128 * i < nV && !(fabs(xv[i] * wr - xr[i] * wk) <= tol)) ok = 0;
+        for (int f = tid + 128 * EXPM_CLASSIFY_REGS; f < nV; f += 128)
             if (!(fabs(v[f] * wr - vr[f] * wk) <= tol)) ok = 0;
     }
     ok = __all_sync(0xffffffffu, ok);
     if ((tid & 31) == 0) bad[tid >> 5] = !ok;
     __syncthreads();
-    if (tid == 0) {
-        a.flag[k] = !(bad[0] | bad[1] | bad[2] | bad[3]);
-        a.weight[k] = wk;
-    }
+    if (tid == 0) expm_classify_result(a, k, g, r, !(bad[0] | bad[1] | bad[2] | bad[3]), wk);
 }
 
 // The same classification with one WARP per entry, eight entries per CTA, for short inputs (compiled hand-overs: ~50 formula
@@ -332,7 +364,7 @@ __global__ void __launch_bounds__(256) expm_classify_warp_kernel(ExpmClassifyArg
             if (!(fabs(v[f] * wr - vr[f] * wk) <= tol)) ok = 0;
     }
     ok = __all_sync(0xffffffffu, ok);
-    if (lane == 0) { a.flag[k] = ok; a.weight[k] = wk; }
+    if (lane == 0) expm_classify_result(a, k, g, r, ok, wk);
 }
 
 // Shared-powers entry k: rho = ||A_k||_inf estimated from its weight, and the squarings expm_poly_kernel chose for it.
@@ -549,15 +581,17 @@ __global__ void __launch_bounds__(256, 2) expm64_dmma_kernel(ExpmArgs a, ExpmTcO
 // Shared-powers path, stage 2: S_m = R^m / m! (PT layout, i.e. powers of the TRANSPOSED reference matrix), m = 1..24, for
 // every group whose reference is (re)established in this batch.  grid = (24, number of such groups); CTA (j, g) produces
 // S_{j+1}:  j = 0 assembles the reference matrix, normalises it (R = A_ref / ||A_ref||_inf -> S_1) and records the
-// group's measures and direction; CTA j >= 1 multiplies two EARLIER coefficient matrices,
+// group's nu, kind and direction; CTA j >= 1 multiplies two EARLIER coefficient matrices,
 //     S_m = S_a S_b / C(m, a),   (a, b) = (1,1) (2,1) (2,2) (4,1..4) (8,1..8) (16,1..8),
 // which it awaits on generation flags (flag[group][m] == gen once S_m is complete; the producer fences before it
 // publishes).  Blocks are dispatched in index order and only wait for lower indices of their own column, so the scheme
 // cannot deadlock even if not all of them are co-resident; waits are time-bounded like every device-side wait here.
-// Critical path: 5 products instead of 23.
+// Critical path: 5 products instead of 23.  The kernel runs on the partition's side stream while the classification runs
+// (launch_expm), so it reads none of the classification's outputs and writes nothing the classification reads for the
+// batch: the groups it rebuilds have no entry classified against their cached direction (plan_shared).
 // ------------------------------------------------------------------------------------------------
 struct ExpmPowersArgs {
-    ExpmArgs a;               // input description (dense or compiled); a.Qres must be null
+    ExpmArgs a;               // input description (dense or compiled); a.Qres must be null, a.weight / a.flag unused
     const int *refs;          // [gridDim.y] batch indices of the reference entries
     ExpmGroup *groups;        // out
     double *pow;              // out [G][EXPM_POW_TERMS][4096]
@@ -605,34 +639,37 @@ __global__ void __launch_bounds__(256, 1) expm_powers_kernel(ExpmPowersArgs pa) 
             red[tid] = s;
         }
         __syncthreads();
-        if (tid == 0) {
-            double mx = 0.0;
-            bool bad = false;
-            for (int i = 0; i < 64; i++) { if (!(red[i] == red[i]) || isinf(red[i])) bad = true; mx = fmax(mx, red[i]); }
-            s_nu = (bad || !(mx > 0.0)) ? 0.0 : mx;
+        if (tid < 32) {                      // max and NaN / inf scan of the 64 row sums, one warp (fmax is exact)
+            double mx = fmax(0.0, fmax(red[tid], red[tid + 32]));
+            bool bad = !(red[tid] == red[tid]) || !(red[tid + 32] == red[tid + 32]) || isinf(red[tid]) || isinf(red[tid + 32]);
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+            bad = __any_sync(0xffffffffu, bad);
+            if (tid == 0) s_nu = (bad || !(mx > 0.0)) ? 0.0 : mx;
         }
         __syncthreads();
         const double nu = s_nu;
-        if (tid == 0) {
-            ExpmGroup gi;
-            gi.nu = nu; gi.weight = pa.a.weight[entry]; gi.kind = nu > 0.0 ? pa.kind : 0; gi.pad = 0;
-            pa.groups[grp] = gi;
+        if (tid == 0) {                      // the weight is the classification's (expm_classify_result), written beside this
+            pa.groups[grp].nu = nu;
+            pa.groups[grp].kind = nu > 0.0 ? pa.kind : 0;
         }
-        for (int f = tid; f < pa.nV; f += 256) pa.refvec[(size_t)grp * pa.refvec_stride + f] = pa.Vin[(size_t)entry * pa.nV + f];
         // (no entry can have been flagged against a reference with nu == 0; the other CTAs of the column still need S_1)
         const double inv = nu > 0.0 ? 1.0 / nu : 0.0;
         for (int idx = tid; idx < 4096; idx += 256) pw[4096 + idx] = X0[(idx >> 6) * LD64 + (idx & 63)] * inv;
         __threadfence();
         __syncthreads();
         if (tid == 0) asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(flags + 1), "l"(pa.gen) : "memory");
+        // the direction is read by later batches only: off the critical path of the products
+        for (int f = tid; f < pa.nV; f += 256) pa.refvec[(size_t)grp * pa.refvec_stride + f] = pa.Vin[(size_t)entry * pa.nV + f];
         return;
     }
     const int a = m <= 2 ? 1 : m <= 4 ? 2 : m <= 8 ? 4 : m <= 16 ? 8 : 16, b = m - a;
     if (tid == 0) expm_await_flag(flags + a, pa.gen, pa.err);
     if (tid == 32) expm_await_flag(flags + b, pa.gen, pa.err);
     __syncthreads();
-    for (int idx = tid; idx < 2048; idx += 256) {                     // both operands as double2, coalesced
-        const int r = idx >> 5, c2 = (idx & 31) * 2;
+#pragma unroll
+    for (int it = 0; it < 8; it++) {                                  // both operands as double2, coalesced, all loads in flight
+        const int idx = tid + 256 * it, r = idx >> 5, c2 = (idx & 31) * 2;
         *reinterpret_cast<double2 *>(X0 + r * LD64 + c2) = __ldcg(reinterpret_cast<const double2 *>(pw + (size_t)a * 4096 + r * 64 + c2));
         *reinterpret_cast<double2 *>(X1 + r * LD64 + c2) = __ldcg(reinterpret_cast<const double2 *>(pw + (size_t)b * 4096 + r * 64 + c2));
     }
