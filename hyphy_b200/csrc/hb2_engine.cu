@@ -279,6 +279,8 @@ struct hb2_partition {
     DeviceBuffer<int> d_bdst, d_bpat, d_bnodeex;
     PinnedBuffer<int> h_bdst;
     DeviceBuffer<int> d_brow;                 // first component row of each branch [B+1]
+    DeviceBuffer<int> d_bcol;                 // caller columns of a chunk (hb2_batch_column_likelihoods) [L][sets]
+    DeviceBuffer<double> d_bpi;               // root vector of the batch calls (the staged d_pi stays the evaluations')
     int b_groups_per_set = 1;
     bool ex_enabled = true;                   // HB2_EXPM_SHARED=0 switches the path off (A/B testing)
     int64_t stage_launches[3] = {0, 0, 0};    // launches per evaluation of the last hb2_time_resident {expm, pruning, root}
@@ -339,8 +341,8 @@ struct hb2_partition {
     std::vector<double *> px_peer;            // host copy of the mapped pointers (entry rank = px_local)
     DeviceBuffer<double *> d_px_peer;
     DeviceBuffer<unsigned> d_px_counter;
-    // simulation scratch (hb2_simulate), grown on demand and used by nothing else: the prefix-sum table, the call's small
-    // vectors, and one chunk of leaf / node / class outputs and internal states
+    // simulation scratch (hb2_simulate, hb2_batch_site_simulate), grown on demand and used by nothing else: the prefix-sum
+    // table, the call's small vectors, and one chunk of leaf / node / class outputs and internal states
     struct SimBuf {
         DeviceBuffer<double> cdf, vec;
         DeviceBuffer<int> ints, cls;
@@ -609,13 +611,13 @@ int enqueue(hb2_partition *p, int queue, int64_t slot, const double *row, Kind k
     return 0;
 }
 
-// Stages the root vector, zero-padded to Dp (unless null), and the first nw class weights (when given).  Every caller
-// synchronises the stream before it returns, so h_small is free again at the next call.
-int stage_root(hb2_partition *p, const double *rootFreqs, const double *weights = nullptr, int nw = 0) {
+// Stages the root vector, zero-padded to Dp (unless null), into d_pi (or dst), and the first nw class weights (when given).
+// Every caller synchronises the stream before it returns, so h_small is free again at the next call.
+int stage_root(hb2_partition *p, const double *rootFreqs, const double *weights = nullptr, int nw = 0, double *dst = nullptr) {
     double *hs = p->h_small;
     if (rootFreqs) {
         for (int k = 0; k < p->Dp; k++) hs[k] = k < p->D ? rootFreqs[k] : 0.0;
-        CU(cudaMemcpyAsync(p->d_pi, hs, p->Dp * sizeof(double), cudaMemcpyHostToDevice, p->stream));
+        CU(cudaMemcpyAsync(dst ? dst : (double *)p->d_pi, hs, p->Dp * sizeof(double), cudaMemcpyHostToDevice, p->stream));
     }
     if (weights) {
         for (int c = 0; c < nw; c++) hs[p->Dp + c] = weights[c];
@@ -1608,13 +1610,25 @@ int hb2_evaluate_classes(hb2_partition *p, const double *weights, int64_t nUpdat
     return evaluate_impl(p, 0, (int)p->C, weights, nUpdate, updateNodes, rootFreqs, lnL, siteL, siteScale);
 }
 
-// Body of both batch entry points.  weights == nullptr: one matrix per branch, row b = branch b (FEL's site model).
+// What a batch call produces.  Likelihoods (siteLnL) of partition patterns (patternOf) or of caller columns (columns
+// [nSets][L], hb2_create's leaf codes); or, with sim, nReps simulated columns of every set.
+struct BatchJob {
+    const int64_t *patternOf = nullptr, *columns = nullptr;
+    double *siteLnL = nullptr;
+    bool sim = false;
+    int64_t nReps = 0, firstSet = 0, firstRep = 0;
+    uint64_t seed = 0;
+    int64_t *leafStates = nullptr, *nodeStates = nullptr;
+};
+
+// Body of every batch entry point.  weights == nullptr: one matrix per branch, row b = branch b (FEL's site model).
 // Otherwise branch b owns branchK[b] (NULL: K) consecutive component rows and its transition matrix is the weighted sum of
-// their exponentials, formed inside prune_batch_kernel<true> (MEME's site model).
-static int batch_sites(hb2_partition *p, int64_t templateId, int64_t nSets, const int64_t *patternOf, int64_t K, const int64_t *branchK,
+// their exponentials, formed inside prune_batch_kernel<true> or sim_cdf_kernel<true> (MEME's site model).
+static int batch_sites(hb2_partition *p, int64_t templateId, int64_t nSets, int64_t K, const int64_t *branchK,
                        const double *formulaValues, const double *weights, const int64_t *branchGroup, const double *rootFreqs,
-                       double *siteLnL) {
-    if (!p || !patternOf || !formulaValues || !rootFreqs || !siteLnL) return fail("null argument");
+                       const BatchJob &job) {
+    if (!p || !formulaValues || !rootFreqs || (job.sim ? !job.leafStates : (!job.siteLnL || !(job.patternOf || job.columns))))
+        return fail("null argument");
     if (nSets < 0) return fail("bad set count");
     if (p->Dp != 64) return fail("hb2_batch_site_likelihoods supports 33..64-state (codon) partitions only");
     if (templateId < 0 || templateId >= (int64_t)p->tmpls.size() || p->tmpls[templateId].nnz == 0) return fail("template %lld has not been defined", (long long)templateId);
@@ -1625,12 +1639,23 @@ static int batch_sites(hb2_partition *p, int64_t templateId, int64_t nSets, cons
             if (branchGroup[b] < 0 || branchGroup[b] >= 8) return fail("branchGroup[%lld]=%lld outside 0..7", (long long)b, (long long)branchGroup[b]);
             gps = std::max(gps, (int)branchGroup[b] + 1);
         }
-    for (int64_t s = 0; s < nSets; s++)
-        if (patternOf[s] < 0 || patternOf[s] >= p->S) return fail("patternOf[%lld]=%lld out of range", (long long)s, (long long)patternOf[s]);
-    if (nSets == 0) return 0;
+    for (int64_t s = 0; job.patternOf && s < nSets; s++)
+        if (job.patternOf[s] < 0 || job.patternOf[s] >= p->S) return fail("patternOf[%lld]=%lld out of range", (long long)s, (long long)job.patternOf[s]);
+    for (int64_t s = 0; job.columns && s < nSets; s++)
+        for (int64_t l = 0; l < p->L; l++) {
+            const int64_t c = job.columns[s * p->L + l];
+            if (c >= p->D || c < -p->nAmb)
+                return fail("hb2_batch_column_likelihoods: set %lld, leaf %lld: code %lld is neither a state 0..%lld nor an ambiguity row -1..-%lld",
+                            (long long)s, (long long)l, (long long)c, (long long)p->D - 1, (long long)p->nAmb);
+        }
+    std::vector<double> root_cdf(p->D);
+    int root_last = -1;
+    if (job.sim && !sim_prefix(rootFreqs, p->D, root_cdf.data(), &root_last))
+        return fail("hb2_batch_site_simulate: root frequencies must be >= 0 and not NaN, with a finite positive total");
+    if (nSets == 0 || (job.sim && job.nReps == 0)) return 0;
     CU(cudaSetDevice(p->device));
     const hb2_partition::Tmpl &t = p->tmpls[templateId];
-    const int64_t B = p->B, nF = t.nF;
+    const int64_t B = p->B, nF = t.nF, D = p->D, L = p->L, I = p->I;
     const bool mix = weights != nullptr;
     // component rows of a set: branch b owns rows row_off[b] .. row_off[b+1]-1.  Component k of every tested branch is the
     // same rate matrix up to the branch length, so the shared-powers group of a row is (set, branchGroup[b], k).
@@ -1638,14 +1663,15 @@ static int batch_sites(hb2_partition *p, int64_t templateId, int64_t nSets, cons
     for (int64_t b = 0; b < B; b++) row_off[b + 1] = row_off[b] + (int)(mix && branchK ? branchK[b] : K);
     const int64_t R = row_off[B];
     const int gk = gps * (int)K;                // groups per set
-    // chunk buffers, capped at ~8 GB
+    // chunk buffers, capped at ~8 GB; a simulation adds the prefix sums and last positive columns of the set's B matrices
+    const double sim_bytes = job.sim ? (double)B * D * (64 * 8 + 4) : 0.0;
     int64_t cap;
     if (!mix)                                   // P matrices of `cap` sets (32 KB per branch)
-        cap = std::min<int64_t>(nSets, std::max<int64_t>(1, (int64_t)(8.0e9 / ((double)B * (4096 + 1024 + (double)nF) * 8))));
+        cap = std::min<int64_t>(nSets, std::max<int64_t>(1, (int64_t)(8.0e9 / ((double)B * (4096 + 1024 + (double)nF) * 8 + sim_bytes))));
     else {                                      // a set's R component matrices, formula values and weights,
                                                 // the power tables of its groups and its node vectors
         const double per_set = (double)R * (4096 + (double)nF + 1) * 8 + (double)gk * hb2::EXPM_POW_TERMS * 4096 * 8 + (double)p->I * 64 * 8;
-        cap = std::min<int64_t>(nSets, std::max<int64_t>(1, (int64_t)(8.0e9 / per_set)));
+        cap = std::min<int64_t>(nSets, std::max<int64_t>(1, (int64_t)(8.0e9 / (per_set + sim_bytes))));
     }
     cap = std::min<int64_t>(cap, 1024);
     // the buffers hold b_cap sets of up to bex.cap / b_cap rows; chunks are b_cap sets wherever they came from
@@ -1655,21 +1681,63 @@ static int batch_sites(hb2_partition *p, int64_t templateId, int64_t nSets, cons
         const int64_t ne = cap * R;
         if (p->bex.alloc((int)(cap * gk), ne, p->stream) || p->d_bPT.alloc((size_t)ne * 4096) || p->d_bV.alloc((size_t)ne * nF) ||
             p->d_bcond.alloc((size_t)cap * p->I * 64) || p->d_bnodeex.alloc((size_t)cap * p->I) || p->d_bout.alloc(cap) || p->d_bdst.alloc(ne) ||
-            p->d_bpat.alloc(cap) || p->h_bdst.alloc(ne + cap) || p->d_bmixw.alloc(ne) || p->d_brow.alloc(B + 1))
+            p->d_bpat.alloc(cap) || p->h_bdst.alloc(ne + cap + cap * L) || p->d_bmixw.alloc(ne) || p->d_brow.alloc(B + 1) ||
+            p->d_bcol.alloc((size_t)cap * L) || p->d_bpi.alloc(64))
             return 1;
         p->b_cap = cap; p->b_groups_per_set = gk; p->b_vcap = ne * nF;
     }
+    // a simulation keeps to its own cap (its table comes on top of buffers an earlier call may have sized for more sets)
+    const int64_t sets_per_chunk = job.sim ? std::min(p->b_cap, cap) : p->b_cap;
     CU(cudaStreamSynchronize(p->stream));
-    if (stage_root(p, rootFreqs)) return 1;
+    if (stage_root(p, rootFreqs, nullptr, 0, p->d_bpi)) return 1;
     if (mix) CU(cudaMemcpyAsync(p->d_brow, row_off.data(), (size_t)(B + 1) * sizeof(int), cudaMemcpyHostToDevice, p->stream));
+    // simulation: the chunk's table, the root's prefix sums, and one launch of columns (set-major, replicates consecutive)
+    hb2::SimArgs sa{};
+    int64_t chunk = 0;
+    size_t sim_smem = 0;
+    std::vector<int> ints;
+    if (job.sim) {
+        const int64_t nbm = std::min(sets_per_chunk, nSets);
+        chunk = job.nReps >= SIM_CHUNK ? SIM_CHUNK : std::min(SIM_CHUNK, nbm * job.nReps);
+        const bool smem_states = (size_t)I * SIM_THREADS <= SIM_SMEM_MAX;
+        hb2_partition::SimBuf &sb = p->sim;
+        if (sim_reserve(p, sb.cdf, sb.cap[0], (size_t)nbm * B * D * 64) || sim_reserve(p, sb.vec, sb.cap[1], (size_t)D) ||
+            sim_reserve(p, sb.ints, sb.cap[2], (size_t)nbm * B * D + nbm + 2) || sim_reserve(p, sb.leaf, sb.cap[3], (size_t)L * chunk) ||
+            (job.nodeStates && sim_reserve(p, sb.node, sb.cap[4], (size_t)I * chunk)) ||
+            (!smem_states && sim_reserve(p, sb.states, sb.cap[6], (size_t)I * chunk)))
+            return 1;
+        ints.assign(nbm + 2, 1);                // every set of a chunk is active | last root state | first bad row
+        ints[nbm] = root_last; ints[nbm + 1] = INT_MAX;
+        int *d_ints = sb.ints + nbm * B * D;
+        CU(cudaMemcpyAsync(sb.vec, root_cdf.data(), (size_t)D * sizeof(double), cudaMemcpyHostToDevice, p->stream));
+        CU(cudaMemcpyAsync(d_ints, ints.data(), ints.size() * sizeof(int), cudaMemcpyHostToDevice, p->stream));
+        sa.PT = p->d_bPT; sa.cdf = sb.cdf; sa.last = sb.ints; sa.active = d_ints; sa.root_last = d_ints + nbm; sa.bad = d_ints + nbm + 1;
+        sa.root_cdf = sb.vec;
+        sa.tree.child_start = p->d_child_start; sa.tree.child_ids = p->d_child_ids;
+        sa.leaf_out = sb.leaf; sa.node_out = job.nodeStates ? (long long *)sb.node : nullptr;
+        sa.states = smem_states ? nullptr : (unsigned char *)sb.states;
+        sa.L = (int)L; sa.I = (int)I; sa.B = (int)B; sa.D = (int)D; sa.Dp = 64; sa.chunk = (int)chunk;
+        sa.g0 = (unsigned long long)job.firstRep; sa.key = make_uint2((unsigned)job.seed, (unsigned)(job.seed >> 32));
+        sa.mix_w = p->d_bmixw; sa.row_off = p->d_brow; sa.R = (int)R; sa.reps = job.nReps;
+        sim_smem = smem_states ? (size_t)I * SIM_THREADS : 0;
+    }
     std::vector<int> grp;
-    for (int64_t s0 = 0; s0 < nSets; s0 += p->b_cap) {
-        const int64_t nb = std::min<int64_t>(p->b_cap, nSets - s0), ne = nb * R;
+    for (int64_t s0 = 0; s0 < nSets; s0 += sets_per_chunk) {
+        const int64_t nb = std::min<int64_t>(sets_per_chunk, nSets - s0), ne = nb * R;
         CU(cudaStreamSynchronize(p->stream));          // previous chunk done: buffers and pinned arrays are free again
         for (int64_t e = 0; e < ne; e++) p->h_bdst[e] = (int)e;                      // slot in the chunk's P area: [set][row]
-        for (int64_t s = 0; s < nb; s++) p->h_bdst[ne + s] = (int)patternOf[s0 + s];
         CU(cudaMemcpyAsync(p->d_bdst, p->h_bdst, (size_t)ne * sizeof(int), cudaMemcpyHostToDevice, p->stream));
-        CU(cudaMemcpyAsync(p->d_bpat, p->h_bdst + ne, (size_t)nb * sizeof(int), cudaMemcpyHostToDevice, p->stream));
+        if (!job.sim) {
+            // set s prunes pattern pat[s] of leaf[L][Sp]: the partition's patterns, or the chunk's columns as leaf[L][nb]
+            for (int64_t s = 0; s < nb; s++) p->h_bdst[ne + s] = job.columns ? (int)s : (int)job.patternOf[s0 + s];
+            CU(cudaMemcpyAsync(p->d_bpat, p->h_bdst + ne, (size_t)nb * sizeof(int), cudaMemcpyHostToDevice, p->stream));
+            if (job.columns) {
+                int *hc = p->h_bdst + ne + nb;
+                for (int64_t s = 0; s < nb; s++)
+                    for (int64_t l = 0; l < L; l++) hc[l * nb + s] = (int)job.columns[(s0 + s) * L + l];
+                CU(cudaMemcpyAsync(p->d_bcol, hc, (size_t)L * nb * sizeof(int), cudaMemcpyHostToDevice, p->stream));
+            }
+        }
         CU(cudaMemcpyAsync(p->d_bV, formulaValues + (size_t)s0 * R * nF, (size_t)ne * nF * sizeof(double), cudaMemcpyHostToDevice, p->stream));
         if (mix) CU(cudaMemcpyAsync(p->d_bmixw, weights + (size_t)s0 * R, (size_t)ne * sizeof(double), cudaMemcpyHostToDevice, p->stream));
         grp.resize(ne);
@@ -1685,16 +1753,48 @@ static int batch_sites(hb2_partition *p, int64_t templateId, int64_t nSets, cons
         if (plan_shared(p, p->h_bdst, ne, 1, grp.data(), sp, (int)templateId, &p->bex, 4) || staged_uploads(p)) return 1;
         // the chunk's P area is scratch: no resident copy is kept
         if (launch_expm(p, {Kind::Compiled, (int)templateId}, p->d_bV, p->d_bdst, (int)ne, false, sp, 0, p->d_bPT)) return 1;
+        if (job.sim) {
+            // the table of every (set, branch), and its check, before any column of the chunk is drawn
+            sa.t0 = (unsigned)(job.firstSet + s0);
+            if (mix) hb2::sim_cdf_kernel<true><<<(unsigned)(nb * B), 64, 0, p->stream>>>(sa);
+            else hb2::sim_cdf_kernel<false><<<(unsigned)(nb * B), 64, 0, p->stream>>>(sa);
+            p->launches++;
+            CU(cudaGetLastError());
+            int chk[2] = {INT_MAX, 0};          // first bad row | device-side wait error
+            CU(cudaMemcpyAsync(&chk[0], sa.bad, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
+            CU(cudaMemcpyAsync(&chk[1], p->d_err, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
+            CU(cudaStreamSynchronize(p->stream));
+            if (chk[1]) { cudaMemsetAsync(p->d_err, 0, sizeof(int), p->stream); return fail("a device-side wait timed out in the batched exponential (code %d)", chk[1]); }
+            if (chk[0] != INT_MAX) {
+                const long long row = chk[0] % D, cb = chk[0] / D;
+                return fail("hb2_batch_site_simulate: row %lld of the transition matrix of set %lld, branch %lld does not have a finite positive total",
+                            row, (long long)s0 + cb / B, cb % B);
+            }
+            const int64_t ncol = nb * job.nReps;
+            for (int64_t c0 = 0; c0 < ncol; c0 += chunk) {
+                const int64_t n = std::min(chunk, ncol - c0);
+                sa.n = (int)n; sa.col0 = c0;
+                hb2::batch_simulate_kernel<<<(unsigned)((n + SIM_THREADS - 1) / SIM_THREADS), SIM_THREADS, sim_smem, p->stream>>>(sa);
+                p->launches++;
+                CU(cudaGetLastError());
+                const size_t col = (size_t)s0 * job.nReps + c0;
+                CU(cudaMemcpyAsync(job.leafStates + col * L, sa.leaf_out, (size_t)n * L * sizeof(int64_t), cudaMemcpyDeviceToHost, p->stream));
+                if (job.nodeStates)
+                    CU(cudaMemcpyAsync(job.nodeStates + col * I, sa.node_out, (size_t)n * I * sizeof(int64_t), cudaMemcpyDeviceToHost, p->stream));
+            }
+            continue;
+        }
         hb2::BatchPruneArgs ba;
-        ba.PT = p->d_bPT; ba.cond = p->d_bcond; ba.node_ex = p->d_bnodeex; ba.pat = p->d_bpat; ba.leaf = p->d_leaf; ba.ambig = p->d_ambig; ba.pi = p->d_pi;
+        ba.PT = p->d_bPT; ba.cond = p->d_bcond; ba.node_ex = p->d_bnodeex; ba.pat = p->d_bpat; ba.ambig = p->d_ambig; ba.pi = p->d_bpi;
+        ba.leaf = job.columns ? (const int *)p->d_bcol : (const int *)p->d_leaf;
         ba.tree.child_start = p->d_child_start; ba.tree.child_ids = p->d_child_ids; ba.out = p->d_bout;
-        ba.L = (int)p->L; ba.I = (int)p->I; ba.B = (int)B; ba.D = (int)p->D; ba.Sp = (int)p->Sp;
+        ba.L = (int)p->L; ba.I = (int)p->I; ba.B = (int)B; ba.D = (int)p->D; ba.Sp = job.columns ? (int)nb : (int)p->Sp;
         ba.mix_w = p->d_bmixw; ba.row_off = p->d_brow; ba.R = (int)R;
         if (mix) hb2::prune_batch_kernel<true><<<(unsigned)nb, 64, 0, p->stream>>>(ba);
         else hb2::prune_batch_kernel<false><<<(unsigned)nb, 64, 0, p->stream>>>(ba);
         p->launches++;
         CU(cudaGetLastError());
-        CU(cudaMemcpyAsync(siteLnL + s0, p->d_bout, (size_t)nb * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
+        CU(cudaMemcpyAsync(job.siteLnL + s0, p->d_bout, (size_t)nb * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
     }
     int err = 0;
     CU(cudaMemcpyAsync(&err, p->d_err, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
@@ -1703,22 +1803,71 @@ static int batch_sites(hb2_partition *p, int64_t templateId, int64_t nSets, cons
     return 0;
 }
 
+// Component counts of a batch call: with weights, K in 1..4 and branchK (nullable) in 1..K; without, one row per branch.
+static int check_rows(const hb2_partition *p, int64_t K, const int64_t *branchK, const double *weights) {
+    if (!weights) {
+        if (K != 1 || branchK) return fail("K=%lld and branchK need weights: without them every branch has one row (K=1, branchK NULL)", (long long)K);
+        return 0;
+    }
+    if (K < 1 || K > 4) return fail("K=%lld outside 1..4", (long long)K);
+    if (branchK)
+        for (int64_t b = 0; b < p->B; b++)
+            if (branchK[b] < 1 || branchK[b] > K) return fail("branchK[%lld]=%lld outside 1..%lld", (long long)b, (long long)branchK[b], (long long)K);
+    return 0;
+}
+
 int hb2_batch_site_likelihoods(hb2_partition *p, int64_t templateId, int64_t nSets, const int64_t *patternOf,
                                const double *formulaValues, const int64_t *branchGroup, const double *rootFreqs, double *siteLnL) {
-    return batch_sites(p, templateId, nSets, patternOf, 1, nullptr, formulaValues, nullptr, branchGroup, rootFreqs, siteLnL);
+    BatchJob job;
+    job.patternOf = patternOf; job.siteLnL = siteLnL;
+    return batch_sites(p, templateId, nSets, 1, nullptr, formulaValues, nullptr, branchGroup, rootFreqs, job);
 }
 
 int hb2_batch_site_mixture_likelihoods(hb2_partition *p, int64_t templateId, int64_t nSets, const int64_t *patternOf, int64_t K,
                                        const int64_t *branchK, const double *formulaValues, const double *weights,
                                        const int64_t *branchGroup, const double *rootFreqs, double *siteLnL) {
     if (!p) return fail("null partition");
-    if (K < 1 || K > 4) return fail("K=%lld outside 1..4", (long long)K);
     if (!weights) return fail("weights must not be null");
     if (!formulaValues) return fail("formulaValues must not be null");
-    if (branchK)
-        for (int64_t b = 0; b < p->B; b++)
-            if (branchK[b] < 1 || branchK[b] > K) return fail("branchK[%lld]=%lld outside 1..%lld", (long long)b, (long long)branchK[b], (long long)K);
-    return batch_sites(p, templateId, nSets, patternOf, K, branchK, formulaValues, weights, branchGroup, rootFreqs, siteLnL);
+    if (check_rows(p, K, branchK, weights)) return 1;
+    BatchJob job;
+    job.patternOf = patternOf; job.siteLnL = siteLnL;
+    return batch_sites(p, templateId, nSets, K, branchK, formulaValues, weights, branchGroup, rootFreqs, job);
+}
+
+int hb2_batch_column_likelihoods(hb2_partition *p, int64_t templateId, int64_t nSets, const int64_t *columns, int64_t K,
+                                 const int64_t *branchK, const double *formulaValues, const double *weights,
+                                 const int64_t *branchGroup, const double *rootFreqs, double *siteLnL) {
+    if (!p) return fail("null partition");
+    if (nSets < 0) return fail("hb2_batch_column_likelihoods: nSets=%lld is negative", (long long)nSets);
+    if (!columns) return fail("hb2_batch_column_likelihoods: columns must not be null");
+    if (!formulaValues) return fail("hb2_batch_column_likelihoods: formulaValues must not be null");
+    if (!rootFreqs) return fail("hb2_batch_column_likelihoods: rootFreqs must not be null");
+    if (!siteLnL) return fail("hb2_batch_column_likelihoods: siteLnL must not be null");
+    if (check_rows(p, K, branchK, weights)) return 1;
+    BatchJob job;
+    job.columns = columns; job.siteLnL = siteLnL;
+    return batch_sites(p, templateId, nSets, K, branchK, formulaValues, weights, branchGroup, rootFreqs, job);
+}
+
+int hb2_batch_site_simulate(hb2_partition *p, int64_t templateId, int64_t nSets, int64_t K, const int64_t *branchK,
+                            const double *formulaValues, const double *weights, const int64_t *branchGroup,
+                            const double *rootFreqs, int64_t nReps, uint64_t seed, int64_t firstSet, int64_t firstRep,
+                            int64_t *leafStates, int64_t *nodeStates) {
+    if (!p) return fail("null partition");
+    if (nSets < 0) return fail("hb2_batch_site_simulate: nSets=%lld is negative", (long long)nSets);
+    if (nReps < 0) return fail("hb2_batch_site_simulate: nReps=%lld is negative", (long long)nReps);
+    if (firstRep < 0 || firstRep > INT64_MAX - nReps) return fail("hb2_batch_site_simulate: firstRep=%lld out of range", (long long)firstRep);
+    if (firstSet < 0 || firstSet > ((int64_t)1 << 32) - nSets)
+        return fail("hb2_batch_site_simulate: firstSet=%lld out of range (firstSet + nSets must not exceed 2^32)", (long long)firstSet);
+    if (!formulaValues) return fail("hb2_batch_site_simulate: formulaValues must not be null");
+    if (!rootFreqs) return fail("hb2_batch_site_simulate: rootFreqs must not be null");
+    if (!leafStates) return fail("hb2_batch_site_simulate: leafStates must not be null");
+    if (check_rows(p, K, branchK, weights)) return 1;
+    BatchJob job;
+    job.sim = true; job.nReps = nReps; job.seed = seed; job.firstSet = firstSet; job.firstRep = firstRep;
+    job.leafStates = leafStates; job.nodeStates = nodeStates;
+    return batch_sites(p, templateId, nSets, K, branchK, formulaValues, weights, branchGroup, rootFreqs, job);
 }
 
 int hb2_read_conditionals(hb2_partition *p, int64_t cat, int64_t inode, double *cond, int32_t *exp2) {
@@ -1812,7 +1961,7 @@ int hb2_simulate(hb2_partition *p, const double *weights, const double *rootFreq
     a.L = (int)L; a.I = (int)I; a.B = (int)B; a.C = (int)C; a.D = (int)D; a.Dp = p->Dp; a.chunk = (int)chunk;
     a.key = make_uint2((unsigned)seed, (unsigned)(seed >> 32));
     // the table of every drawn class, and its check: a refused call writes nothing
-    hb2::sim_cdf_kernel<<<(unsigned)(C * B), 64, 0, p->stream>>>(a);
+    hb2::sim_cdf_kernel<false><<<(unsigned)(C * B), 64, 0, p->stream>>>(a);
     p->launches++;
     CU(cudaGetLastError());
     int bad = INT_MAX;

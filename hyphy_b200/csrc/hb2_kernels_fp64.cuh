@@ -1585,9 +1585,10 @@ __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
     return c;
 }
 
-// Uniform in [0, 1) of draw `slot` of global site g.
-__device__ __forceinline__ double sim_uniform(unsigned long long g, unsigned slot, uint2 key) {
-    const uint4 x = philox4x32_10(make_uint4((unsigned)g, (unsigned)(g >> 32), slot, 0u), key);
+// Uniform in [0, 1) of draw `slot` of global site g; t is the fourth counter word (0 for hb2_simulate, the global set of
+// hb2_batch_site_simulate).
+__device__ __forceinline__ double sim_uniform(unsigned long long g, unsigned slot, uint2 key, unsigned t = 0u) {
+    const uint4 x = philox4x32_10(make_uint4((unsigned)g, (unsigned)(g >> 32), slot, t), key);
     return (double)(((unsigned long long)x.x << 21) + (x.y >> 11)) * 0x1p-53;
 }
 
@@ -1636,15 +1637,25 @@ struct SimArgs {
     int *class_out;            // [chunk] or null
     unsigned char *states;     // [I][chunk] internal states, used when they do not fit in shared memory (else null)
     int L, I, B, C, D, Dp, chunk, n;
-    unsigned long long g0;     // global site of the chunk's first site
+    unsigned long long g0;     // global site of the chunk's first site (per-set: global replicate of the set's first column)
     uint2 key;
+    // per-set mode (hb2_batch_site_simulate): "class" = set of the chunk
+    const double *mix_w;       // MIX: [sets][R] component weights
+    const int *row_off;        // MIX: [B+1] first component row of each branch (PT is [sets][R][Dp*Dp])
+    int R;                     // MIX: component rows per set
+    long long reps;            // replicates per set
+    long long col0;            // chunk column of the launch's first thread (column = set * reps + replicate)
+    unsigned t0;               // global set of the chunk's first set
 };
 
 // One CTA of 64 threads per (class, branch) of a drawn class; thread `row` forms the sequential prefix sums of its row
 // (PT column `row`: adjacent threads read adjacent doubles) in shared memory, padded to 65 doubles per row against bank
 // conflicts, and the CTA then stores the matrix's D x Dp block of the table with consecutive threads on consecutive
 // doubles.  A row whose total is not finite and > 0 is reported through atomicMin.
+// MIX (per-set mode, explicit-form mixtures): branch b of set c mixes its component rows row_off[b] .. row_off[b+1]-1 entry
+// by entry, w_0 P_0 then fma(w_k, P_k, .) in component order, exactly as prune_batch_kernel<true> forms them.
 constexpr int SIM_CDF_LD = 65;
+template <bool MIX>
 __global__ void __launch_bounds__(64) sim_cdf_kernel(SimArgs a) {
     __shared__ double rows[64 * SIM_CDF_LD];
     const long long cb = blockIdx.x;                       // class * B + branch
@@ -1652,12 +1663,28 @@ __global__ void __launch_bounds__(64) sim_cdf_kernel(SimArgs a) {
     const int row = threadIdx.x;
     if (row < a.D) {
         const double *P = a.PT + (size_t)cb * a.Dp * a.Dp + row;
+        double wc[4];
+        int nc = 1;
+        if constexpr (MIX) {
+            const long long set = cb / a.B;
+            const int b = (int)(cb - set * a.B), r0 = a.row_off[b];
+            nc = a.row_off[b + 1] - r0;
+            P = a.PT + ((size_t)set * a.R + r0) * a.Dp * a.Dp + row;
+#pragma unroll
+            for (int k = 0; k < 4; k++) wc[k] = k < nc ? a.mix_w[(size_t)set * a.R + r0 + k] : 0.0;
+        }
         double *c = rows + row * SIM_CDF_LD;
         double s = 0.0;
         int last = -1;
 #pragma unroll 4
         for (int j = 0; j < a.D; j++) {
-            const double v = P[(size_t)j * a.Dp];
+            double v = P[(size_t)j * a.Dp];
+            if constexpr (MIX) {
+                v = wc[0] * v;
+#pragma unroll
+                for (int k = 1; k < 4; k++)
+                    if (k < nc) v = fma(wc[k], P[(size_t)k * a.Dp * a.Dp + (size_t)j * a.Dp], v);
+            }
             if (v > 0.0) { s = __dadd_rn(s, v); last = j; }
             c[j] = s;
         }
@@ -1701,6 +1728,39 @@ __global__ void __launch_bounds__(128) simulate_kernel(SimArgs a) {
             } else {
                 st[(size_t)(ch - L) * stride] = (unsigned char)x;
                 if (a.node_out) a.node_out[(size_t)(ch - L) * a.chunk + i] = x;
+            }
+        }
+    }
+}
+
+// Per-set mode (hb2_batch_site_simulate): one thread per column (set, replicate) of the chunk, column = set * reps +
+// replicate, consecutive threads on consecutive replicates of one set.  The set is the "class" of the table and t0 + set
+// the fourth counter word; there is no class draw.  Outputs are column-major: leaf_out [n][L], node_out [n][I].
+__global__ void __launch_bounds__(128) batch_simulate_kernel(SimArgs a) {
+    extern __shared__ unsigned char sim_smem[];
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= a.n) return;
+    const long long col = a.col0 + i, set = col / a.reps;
+    const unsigned long long g = a.g0 + (unsigned long long)(col - set * a.reps);
+    const unsigned t = a.t0 + (unsigned)set;
+    const int L = a.L, I = a.I;
+    unsigned char *st = a.states ? a.states + i : sim_smem + threadIdx.x;
+    const size_t stride = a.states ? (size_t)a.chunk : (size_t)blockDim.x;
+    int s = sim_draw(a.root_cdf, a.D, a.root_last, sim_uniform(g, (unsigned)(L + I - 1), a.key, t));
+    if (a.node_out) a.node_out[(size_t)i * I + I - 1] = s;
+    const size_t set_rows = (size_t)set * a.B;
+    for (int n = I - 1; n >= 0; n--) {
+        if (n < I - 1) s = st[(size_t)n * stride];
+        const int c_end = a.tree.child_start[n + 1];
+        for (int ci = a.tree.child_start[n]; ci < c_end; ci++) {
+            const int ch = a.tree.child_ids[ci];
+            const size_t r = (set_rows + ch) * a.D + s;
+            const int x = sim_draw(a.cdf + r * a.Dp, a.D, a.last + r, sim_uniform(g, (unsigned)ch, a.key, t));
+            if (ch < L) {
+                a.leaf_out[(size_t)i * L + ch] = x;
+            } else {
+                st[(size_t)(ch - L) * stride] = (unsigned char)x;
+                if (a.node_out) a.node_out[(size_t)i * I + ch - L] = x;
             }
         }
     }

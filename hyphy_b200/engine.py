@@ -44,9 +44,12 @@ ABI = [
     ("hb2_evaluate_classes", C.c_int, [C.c_void_p, _dp, C.c_int64, _ip, _dp, _dp, _dp, _ip]),
     ("hb2_batch_site_likelihoods", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, _dp, _ip, _dp, _dp]),
     ("hb2_batch_site_mixture_likelihoods", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, C.c_int64, _ip, _dp, _dp, _ip, _dp, _dp]),
+    ("hb2_batch_column_likelihoods", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, C.c_int64, _ip, _dp, _dp, _ip, _dp, _dp]),
     ("hb2_read_conditionals", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _dp, _i32p]),
     ("hb2_read_transition", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _dp]),
     ("hb2_simulate", C.c_int, [C.c_void_p, _dp, _dp, C.c_int64, C.c_uint64, C.c_int64, _ip, _ip, _i32p]),
+    ("hb2_batch_site_simulate", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, _ip, _dp, _dp, _ip, _dp, C.c_int64,
+                                          C.c_uint64, C.c_int64, C.c_int64, _ip, _ip]),
     ("hb2_comm_unique_id", C.c_int, [C.c_void_p]),
     ("hb2_branch_cache_build", C.c_int, [C.c_void_p, C.c_int64, _dp]),
     ("hb2_branch_cache_evaluate", C.c_int, [C.c_void_p, C.c_int64, _dp, C.POINTER(C.c_double), _dp, _ip]),
@@ -277,26 +280,70 @@ class Partition:
         """MEME's site model: branch b mixes branch_k[b] components (None: weights.shape[1] / B on every branch).
         formula_values: [nSets, R, nF], weights: [nSets, R], R = sum of branch_k; returns the nSets log-likelihoods."""
         po, ppo = _i(pattern_of)
-        v, pv = _d(formula_values)
-        w, pw = _d(weights)
-        assert v.ndim == 3 and v.shape[0] == len(po) and w.shape == v.shape[:2]
-        pbk = None
-        if branch_k is None:
-            assert w.shape[1] % self.B == 0
-            K = w.shape[1] // self.B
-        else:
-            bk, pbk = _i(branch_k)
-            assert bk.shape == (self.B,) and bk.sum() == w.shape[1]
-            K = int(bk.max())
+        assert weights is not None
+        K, pbk, pv, pw, pbg, keep = self._batch_rows(len(po), formula_values, weights, branch_k, branch_group)
         pi, ppi = _d(root_freqs)
-        pbg = None
-        if branch_group is not None:
-            bg, pbg = _i(branch_group)
-            assert bg.shape == (self.B,)
         out = np.empty(len(po))
         _check(self._lib.hb2_batch_site_mixture_likelihoods(self._h, int(template), len(po), ppo, K, pbk, pv, pw, pbg, ppi,
                                                             out.ctypes.data_as(_dp)))
         return out
+
+    def _batch_rows(self, n_sets, formula_values, weights, branch_k, branch_group):
+        """Checked arguments of the batch entry points that take both set layouts: weights None means one row per branch
+        (formula_values [nSets, B, nF]); otherwise as batch_site_mixture_likelihoods."""
+        v, pv = _d(formula_values)
+        assert v.ndim == 3 and v.shape[0] == n_sets
+        K, pw, pbk, pbg, keep = 1, None, None, None, [v]
+        if weights is None:
+            assert branch_k is None and v.shape[1] == self.B
+        else:
+            w, pw = _d(weights)
+            assert w.shape == v.shape[:2]
+            keep.append(w)
+            if branch_k is None:
+                assert w.shape[1] % self.B == 0
+                K = w.shape[1] // self.B
+            else:
+                bk, pbk = _i(branch_k)
+                assert bk.shape == (self.B,) and bk.sum() == w.shape[1]
+                K = int(bk.max())
+                keep.append(bk)
+        if branch_group is not None:
+            bg, pbg = _i(branch_group)
+            assert bg.shape == (self.B,)
+            keep.append(bg)
+        return K, pbk, pv, pw, pbg, keep
+
+    def batch_column_likelihoods(self, columns, formula_values, root_freqs, weights=None, branch_k=None, branch_group=None,
+                                 template=0):
+        """Batch likelihoods of caller-given columns [nSets, L] (hb2_create's leaf codes) instead of partition patterns;
+        sets as batch_site_likelihoods (weights None) or batch_site_mixture_likelihoods.  Returns the nSets log-likelihoods."""
+        col, pcol = _i(columns)
+        assert col.ndim == 2 and col.shape[1] == self.L
+        K, pbk, pv, pw, pbg, keep = self._batch_rows(len(col), formula_values, weights, branch_k, branch_group)
+        pi, ppi = _d(root_freqs)
+        out = np.empty(len(col))
+        _check(self._lib.hb2_batch_column_likelihoods(self._h, int(template), len(col), pcol, K, pbk, pv, pw, pbg, ppi,
+                                                      out.ctypes.data_as(_dp)))
+        return out
+
+    def batch_site_simulate(self, formula_values, root_freqs, n_reps, weights=None, branch_k=None, branch_group=None, seed=0,
+                            first_set=0, first_rep=0, want_nodes=False, template=0):
+        """Replicates first_rep .. first_rep + n_reps - 1 of sets first_set .. of the stream `seed`, each simulated from its
+        own set's model (hb2_batch_site_simulate); sets as batch_column_likelihoods.  Returns (leaf states
+        [nSets, n_reps, L] int64, internal-node states [nSets, n_reps, I] int64 or None)."""
+        v = np.asarray(formula_values)
+        n = len(v)
+        K, pbk, pv, pw, pbg, keep = self._batch_rows(n, v, weights, branch_k, branch_group)
+        pi, ppi = _d(root_freqs)
+        assert pi.shape == (self.D,)
+        r = max(int(n_reps), 0)
+        leaf = np.empty((n, r, self.L), dtype=np.int64)
+        nodes = np.empty((n, r, self.I), dtype=np.int64) if want_nodes else None
+        _check(self._lib.hb2_batch_site_simulate(self._h, int(template), n, K, pbk, pv, pw, pbg, ppi, int(n_reps),
+                                                 int(seed) & 0xFFFFFFFFFFFFFFFF, int(first_set), int(first_rep),
+                                                 leaf.ctypes.data_as(_ip), nodes.ctypes.data_as(_ip) if want_nodes else None))
+        return leaf, nodes
 
     # -- read-backs --------------------------------------------------------------------------------
     def read_conditionals(self, cat, inode):

@@ -172,6 +172,17 @@ int hb2_batch_site_mixture_likelihoods(hb2_partition *p, int64_t templateId, int
                                        const double *weights, const int64_t *branchGroup, const double *rootFreqs,
                                        double *siteLnL);
 
+/* The batch likelihoods of caller-given columns instead of partition patterns (the refits of a parametric bootstrap score
+ * columns simulated by hb2_batch_site_simulate, which are not patterns of the partition): set s scores
+ * columns[s][0..L-1], in hb2_create's leafState codes (>= 0: a state < D; < 0: ambiguity row -(code+1) < nAmb).
+ * weights == NULL: one row per branch, formulaValues [nSets][B][nFormulas] as hb2_batch_site_likelihoods (K must be 1 and
+ * branchK NULL); otherwise rows, weights, K and branchK as hb2_batch_site_mixture_likelihoods.  A code out of range is
+ * refused on the host with its set and leaf, and nothing is written.  Everything else, outputs included, as
+ * hb2_batch_site_mixture_likelihoods: a column that equals pattern q gives exactly what patternOf = q gives. */
+int hb2_batch_column_likelihoods(hb2_partition *p, int64_t templateId, int64_t nSets, const int64_t *columns,
+                                 int64_t K, const int64_t *branchK, const double *formulaValues, const double *weights,
+                                 const int64_t *branchGroup, const double *rootFreqs, double *siteLnL);
+
 /* FillInConditionals-style read-back (tree.cpp:3335): conditionals of internal node `inode` (0..I-1), class cat,
  * as S*D doubles (original pattern order) and S binary exponents: true value = cond * 2^exp2. */
 int hb2_read_conditionals(hb2_partition *p, int64_t cat, int64_t inode, double *cond, int32_t *exp2);
@@ -207,6 +218,34 @@ int hb2_read_transition(hb2_partition *p, int64_t cat, int64_t node, double *P);
  * Nothing an evaluation reads is touched: conditionals, scalers, walk plans and tags, the branch cache, the root vector. */
 int hb2_simulate(hb2_partition *p, const double *weights, const double *rootFreqs, int64_t nSites, uint64_t seed,
                  int64_t firstSite, int64_t *leafStates, int64_t *nodeStates, int32_t *siteClass);
+
+/* Site-level parametric bootstrap (FEL.bf:803-818, MEME.bf:1445-1458, --resample N): nReps replicate columns simulated
+ * from EACH set's own model (SimulateDataSet on the one-site likelihood function).  Sets have the layout of the batch
+ * entry points: weights == NULL: one row per branch, formulaValues [nSets][B][nFormulas], K must be 1 and branchK NULL;
+ * otherwise rows, weights, K, branchK as hb2_batch_site_mixture_likelihoods.  branchGroup is the same shared-powers hint.
+ * The matrix simulated from is the one the likelihood entry points use for the set: entry (k, j) of a mixture branch is
+ * e = w_0 P_0[k][j], then e = fma(w_c, P_c[k][j], e) for c = 1..n-1 (the order of the batch pruning and of
+ * hb2_set_mixture_matrices), exponentials from the same batched pipeline.
+ *   rootFreqs  D root-state weights, one vector for every set.
+ *   leafStates [nSets][nReps][L]: leaf states 0..D-1, column by column -- directly the `columns` of
+ *              hb2_batch_column_likelihoods for nSets*nReps sets.
+ *   nodeStates nullable [nSets][nReps][I]: internal-node states, root at I-1.
+ * The stream is hb2_simulate's with the set in the fourth counter word: one Philox4x32-10 call per draw on counter
+ * (lo32(g), hi32(g), slot, t), key (lo32(seed), hi32(seed)), g = firstRep + r for replicate r, t = firstSet + s for set s
+ * of the call; slot n < L+I-1 is flat node n's state, slot L+I-1 the root (no class slot: a set has one model); uniform and
+ * draw rule as hb2_simulate.  Results depend only on the set's matrices, rootFreqs, seed, t and g: splitting sets or
+ * replicates across calls or chunks changes nothing, and set t = 0 draws exactly hb2_simulate's stream.
+ * Refusals before anything runs (nothing is written): everything hb2_batch_site_mixture_likelihoods refuses; nSets < 0 or
+ * nReps < 0; firstRep < 0 or firstRep > INT64_MAX - nReps; firstSet < 0 or firstSet + nSets > 2^32; root frequencies
+ * refused by hb2_simulate's rule.  A set whose matrix has a row whose total is not finite and > 0 (NaN formula values,
+ * for example) is found on the device: the call fails naming the first such (set of the call, branch, row) in call
+ * order, and the output of the set chunks finished before it is unspecified.  nSets == 0 or nReps == 0 after the checks
+ * does nothing.  As with the other batch entry points, nothing an evaluation reads is touched: conditionals, scalers,
+ * walk plans, the branch cache, the staged root vector.  33..64 states only. */
+int hb2_batch_site_simulate(hb2_partition *p, int64_t templateId, int64_t nSets, int64_t K, const int64_t *branchK,
+                            const double *formulaValues, const double *weights, const int64_t *branchGroup,
+                            const double *rootFreqs, int64_t nReps, uint64_t seed, int64_t firstSet, int64_t firstRep,
+                            int64_t *leafStates, int64_t *nodeStates);
 
 /* Multi-GPU (one process per GPU, patterns sharded by the caller: each rank creates its partition with its own
  * pattern shard).  After hb2_comm_init every hb2_evaluate* returns the SUM over ranks of the partial lnL
