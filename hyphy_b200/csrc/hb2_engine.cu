@@ -130,6 +130,14 @@ public:
         ptr_ = static_cast<T *>(q); n_ = n;
         return 0;
     }
+    // Grows the block to at least n elements; its contents are not kept.  Work queued on `stream` may still use the old
+    // block, so the stream is synchronised before it goes back to the pool.
+    int reserve(size_t n, cudaStream_t stream) {
+        if (n <= n_) return 0;
+        CU(cudaStreamSynchronize(stream));
+        return alloc(n);
+    }
+    size_t size() const { return n_; }
     // Clears all n elements on `stream` (device buffers).
     int zero(cudaStream_t stream) {
         CU(cudaMemsetAsync(ptr_, 0, n_ * sizeof(T), stream));
@@ -222,6 +230,12 @@ struct Slot {
     int entry = -1;                           // index of the pending entry in that queue, -1 none
 };
 
+// Shape of a batch call (batch_shape).
+struct BatchShape {
+    std::vector<int> row_off;                 // branch b of a set owns component rows row_off[b] .. row_off[b+1]-1
+    int64_t R = 0, nF = 0, gk = 0, sets = 0;  // rows per set, formula values per row, groups per set; sets per chunk
+};
+
 }  // namespace
 
 struct hb2_partition {
@@ -247,7 +261,6 @@ struct hb2_partition {
     DeviceBuffer<double> d_mix_scratch, d_mix_Q;   // [cap][Dp*Dp], [cap][D*D] | [cap] weights
     PinnedBuffer<double> h_mix;                    // as d_mix_Q, then 2 cap ints
     DeviceBuffer<int> d_mix_dst;
-    int64_t mix_capacity = 0;
     // shared-powers expm (64 padded states, hb2_kernels_fp64.cuh "Shared powers"): group = rate class (plain batches) or
     // C + mixture component; per-entry arrays are indexed like the batch
     struct ExBuf {
@@ -271,17 +284,37 @@ struct hb2_partition {
         }
     };
     ExBuf ex;                                 // the partition's own hand-overs
-    ExBuf bex;                                // batched one-pattern likelihoods (hb2_batch_site_likelihoods): one group per set
-    int64_t b_cap = 0;                        // sets per chunk of the batch buffers below
-    int64_t b_vcap = 0;                       // formula values d_bV holds
-    DeviceBuffer<double> d_bPT, d_bV, d_bcond, d_bout;
-    DeviceBuffer<double> d_bmixw;             // mixture weights of a chunk [sets][rows]
-    DeviceBuffer<int> d_bdst, d_bpat, d_bnodeex;
-    PinnedBuffer<int> h_bdst;
-    DeviceBuffer<int> d_brow;                 // first component row of each branch [B+1]
-    DeviceBuffer<int> d_bcol;                 // caller columns of a chunk (hb2_batch_column_likelihoods) [L][sets]
-    DeviceBuffer<double> d_bpi;               // root vector of the batch calls (the staged d_pi stays the evaluations')
-    int b_groups_per_set = 1;
+    // Workspace of the batch entry points (hb2_batch_*) for one chunk of `sets` sets: the chunk's expm entries are its
+    // sets' component rows in [set][row] order, and entry e goes to slot e of the chunk's P area.  The batch calls stage
+    // their own root vector, so the staged d_pi stays the evaluations'.
+    struct BatchWorkspace {
+        ExBuf ex;                             // shared-powers groups of the chunk: [set][groups per set]
+        DeviceBuffer<double> PT, V, mixw;     // P area [entries][4096], formula values [entries][nF], weights [sets][rows]
+        DeviceBuffer<double> cond, out, pi;   // node vectors [sets][I][64], log-likelihoods [sets], root vector [64]
+        DeviceBuffer<int> slot, pat, node_ex; // identity slots [entries], patterns [sets], node exponents [sets][I]
+        DeviceBuffer<int> row, col;           // first component row of each branch [B+1], caller columns [L][sets]
+        PinnedBuffer<int> h_slot, h_pat, h_col;   // staging of slot, pat and col
+        // Sizes the workspace for chunks of `sh`.  A chunk that does not fit re-sizes the whole workspace for this call,
+        // after releasing it, so that memory stays at one call's chunk footprint (~8 GB) instead of adding up the largest
+        // buffers of different calls' shapes.
+        int fit(const BatchShape &sh, int64_t L, int64_t I, cudaStream_t stream) {
+            const int64_t sets = sh.sets, ne = sets * sh.R;
+            if (sets <= (int64_t)out.size() && ne <= (int64_t)slot.size() && sets * sh.gk <= ex.G && ne * sh.nF <= (int64_t)V.size())
+                return 0;
+            CU(cudaStreamSynchronize(stream));
+            *this = BatchWorkspace();
+            if (ex.alloc((int)(sets * sh.gk), ne, stream) || PT.alloc((size_t)ne * 4096) || V.alloc((size_t)ne * sh.nF) ||
+                mixw.alloc(ne) || cond.alloc((size_t)sets * I * 64) || out.alloc(sets) || slot.alloc(ne) || pat.alloc(sets) ||
+                node_ex.alloc((size_t)sets * I) || row.alloc(sh.row_off.size()) || col.alloc((size_t)sets * L) || pi.alloc(64) ||
+                h_slot.alloc(ne) || h_pat.alloc(sets) || h_col.alloc((size_t)sets * L)) {
+                *this = BatchWorkspace();     // fits nothing: the next call sizes it again
+                return 1;
+            }
+            for (int64_t e = 0; e < ne; e++) h_slot[e] = (int)e;
+            CU(cudaMemcpyAsync(slot, h_slot, (size_t)ne * sizeof(int), cudaMemcpyHostToDevice, stream));
+            return 0;
+        }
+    } batch;
     bool ex_enabled = true;                   // HB2_EXPM_SHARED=0 switches the path off (A/B testing)
     int64_t stage_launches[3] = {0, 0, 0};    // launches per evaluation of the last hb2_time_resident {expm, pruning, root}
     // compiled rate-matrix templates (hb2_set_rate_template*): static scatter map + own queue of per-evaluation formula
@@ -348,7 +381,6 @@ struct hb2_partition {
         DeviceBuffer<int> ints, cls;
         DeviceBuffer<long long> leaf, node;
         DeviceBuffer<unsigned char> states;
-        size_t cap[7] = {0, 0, 0, 0, 0, 0, 0};
     } sim;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
     // side stream of the expm stage: the power tables are built on it while the classification runs on `stream`
@@ -1289,14 +1321,45 @@ bool sim_prefix(const double *v, int64_t m, double *c, int *last) {
     return s > 0.0 && std::isfinite(s);
 }
 
-// Grows a simulation buffer to n elements (its contents are not kept).
-template <typename T>
-int sim_reserve(hb2_partition *p, DeviceBuffer<T> &b, size_t &cap, size_t n) {
-    if (n <= cap) return 0;
+// Set-up of hb2_simulate and of each chunk of hb2_batch_site_simulate, whose table holds `nblk` blocks (rate classes, or
+// sets) of B matrices of a.PT: reserves the scratch for `chunk` columns per launch, uploads the prefix sums `cdf` (class
+// weights, if any | root frequencies) and `ints` (active blocks [nblk] | last class | last root state | first bad row),
+// fills the fields of `a` both calls share, and builds and checks the table.  A bad row refuses the call before any column
+// is drawn, as "<fn>: row r of the transition matrix of <block>", `block` formatting (blk0 + block, branch).
+int sim_tables(hb2_partition *p, hb2::SimArgs &a, int64_t nblk, int64_t chunk, uint64_t seed, const std::vector<double> &cdf,
+               const std::vector<int> &ints, bool nodes, bool classes, bool mix, const char *fn, const char *block, int64_t blk0) {
+    const int64_t B = p->B, D = p->D, L = p->L, I = p->I;
+    const bool smem_states = (size_t)I * SIM_THREADS <= SIM_SMEM_MAX;
+    hb2_partition::SimBuf &sb = p->sim;
+    if (sb.cdf.reserve((size_t)nblk * B * D * p->Dp, p->stream) || sb.vec.reserve(cdf.size(), p->stream) ||
+        sb.ints.reserve((size_t)nblk * B * D + ints.size(), p->stream) || sb.leaf.reserve((size_t)L * chunk, p->stream) ||
+        (nodes && sb.node.reserve((size_t)I * chunk, p->stream)) || (classes && sb.cls.reserve((size_t)chunk, p->stream)) ||
+        (!smem_states && sb.states.reserve((size_t)I * chunk, p->stream)))
+        return 1;
+    int *d_ints = sb.ints + nblk * B * D;
+    CU(cudaMemcpyAsync(sb.vec, cdf.data(), cdf.size() * sizeof(double), cudaMemcpyHostToDevice, p->stream));
+    CU(cudaMemcpyAsync(d_ints, ints.data(), ints.size() * sizeof(int), cudaMemcpyHostToDevice, p->stream));
+    a.cdf = sb.cdf; a.last = sb.ints; a.class_cdf = sb.vec; a.root_cdf = sb.vec + (cdf.size() - D);
+    a.active = d_ints; a.class_last = d_ints + nblk; a.root_last = d_ints + nblk + 1; a.bad = d_ints + nblk + 2;
+    a.tree.child_start = p->d_child_start; a.tree.child_ids = p->d_child_ids;
+    a.leaf_out = sb.leaf; a.node_out = nodes ? (long long *)sb.node : nullptr; a.class_out = classes ? (int *)sb.cls : nullptr;
+    a.states = smem_states ? nullptr : (unsigned char *)sb.states;
+    a.L = (int)L; a.I = (int)I; a.B = (int)B; a.D = (int)D; a.Dp = p->Dp; a.chunk = (int)chunk;
+    a.key = make_uint2((unsigned)seed, (unsigned)(seed >> 32));
+    if (mix) hb2::sim_cdf_kernel<true><<<(unsigned)(nblk * B), 64, 0, p->stream>>>(a);
+    else hb2::sim_cdf_kernel<false><<<(unsigned)(nblk * B), 64, 0, p->stream>>>(a);
+    p->launches++;
+    CU(cudaGetLastError());
+    int *chk = reinterpret_cast<int *>(p->h_small + p->Dp + p->C + 1);   // first bad row | device-side wait error
+    CU(cudaMemcpyAsync(&chk[0], a.bad, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
+    CU(cudaMemcpyAsync(&chk[1], p->d_err, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
     CU(cudaStreamSynchronize(p->stream));
-    cap = 0;
-    if (b.alloc(std::max<size_t>(n, 1))) return 1;
-    cap = n;
+    if (chk[1]) { cudaMemsetAsync(p->d_err, 0, sizeof(int), p->stream); return fail("a device-side wait timed out in the batched exponential (code %d)", chk[1]); }
+    if (chk[0] != INT_MAX) {
+        const long long row = chk[0] % D, cb = chk[0] / D;
+        const std::string msg = std::string(fn) + ": row %lld of the transition matrix of " + block + " does not have a finite positive total";
+        return fail(msg.c_str(), row, (long long)blk0 + cb / B, cb % B);
+    }
     return 0;
 }
 
@@ -1486,14 +1549,10 @@ int hb2_set_mixture_matrices(hb2_partition *p, int64_t cat, int64_t n, const int
     const size_t dd = (size_t)p->D * p->D, dpdp = (size_t)p->Dp * p->Dp;
     const int64_t nk = n * K;
     if (wait_staging(p)) return 1;
-    if (nk > p->mix_capacity) {
-        CU(cudaStreamSynchronize(p->stream));
-        p->mix_capacity = 0;
-        if (p->d_mix_scratch.alloc((size_t)nk * dpdp) || p->d_mix_Q.alloc((size_t)nk * (dd + 1)) || p->d_mix_dst.alloc((size_t)2 * nk) ||
-            p->h_mix.alloc((size_t)nk * (dd + 2)))      // 2 nk ints take nk doubles
-            return 1;
-        p->mix_capacity = nk;
-    }
+    if (p->d_mix_scratch.reserve((size_t)nk * dpdp, p->stream) || p->d_mix_Q.reserve((size_t)nk * (dd + 1), p->stream) ||
+        p->d_mix_dst.reserve((size_t)2 * nk, p->stream) ||
+        p->h_mix.reserve((size_t)nk * (dd + 2), p->stream))      // 2 nk ints take nk doubles
+        return 1;
     memcpy(p->h_mix, M, (size_t)nk * dd * sizeof(double));
     memcpy(p->h_mix + (size_t)nk * dd, w, (size_t)nk * sizeof(double));
     int *h_idx = reinterpret_cast<int *>(p->h_mix + (size_t)nk * (dd + 1));      // [nk] scratch slots 0..nk-1 | [n] P-cache slots
@@ -1610,191 +1669,196 @@ int hb2_evaluate_classes(hb2_partition *p, const double *weights, int64_t nUpdat
     return evaluate_impl(p, 0, (int)p->C, weights, nUpdate, updateNodes, rootFreqs, lnL, siteL, siteScale);
 }
 
-// What a batch call produces.  Likelihoods (siteLnL) of partition patterns (patternOf) or of caller columns (columns
-// [nSets][L], hb2_create's leaf codes); or, with sim, nReps simulated columns of every set.
-struct BatchJob {
+// A batch call: its entry point, the sets' models, and what it produces -- likelihoods (siteLnL) of partition patterns
+// (patternOf) or of caller columns (columns [nSets][L], hb2_create's leaf codes), or nReps simulated columns of every set.
+// weights == nullptr: one matrix per branch, row b = branch b (FEL's site model).  Otherwise branch b owns branchK[b]
+// (NULL: K) consecutive component rows and its transition matrix is the weighted sum of their exponentials, formed inside
+// prune_batch_kernel<true> or sim_cdf_kernel<true> (MEME's site model).
+enum class BatchEntry { Sites, MixtureSites, Columns, Simulate };
+struct BatchCall {
+    BatchEntry entry;
+    int64_t templateId, nSets, K;
+    const int64_t *branchK, *branchGroup;
+    const double *formulaValues, *weights, *rootFreqs;
     const int64_t *patternOf = nullptr, *columns = nullptr;
     double *siteLnL = nullptr;
-    bool sim = false;
     int64_t nReps = 0, firstSet = 0, firstRep = 0;
     uint64_t seed = 0;
     int64_t *leafStates = nullptr, *nodeStates = nullptr;
 };
 
-// Body of every batch entry point.  weights == nullptr: one matrix per branch, row b = branch b (FEL's site model).
-// Otherwise branch b owns branchK[b] (NULL: K) consecutive component rows and its transition matrix is the weighted sum of
-// their exponentials, formed inside prune_batch_kernel<true> or sim_cdf_kernel<true> (MEME's site model).
-static int batch_sites(hb2_partition *p, int64_t templateId, int64_t nSets, int64_t K, const int64_t *branchK,
-                       const double *formulaValues, const double *weights, const int64_t *branchGroup, const double *rootFreqs,
-                       const BatchJob &job) {
-    if (!p || !formulaValues || !rootFreqs || (job.sim ? !job.leafStates : (!job.siteLnL || !(job.patternOf || job.columns))))
-        return fail("null argument");
-    if (nSets < 0) return fail("bad set count");
+// Every refusal of the batch entry points, before anything is launched or written.
+static int check_batch(const hb2_partition *p, const BatchCall &c) {
+    const bool sites = c.entry == BatchEntry::Sites || c.entry == BatchEntry::MixtureSites, sim = c.entry == BatchEntry::Simulate;
+    const char *fn = sim ? "hb2_batch_site_simulate" : "hb2_batch_column_likelihoods";
+    if (!p) return fail(c.entry == BatchEntry::Sites ? "null argument" : "null partition");
+    if (sites) {
+        if (c.entry == BatchEntry::MixtureSites && !c.weights) return fail("weights must not be null");
+        if (c.entry == BatchEntry::MixtureSites && !c.formulaValues) return fail("formulaValues must not be null");
+        if (!c.formulaValues || !c.rootFreqs || !c.siteLnL || !c.patternOf) return fail("null argument");
+        if (c.nSets < 0) return fail("bad set count");
+    } else {
+        if (c.nSets < 0) return fail("%s: nSets=%lld is negative", fn, (long long)c.nSets);
+        if (sim) {
+            if (c.nReps < 0) return fail("%s: nReps=%lld is negative", fn, (long long)c.nReps);
+            if (c.firstRep < 0 || c.firstRep > INT64_MAX - c.nReps) return fail("%s: firstRep=%lld out of range", fn, (long long)c.firstRep);
+            if (c.firstSet < 0 || c.firstSet > ((int64_t)1 << 32) - c.nSets)
+                return fail("%s: firstSet=%lld out of range (firstSet + nSets must not exceed 2^32)", fn, (long long)c.firstSet);
+        } else if (!c.columns) {
+            return fail("%s: columns must not be null", fn);
+        }
+        if (!c.formulaValues) return fail("%s: formulaValues must not be null", fn);
+        if (!c.rootFreqs) return fail("%s: rootFreqs must not be null", fn);
+        if (sim ? !c.leafStates : !c.siteLnL) return fail("%s: %s must not be null", fn, sim ? "leafStates" : "siteLnL");
+    }
+    // component counts: with weights, K in 1..4 and branchK (nullable) in 1..K; without, one row per branch
+    if (!c.weights && (c.K != 1 || c.branchK))
+        return fail("K=%lld and branchK need weights: without them every branch has one row (K=1, branchK NULL)", (long long)c.K);
+    if (c.weights && (c.K < 1 || c.K > 4)) return fail("K=%lld outside 1..4", (long long)c.K);
+    for (int64_t b = 0; c.weights && c.branchK && b < p->B; b++)
+        if (c.branchK[b] < 1 || c.branchK[b] > c.K)
+            return fail("branchK[%lld]=%lld outside 1..%lld", (long long)b, (long long)c.branchK[b], (long long)c.K);
     if (p->Dp != 64) return fail("hb2_batch_site_likelihoods supports 33..64-state (codon) partitions only");
-    if (templateId < 0 || templateId >= (int64_t)p->tmpls.size() || p->tmpls[templateId].nnz == 0) return fail("template %lld has not been defined", (long long)templateId);
+    if (c.templateId < 0 || c.templateId >= (int64_t)p->tmpls.size() || p->tmpls[c.templateId].nnz == 0)
+        return fail("template %lld has not been defined", (long long)c.templateId);
     if (p->cg_G > 1) return fail("hb2_batch_site_likelihoods is not available with class groups (shard the SETS across ranks instead)");
-    int gps = 1;                                // shared-powers groups per set: branches with the same branchGroup share a direction
-    if (branchGroup)
-        for (int64_t b = 0; b < p->B; b++) {
-            if (branchGroup[b] < 0 || branchGroup[b] >= 8) return fail("branchGroup[%lld]=%lld outside 0..7", (long long)b, (long long)branchGroup[b]);
-            gps = std::max(gps, (int)branchGroup[b] + 1);
-        }
-    for (int64_t s = 0; job.patternOf && s < nSets; s++)
-        if (job.patternOf[s] < 0 || job.patternOf[s] >= p->S) return fail("patternOf[%lld]=%lld out of range", (long long)s, (long long)job.patternOf[s]);
-    for (int64_t s = 0; job.columns && s < nSets; s++)
+    for (int64_t b = 0; c.branchGroup && b < p->B; b++)
+        if (c.branchGroup[b] < 0 || c.branchGroup[b] >= 8) return fail("branchGroup[%lld]=%lld outside 0..7", (long long)b, (long long)c.branchGroup[b]);
+    for (int64_t s = 0; c.patternOf && s < c.nSets; s++)
+        if (c.patternOf[s] < 0 || c.patternOf[s] >= p->S) return fail("patternOf[%lld]=%lld out of range", (long long)s, (long long)c.patternOf[s]);
+    for (int64_t s = 0; c.columns && s < c.nSets; s++)
         for (int64_t l = 0; l < p->L; l++) {
-            const int64_t c = job.columns[s * p->L + l];
-            if (c >= p->D || c < -p->nAmb)
+            const int64_t code = c.columns[s * p->L + l];
+            if (code >= p->D || code < -p->nAmb)
                 return fail("hb2_batch_column_likelihoods: set %lld, leaf %lld: code %lld is neither a state 0..%lld nor an ambiguity row -1..-%lld",
-                            (long long)s, (long long)l, (long long)c, (long long)p->D - 1, (long long)p->nAmb);
+                            (long long)s, (long long)l, (long long)code, (long long)p->D - 1, (long long)p->nAmb);
         }
-    std::vector<double> root_cdf(p->D);
-    int root_last = -1;
-    if (job.sim && !sim_prefix(rootFreqs, p->D, root_cdf.data(), &root_last))
+    double root_cdf[64];
+    int root_last;
+    if (sim && !sim_prefix(c.rootFreqs, p->D, root_cdf, &root_last))
         return fail("hb2_batch_site_simulate: root frequencies must be >= 0 and not NaN, with a finite positive total");
-    if (nSets == 0 || (job.sim && job.nReps == 0)) return 0;
-    CU(cudaSetDevice(p->device));
-    const hb2_partition::Tmpl &t = p->tmpls[templateId];
-    const int64_t B = p->B, nF = t.nF, D = p->D, L = p->L, I = p->I;
-    const bool mix = weights != nullptr;
-    // component rows of a set: branch b owns rows row_off[b] .. row_off[b+1]-1.  Component k of every tested branch is the
-    // same rate matrix up to the branch length, so the shared-powers group of a row is (set, branchGroup[b], k).
-    std::vector<int> row_off(B + 1, 0);
-    for (int64_t b = 0; b < B; b++) row_off[b + 1] = row_off[b] + (int)(mix && branchK ? branchK[b] : K);
-    const int64_t R = row_off[B];
-    const int gk = gps * (int)K;                // groups per set
+    return 0;
+}
+
+static BatchShape batch_shape(const hb2_partition *p, const BatchCall &c) {
+    const int64_t B = p->B, D = p->D;
+    BatchShape sh;
+    sh.nF = p->tmpls[c.templateId].nF;
+    // component k of every tested branch is the same rate matrix up to the branch length, so the shared-powers group of a
+    // row is (set, branchGroup[b], k)
+    sh.row_off.assign(B + 1, 0);
+    for (int64_t b = 0; b < B; b++) sh.row_off[b + 1] = sh.row_off[b] + (int)(c.weights && c.branchK ? c.branchK[b] : c.K);
+    sh.R = sh.row_off[B];
+    int64_t gps = 1;                            // groups per set and component: branches with the same branchGroup share one
+    for (int64_t b = 0; c.branchGroup && b < B; b++) gps = std::max(gps, c.branchGroup[b] + 1);
+    sh.gk = gps * c.K;
     // chunk buffers, capped at ~8 GB; a simulation adds the prefix sums and last positive columns of the set's B matrices
-    const double sim_bytes = job.sim ? (double)B * D * (64 * 8 + 4) : 0.0;
-    int64_t cap;
-    if (!mix)                                   // P matrices of `cap` sets (32 KB per branch)
-        cap = std::min<int64_t>(nSets, std::max<int64_t>(1, (int64_t)(8.0e9 / ((double)B * (4096 + 1024 + (double)nF) * 8 + sim_bytes))));
-    else {                                      // a set's R component matrices, formula values and weights,
+    const double sim_bytes = c.entry == BatchEntry::Simulate ? (double)B * D * (64 * 8 + 4) : 0.0;
+    double per_set;
+    if (!c.weights)                             // P matrices (32 KB per branch)
+        per_set = (double)B * (4096 + 1024 + (double)sh.nF) * 8;
+    else                                        // a set's R component matrices, formula values and weights,
                                                 // the power tables of its groups and its node vectors
-        const double per_set = (double)R * (4096 + (double)nF + 1) * 8 + (double)gk * hb2::EXPM_POW_TERMS * 4096 * 8 + (double)p->I * 64 * 8;
-        cap = std::min<int64_t>(nSets, std::max<int64_t>(1, (int64_t)(8.0e9 / (per_set + sim_bytes))));
-    }
-    cap = std::min<int64_t>(cap, 1024);
-    // the buffers hold b_cap sets of up to bex.cap / b_cap rows; chunks are b_cap sets wherever they came from
-    if (cap > p->b_cap || gk > p->b_groups_per_set || p->b_cap * R > p->bex.cap || p->b_cap * R * nF > p->b_vcap) {
-        CU(cudaStreamSynchronize(p->stream));
-        p->b_cap = 0; p->b_vcap = 0;
-        const int64_t ne = cap * R;
-        if (p->bex.alloc((int)(cap * gk), ne, p->stream) || p->d_bPT.alloc((size_t)ne * 4096) || p->d_bV.alloc((size_t)ne * nF) ||
-            p->d_bcond.alloc((size_t)cap * p->I * 64) || p->d_bnodeex.alloc((size_t)cap * p->I) || p->d_bout.alloc(cap) || p->d_bdst.alloc(ne) ||
-            p->d_bpat.alloc(cap) || p->h_bdst.alloc(ne + cap + cap * L) || p->d_bmixw.alloc(ne) || p->d_brow.alloc(B + 1) ||
-            p->d_bcol.alloc((size_t)cap * L) || p->d_bpi.alloc(64))
-            return 1;
-        p->b_cap = cap; p->b_groups_per_set = gk; p->b_vcap = ne * nF;
-    }
-    // a simulation keeps to its own cap (its table comes on top of buffers an earlier call may have sized for more sets)
-    const int64_t sets_per_chunk = job.sim ? std::min(p->b_cap, cap) : p->b_cap;
-    CU(cudaStreamSynchronize(p->stream));
-    if (stage_root(p, rootFreqs, nullptr, 0, p->d_bpi)) return 1;
-    if (mix) CU(cudaMemcpyAsync(p->d_brow, row_off.data(), (size_t)(B + 1) * sizeof(int), cudaMemcpyHostToDevice, p->stream));
-    // simulation: the chunk's table, the root's prefix sums, and one launch of columns (set-major, replicates consecutive)
-    hb2::SimArgs sa{};
-    int64_t chunk = 0;
-    size_t sim_smem = 0;
-    std::vector<int> ints;
-    if (job.sim) {
-        const int64_t nbm = std::min(sets_per_chunk, nSets);
-        chunk = job.nReps >= SIM_CHUNK ? SIM_CHUNK : std::min(SIM_CHUNK, nbm * job.nReps);
-        const bool smem_states = (size_t)I * SIM_THREADS <= SIM_SMEM_MAX;
-        hb2_partition::SimBuf &sb = p->sim;
-        if (sim_reserve(p, sb.cdf, sb.cap[0], (size_t)nbm * B * D * 64) || sim_reserve(p, sb.vec, sb.cap[1], (size_t)D) ||
-            sim_reserve(p, sb.ints, sb.cap[2], (size_t)nbm * B * D + nbm + 2) || sim_reserve(p, sb.leaf, sb.cap[3], (size_t)L * chunk) ||
-            (job.nodeStates && sim_reserve(p, sb.node, sb.cap[4], (size_t)I * chunk)) ||
-            (!smem_states && sim_reserve(p, sb.states, sb.cap[6], (size_t)I * chunk)))
-            return 1;
-        ints.assign(nbm + 2, 1);                // every set of a chunk is active | last root state | first bad row
-        ints[nbm] = root_last; ints[nbm + 1] = INT_MAX;
-        int *d_ints = sb.ints + nbm * B * D;
-        CU(cudaMemcpyAsync(sb.vec, root_cdf.data(), (size_t)D * sizeof(double), cudaMemcpyHostToDevice, p->stream));
-        CU(cudaMemcpyAsync(d_ints, ints.data(), ints.size() * sizeof(int), cudaMemcpyHostToDevice, p->stream));
-        sa.PT = p->d_bPT; sa.cdf = sb.cdf; sa.last = sb.ints; sa.active = d_ints; sa.root_last = d_ints + nbm; sa.bad = d_ints + nbm + 1;
-        sa.root_cdf = sb.vec;
-        sa.tree.child_start = p->d_child_start; sa.tree.child_ids = p->d_child_ids;
-        sa.leaf_out = sb.leaf; sa.node_out = job.nodeStates ? (long long *)sb.node : nullptr;
-        sa.states = smem_states ? nullptr : (unsigned char *)sb.states;
-        sa.L = (int)L; sa.I = (int)I; sa.B = (int)B; sa.D = (int)D; sa.Dp = 64; sa.chunk = (int)chunk;
-        sa.g0 = (unsigned long long)job.firstRep; sa.key = make_uint2((unsigned)job.seed, (unsigned)(job.seed >> 32));
-        sa.mix_w = p->d_bmixw; sa.row_off = p->d_brow; sa.R = (int)R; sa.reps = job.nReps;
-        sim_smem = smem_states ? (size_t)I * SIM_THREADS : 0;
-    }
-    std::vector<int> grp;
-    for (int64_t s0 = 0; s0 < nSets; s0 += sets_per_chunk) {
-        const int64_t nb = std::min<int64_t>(sets_per_chunk, nSets - s0), ne = nb * R;
-        CU(cudaStreamSynchronize(p->stream));          // previous chunk done: buffers and pinned arrays are free again
-        for (int64_t e = 0; e < ne; e++) p->h_bdst[e] = (int)e;                      // slot in the chunk's P area: [set][row]
-        CU(cudaMemcpyAsync(p->d_bdst, p->h_bdst, (size_t)ne * sizeof(int), cudaMemcpyHostToDevice, p->stream));
-        if (!job.sim) {
-            // set s prunes pattern pat[s] of leaf[L][Sp]: the partition's patterns, or the chunk's columns as leaf[L][nb]
-            for (int64_t s = 0; s < nb; s++) p->h_bdst[ne + s] = job.columns ? (int)s : (int)job.patternOf[s0 + s];
-            CU(cudaMemcpyAsync(p->d_bpat, p->h_bdst + ne, (size_t)nb * sizeof(int), cudaMemcpyHostToDevice, p->stream));
-            if (job.columns) {
-                int *hc = p->h_bdst + ne + nb;
-                for (int64_t s = 0; s < nb; s++)
-                    for (int64_t l = 0; l < L; l++) hc[l * nb + s] = (int)job.columns[(s0 + s) * L + l];
-                CU(cudaMemcpyAsync(p->d_bcol, hc, (size_t)L * nb * sizeof(int), cudaMemcpyHostToDevice, p->stream));
-            }
-        }
-        CU(cudaMemcpyAsync(p->d_bV, formulaValues + (size_t)s0 * R * nF, (size_t)ne * nF * sizeof(double), cudaMemcpyHostToDevice, p->stream));
-        if (mix) CU(cudaMemcpyAsync(p->d_bmixw, weights + (size_t)s0 * R, (size_t)ne * sizeof(double), cudaMemcpyHostToDevice, p->stream));
-        grp.resize(ne);
+        per_set = (double)sh.R * (4096 + (double)sh.nF + 1) * 8 + (double)sh.gk * hb2::EXPM_POW_TERMS * 4096 * 8 + (double)p->I * 64 * 8;
+    sh.sets = std::min<int64_t>({c.nSets, std::max<int64_t>(1, (int64_t)(8.0e9 / (per_set + sim_bytes))), 1024});
+    return sh;
+}
+
+// Uploads the formula values (and weights) of sets s0 .. s0+nb-1, plans their shared-powers groups and exponentiates them
+// into the chunk's P area, PT[set][row].
+static int exponentiate_chunk(hb2_partition *p, const BatchCall &c, const BatchShape &sh, int64_t s0, int64_t nb) {
+    hb2_partition::BatchWorkspace &ws = p->batch;
+    const int64_t R = sh.R, ne = nb * R;
+    CU(cudaMemcpyAsync(ws.V, c.formulaValues + (size_t)s0 * R * sh.nF, (size_t)ne * sh.nF * sizeof(double), cudaMemcpyHostToDevice, p->stream));
+    if (c.weights) CU(cudaMemcpyAsync(ws.mixw, c.weights + (size_t)s0 * R, (size_t)ne * sizeof(double), cudaMemcpyHostToDevice, p->stream));
+    std::vector<int> grp(ne);
+    for (int64_t s = 0; s < nb; s++)
+        for (int64_t b = 0; b < p->B; b++)
+            for (int k = 0; k < sh.row_off[b + 1] - sh.row_off[b]; k++)
+                grp[s * R + sh.row_off[b] + k] = (int)(s * sh.gk + (c.branchGroup ? c.branchGroup[b] : 0) * c.K + k);
+    SharedPlan sp;
+    // every chunk rebuilds its tables: a group with fewer than 4 branches must not be compared with a direction cached by
+    // an earlier chunk or call, whose table may come from another template or other column frequencies
+    std::fill(ws.ex.kind.begin(), ws.ex.kind.end(), 0);
+    CU(cudaMemsetAsync(ws.ex.d_groups, 0, (size_t)ws.ex.G * sizeof(hb2::ExpmGroup), p->stream));
+    if (plan_shared(p, ws.h_slot, ne, 1, grp.data(), sp, (int)c.templateId, &ws.ex, 4) || staged_uploads(p)) return 1;
+    // the chunk's P area is scratch: no resident copy is kept
+    return launch_expm(p, {Kind::Compiled, (int)c.templateId}, ws.V, ws.slot, (int)ne, false, sp, 0, ws.PT);
+}
+
+// Likelihoods of sets s0 .. s0+nb-1 from the chunk's P area.
+static int score_chunk(hb2_partition *p, const BatchCall &c, const BatchShape &sh, int64_t s0, int64_t nb) {
+    hb2_partition::BatchWorkspace &ws = p->batch;
+    const int64_t L = p->L;
+    // set s prunes pattern pat[s] of leaf[L][Sp]: the partition's patterns, or the chunk's columns as leaf[L][nb]
+    for (int64_t s = 0; s < nb; s++) ws.h_pat[s] = c.columns ? (int)s : (int)c.patternOf[s0 + s];
+    CU(cudaMemcpyAsync(ws.pat, ws.h_pat, (size_t)nb * sizeof(int), cudaMemcpyHostToDevice, p->stream));
+    if (c.columns) {
         for (int64_t s = 0; s < nb; s++)
-            for (int64_t b = 0; b < B; b++)
-                for (int k = 0; k < row_off[b + 1] - row_off[b]; k++)
-                    grp[s * R + row_off[b] + k] = (int)(s * p->b_groups_per_set + (branchGroup ? branchGroup[b] : 0) * K + k);
-        SharedPlan sp;
-        // every chunk rebuilds its tables: a group with fewer than 4 branches must not be compared with a direction cached by
-        // an earlier chunk or call, whose table may come from another template or other column frequencies
-        std::fill(p->bex.kind.begin(), p->bex.kind.end(), 0);
-        CU(cudaMemsetAsync(p->bex.d_groups, 0, (size_t)p->bex.G * sizeof(hb2::ExpmGroup), p->stream));
-        if (plan_shared(p, p->h_bdst, ne, 1, grp.data(), sp, (int)templateId, &p->bex, 4) || staged_uploads(p)) return 1;
-        // the chunk's P area is scratch: no resident copy is kept
-        if (launch_expm(p, {Kind::Compiled, (int)templateId}, p->d_bV, p->d_bdst, (int)ne, false, sp, 0, p->d_bPT)) return 1;
-        if (job.sim) {
-            // the table of every (set, branch), and its check, before any column of the chunk is drawn
-            sa.t0 = (unsigned)(job.firstSet + s0);
-            if (mix) hb2::sim_cdf_kernel<true><<<(unsigned)(nb * B), 64, 0, p->stream>>>(sa);
-            else hb2::sim_cdf_kernel<false><<<(unsigned)(nb * B), 64, 0, p->stream>>>(sa);
-            p->launches++;
-            CU(cudaGetLastError());
-            int chk[2] = {INT_MAX, 0};          // first bad row | device-side wait error
-            CU(cudaMemcpyAsync(&chk[0], sa.bad, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
-            CU(cudaMemcpyAsync(&chk[1], p->d_err, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
-            CU(cudaStreamSynchronize(p->stream));
-            if (chk[1]) { cudaMemsetAsync(p->d_err, 0, sizeof(int), p->stream); return fail("a device-side wait timed out in the batched exponential (code %d)", chk[1]); }
-            if (chk[0] != INT_MAX) {
-                const long long row = chk[0] % D, cb = chk[0] / D;
-                return fail("hb2_batch_site_simulate: row %lld of the transition matrix of set %lld, branch %lld does not have a finite positive total",
-                            row, (long long)s0 + cb / B, cb % B);
-            }
-            const int64_t ncol = nb * job.nReps;
-            for (int64_t c0 = 0; c0 < ncol; c0 += chunk) {
-                const int64_t n = std::min(chunk, ncol - c0);
-                sa.n = (int)n; sa.col0 = c0;
-                hb2::batch_simulate_kernel<<<(unsigned)((n + SIM_THREADS - 1) / SIM_THREADS), SIM_THREADS, sim_smem, p->stream>>>(sa);
-                p->launches++;
-                CU(cudaGetLastError());
-                const size_t col = (size_t)s0 * job.nReps + c0;
-                CU(cudaMemcpyAsync(job.leafStates + col * L, sa.leaf_out, (size_t)n * L * sizeof(int64_t), cudaMemcpyDeviceToHost, p->stream));
-                if (job.nodeStates)
-                    CU(cudaMemcpyAsync(job.nodeStates + col * I, sa.node_out, (size_t)n * I * sizeof(int64_t), cudaMemcpyDeviceToHost, p->stream));
-            }
-            continue;
-        }
-        hb2::BatchPruneArgs ba;
-        ba.PT = p->d_bPT; ba.cond = p->d_bcond; ba.node_ex = p->d_bnodeex; ba.pat = p->d_bpat; ba.ambig = p->d_ambig; ba.pi = p->d_bpi;
-        ba.leaf = job.columns ? (const int *)p->d_bcol : (const int *)p->d_leaf;
-        ba.tree.child_start = p->d_child_start; ba.tree.child_ids = p->d_child_ids; ba.out = p->d_bout;
-        ba.L = (int)p->L; ba.I = (int)p->I; ba.B = (int)B; ba.D = (int)p->D; ba.Sp = job.columns ? (int)nb : (int)p->Sp;
-        ba.mix_w = p->d_bmixw; ba.row_off = p->d_brow; ba.R = (int)R;
-        if (mix) hb2::prune_batch_kernel<true><<<(unsigned)nb, 64, 0, p->stream>>>(ba);
-        else hb2::prune_batch_kernel<false><<<(unsigned)nb, 64, 0, p->stream>>>(ba);
+            for (int64_t l = 0; l < L; l++) ws.h_col[l * nb + s] = (int)c.columns[(s0 + s) * L + l];
+        CU(cudaMemcpyAsync(ws.col, ws.h_col, (size_t)L * nb * sizeof(int), cudaMemcpyHostToDevice, p->stream));
+    }
+    hb2::BatchPruneArgs ba;
+    ba.PT = ws.PT; ba.cond = ws.cond; ba.node_ex = ws.node_ex; ba.pat = ws.pat; ba.ambig = p->d_ambig; ba.pi = ws.pi;
+    ba.leaf = c.columns ? (const int *)ws.col : (const int *)p->d_leaf;
+    ba.tree.child_start = p->d_child_start; ba.tree.child_ids = p->d_child_ids; ba.out = ws.out;
+    ba.L = (int)L; ba.I = (int)p->I; ba.B = (int)p->B; ba.D = (int)p->D; ba.Sp = c.columns ? (int)nb : (int)p->Sp;
+    ba.mix_w = ws.mixw; ba.row_off = ws.row; ba.R = (int)sh.R;
+    if (c.weights) hb2::prune_batch_kernel<true><<<(unsigned)nb, 64, 0, p->stream>>>(ba);
+    else hb2::prune_batch_kernel<false><<<(unsigned)nb, 64, 0, p->stream>>>(ba);
+    p->launches++;
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(c.siteLnL + s0, ws.out, (size_t)nb * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
+    return 0;
+}
+
+// nReps columns of each of sets s0 .. s0+nb-1 from the chunk's P area: the chunk's table and its check, then launches of
+// columns (set-major, a set's replicates consecutive) copied to the caller's [nSets][nReps][L] (and [I]) arrays.
+static int simulate_chunk(hb2_partition *p, const BatchCall &c, const BatchShape &sh, int64_t s0, int64_t nb) {
+    const int64_t L = p->L, I = p->I;
+    const int64_t chunk = c.nReps >= SIM_CHUNK ? SIM_CHUNK : std::min(SIM_CHUNK, sh.sets * c.nReps);   // columns per launch
+    std::vector<double> root_cdf(p->D);
+    std::vector<int> ints(nb + 3, 1);           // every set of the chunk is active | no class | last root state | first bad row
+    sim_prefix(c.rootFreqs, p->D, root_cdf.data(), &ints[nb + 1]);     // checked with the call's arguments
+    ints[nb] = 0; ints[nb + 2] = INT_MAX;
+    hb2::SimArgs a{};
+    a.PT = p->batch.PT; a.mix_w = p->batch.mixw; a.row_off = p->batch.row; a.R = (int)sh.R; a.reps = c.nReps;
+    a.g0 = (unsigned long long)c.firstRep; a.t0 = (unsigned)(c.firstSet + s0);
+    if (sim_tables(p, a, nb, chunk, c.seed, root_cdf, ints, c.nodeStates, false, c.weights, "hb2_batch_site_simulate",
+                   "set %lld, branch %lld", s0))
+        return 1;
+    const size_t smem = a.states ? 0 : (size_t)I * SIM_THREADS;
+    const int64_t ncol = nb * c.nReps;
+    for (int64_t c0 = 0; c0 < ncol; c0 += chunk) {
+        const int64_t n = std::min(chunk, ncol - c0);
+        a.n = (int)n; a.col0 = c0;
+        hb2::batch_simulate_kernel<<<(unsigned)((n + SIM_THREADS - 1) / SIM_THREADS), SIM_THREADS, smem, p->stream>>>(a);
         p->launches++;
         CU(cudaGetLastError());
-        CU(cudaMemcpyAsync(job.siteLnL + s0, p->d_bout, (size_t)nb * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
+        const size_t col = (size_t)s0 * c.nReps + c0;
+        CU(cudaMemcpyAsync(c.leafStates + col * L, a.leaf_out, (size_t)n * L * sizeof(int64_t), cudaMemcpyDeviceToHost, p->stream));
+        if (c.nodeStates)
+            CU(cudaMemcpyAsync(c.nodeStates + col * I, a.node_out, (size_t)n * I * sizeof(int64_t), cudaMemcpyDeviceToHost, p->stream));
+    }
+    return 0;
+}
+
+// Body of every batch entry point: per chunk of sets, the batched exponential, then the call's consumer.
+static int batch_sites(hb2_partition *p, const BatchCall &c) {
+    if (check_batch(p, c)) return 1;
+    const bool sim = c.entry == BatchEntry::Simulate;
+    if (c.nSets == 0 || (sim && c.nReps == 0)) return 0;
+    CU(cudaSetDevice(p->device));
+    const BatchShape sh = batch_shape(p, c);
+    if (p->batch.fit(sh, p->L, p->I, p->stream)) return 1;
+    CU(cudaStreamSynchronize(p->stream));
+    if (stage_root(p, c.rootFreqs, nullptr, 0, p->batch.pi)) return 1;
+    if (c.weights) CU(cudaMemcpyAsync(p->batch.row, sh.row_off.data(), sh.row_off.size() * sizeof(int), cudaMemcpyHostToDevice, p->stream));
+    for (int64_t s0 = 0; s0 < c.nSets; s0 += sh.sets) {
+        const int64_t nb = std::min(sh.sets, c.nSets - s0);
+        CU(cudaStreamSynchronize(p->stream));          // previous chunk done: buffers and pinned arrays are free again
+        if (exponentiate_chunk(p, c, sh, s0, nb) || (sim ? simulate_chunk(p, c, sh, s0, nb) : score_chunk(p, c, sh, s0, nb)))
+            return 1;
     }
     int err = 0;
     CU(cudaMemcpyAsync(&err, p->d_err, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
@@ -1803,71 +1867,32 @@ static int batch_sites(hb2_partition *p, int64_t templateId, int64_t nSets, int6
     return 0;
 }
 
-// Component counts of a batch call: with weights, K in 1..4 and branchK (nullable) in 1..K; without, one row per branch.
-static int check_rows(const hb2_partition *p, int64_t K, const int64_t *branchK, const double *weights) {
-    if (!weights) {
-        if (K != 1 || branchK) return fail("K=%lld and branchK need weights: without them every branch has one row (K=1, branchK NULL)", (long long)K);
-        return 0;
-    }
-    if (K < 1 || K > 4) return fail("K=%lld outside 1..4", (long long)K);
-    if (branchK)
-        for (int64_t b = 0; b < p->B; b++)
-            if (branchK[b] < 1 || branchK[b] > K) return fail("branchK[%lld]=%lld outside 1..%lld", (long long)b, (long long)branchK[b], (long long)K);
-    return 0;
-}
-
 int hb2_batch_site_likelihoods(hb2_partition *p, int64_t templateId, int64_t nSets, const int64_t *patternOf,
                                const double *formulaValues, const int64_t *branchGroup, const double *rootFreqs, double *siteLnL) {
-    BatchJob job;
-    job.patternOf = patternOf; job.siteLnL = siteLnL;
-    return batch_sites(p, templateId, nSets, 1, nullptr, formulaValues, nullptr, branchGroup, rootFreqs, job);
+    return batch_sites(p, {BatchEntry::Sites, templateId, nSets, 1, nullptr, branchGroup, formulaValues, nullptr, rootFreqs,
+                           patternOf, nullptr, siteLnL});
 }
 
 int hb2_batch_site_mixture_likelihoods(hb2_partition *p, int64_t templateId, int64_t nSets, const int64_t *patternOf, int64_t K,
                                        const int64_t *branchK, const double *formulaValues, const double *weights,
                                        const int64_t *branchGroup, const double *rootFreqs, double *siteLnL) {
-    if (!p) return fail("null partition");
-    if (!weights) return fail("weights must not be null");
-    if (!formulaValues) return fail("formulaValues must not be null");
-    if (check_rows(p, K, branchK, weights)) return 1;
-    BatchJob job;
-    job.patternOf = patternOf; job.siteLnL = siteLnL;
-    return batch_sites(p, templateId, nSets, K, branchK, formulaValues, weights, branchGroup, rootFreqs, job);
+    return batch_sites(p, {BatchEntry::MixtureSites, templateId, nSets, K, branchK, branchGroup, formulaValues, weights, rootFreqs,
+                           patternOf, nullptr, siteLnL});
 }
 
 int hb2_batch_column_likelihoods(hb2_partition *p, int64_t templateId, int64_t nSets, const int64_t *columns, int64_t K,
                                  const int64_t *branchK, const double *formulaValues, const double *weights,
                                  const int64_t *branchGroup, const double *rootFreqs, double *siteLnL) {
-    if (!p) return fail("null partition");
-    if (nSets < 0) return fail("hb2_batch_column_likelihoods: nSets=%lld is negative", (long long)nSets);
-    if (!columns) return fail("hb2_batch_column_likelihoods: columns must not be null");
-    if (!formulaValues) return fail("hb2_batch_column_likelihoods: formulaValues must not be null");
-    if (!rootFreqs) return fail("hb2_batch_column_likelihoods: rootFreqs must not be null");
-    if (!siteLnL) return fail("hb2_batch_column_likelihoods: siteLnL must not be null");
-    if (check_rows(p, K, branchK, weights)) return 1;
-    BatchJob job;
-    job.columns = columns; job.siteLnL = siteLnL;
-    return batch_sites(p, templateId, nSets, K, branchK, formulaValues, weights, branchGroup, rootFreqs, job);
+    return batch_sites(p, {BatchEntry::Columns, templateId, nSets, K, branchK, branchGroup, formulaValues, weights, rootFreqs,
+                           nullptr, columns, siteLnL});
 }
 
 int hb2_batch_site_simulate(hb2_partition *p, int64_t templateId, int64_t nSets, int64_t K, const int64_t *branchK,
                             const double *formulaValues, const double *weights, const int64_t *branchGroup,
                             const double *rootFreqs, int64_t nReps, uint64_t seed, int64_t firstSet, int64_t firstRep,
                             int64_t *leafStates, int64_t *nodeStates) {
-    if (!p) return fail("null partition");
-    if (nSets < 0) return fail("hb2_batch_site_simulate: nSets=%lld is negative", (long long)nSets);
-    if (nReps < 0) return fail("hb2_batch_site_simulate: nReps=%lld is negative", (long long)nReps);
-    if (firstRep < 0 || firstRep > INT64_MAX - nReps) return fail("hb2_batch_site_simulate: firstRep=%lld out of range", (long long)firstRep);
-    if (firstSet < 0 || firstSet > ((int64_t)1 << 32) - nSets)
-        return fail("hb2_batch_site_simulate: firstSet=%lld out of range (firstSet + nSets must not exceed 2^32)", (long long)firstSet);
-    if (!formulaValues) return fail("hb2_batch_site_simulate: formulaValues must not be null");
-    if (!rootFreqs) return fail("hb2_batch_site_simulate: rootFreqs must not be null");
-    if (!leafStates) return fail("hb2_batch_site_simulate: leafStates must not be null");
-    if (check_rows(p, K, branchK, weights)) return 1;
-    BatchJob job;
-    job.sim = true; job.nReps = nReps; job.seed = seed; job.firstSet = firstSet; job.firstRep = firstRep;
-    job.leafStates = leafStates; job.nodeStates = nodeStates;
-    return batch_sites(p, templateId, nSets, K, branchK, formulaValues, weights, branchGroup, rootFreqs, job);
+    return batch_sites(p, {BatchEntry::Simulate, templateId, nSets, K, branchK, branchGroup, formulaValues, weights, rootFreqs,
+                           nullptr, nullptr, nullptr, nReps, firstSet, firstRep, seed, leafStates, nodeStates});
 }
 
 int hb2_read_conditionals(hb2_partition *p, int64_t cat, int64_t inode, double *cond, int32_t *exp2) {
@@ -1941,50 +1966,24 @@ int hb2_simulate(hb2_partition *p, const double *weights, const double *rootFreq
     CU(cudaSetDevice(p->device));
     if (flush_matrices(p)) return 1;
     const int64_t chunk = std::min(nSites, SIM_CHUNK);
-    const bool smem_states = (size_t)I * SIM_THREADS <= SIM_SMEM_MAX;
-    hb2_partition::SimBuf &sb = p->sim;
-    if (sim_reserve(p, sb.cdf, sb.cap[0], (size_t)C * B * D * p->Dp) || sim_reserve(p, sb.vec, sb.cap[1], vec.size()) ||
-        sim_reserve(p, sb.ints, sb.cap[2], (size_t)C * B * D + ints.size()) || sim_reserve(p, sb.leaf, sb.cap[3], (size_t)L * chunk) ||
-        (nodeStates && sim_reserve(p, sb.node, sb.cap[4], (size_t)I * chunk)) ||
-        (siteClass && sim_reserve(p, sb.cls, sb.cap[5], (size_t)chunk)) ||
-        (!smem_states && sim_reserve(p, sb.states, sb.cap[6], (size_t)I * chunk)))
-        return 1;
-    int *d_last = sb.ints, *d_ints = sb.ints + C * B * D;
-    CU(cudaMemcpyAsync(sb.vec, vec.data(), vec.size() * sizeof(double), cudaMemcpyHostToDevice, p->stream));
-    CU(cudaMemcpyAsync(d_ints, ints.data(), ints.size() * sizeof(int), cudaMemcpyHostToDevice, p->stream));
     hb2::SimArgs a{};
-    a.PT = p->d_PT; a.cdf = sb.cdf; a.last = d_last; a.active = d_ints; a.bad = d_ints + C + 2;
-    a.class_cdf = sb.vec; a.root_cdf = sb.vec + C; a.class_last = d_ints + C; a.root_last = d_ints + C + 1;
-    a.tree.child_start = p->d_child_start; a.tree.child_ids = p->d_child_ids;
-    a.leaf_out = sb.leaf; a.node_out = nodeStates ? (long long *)sb.node : nullptr; a.class_out = siteClass ? (int *)sb.cls : nullptr;
-    a.states = smem_states ? nullptr : (unsigned char *)sb.states;
-    a.L = (int)L; a.I = (int)I; a.B = (int)B; a.C = (int)C; a.D = (int)D; a.Dp = p->Dp; a.chunk = (int)chunk;
-    a.key = make_uint2((unsigned)seed, (unsigned)(seed >> 32));
+    a.PT = p->d_PT; a.C = (int)C;
     // the table of every drawn class, and its check: a refused call writes nothing
-    hb2::sim_cdf_kernel<false><<<(unsigned)(C * B), 64, 0, p->stream>>>(a);
-    p->launches++;
-    CU(cudaGetLastError());
-    int bad = INT_MAX;
-    CU(cudaMemcpyAsync(&bad, a.bad, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
-    CU(cudaStreamSynchronize(p->stream));
-    if (bad != INT_MAX) {
-        const long long row = bad % D, cb = bad / D;
-        return fail("hb2_simulate: row %lld of the transition matrix of rate class %lld, node %lld does not have a finite positive total",
-                    row, cb / B, cb % B);
-    }
-    const size_t smem = smem_states ? (size_t)I * SIM_THREADS : 0;
+    if (sim_tables(p, a, C, chunk, seed, vec, ints, nodeStates, siteClass, false, "hb2_simulate", "rate class %lld, node %lld", 0))
+        return 1;
+    const size_t smem = a.states ? 0 : (size_t)I * SIM_THREADS;
     for (int64_t s0 = 0; s0 < nSites; s0 += chunk) {
         const int64_t n = std::min(chunk, nSites - s0);
         a.n = (int)n; a.g0 = (unsigned long long)(firstSite + s0);
         hb2::simulate_kernel<<<(unsigned)((n + SIM_THREADS - 1) / SIM_THREADS), SIM_THREADS, smem, p->stream>>>(a);
         p->launches++;
         CU(cudaGetLastError());
-        CU(cudaMemcpy2DAsync(leafStates + s0, nSites * sizeof(int64_t), sb.leaf, chunk * sizeof(long long), n * sizeof(int64_t), L,
+        CU(cudaMemcpy2DAsync(leafStates + s0, nSites * sizeof(int64_t), a.leaf_out, chunk * sizeof(long long), n * sizeof(int64_t), L,
                              cudaMemcpyDeviceToHost, p->stream));
         if (nodeStates)
-            CU(cudaMemcpy2DAsync(nodeStates + s0, nSites * sizeof(int64_t), sb.node, chunk * sizeof(long long), n * sizeof(int64_t), I,
+            CU(cudaMemcpy2DAsync(nodeStates + s0, nSites * sizeof(int64_t), a.node_out, chunk * sizeof(long long), n * sizeof(int64_t), I,
                                  cudaMemcpyDeviceToHost, p->stream));
-        if (siteClass) CU(cudaMemcpyAsync(siteClass + s0, sb.cls, n * sizeof(int32_t), cudaMemcpyDeviceToHost, p->stream));
+        if (siteClass) CU(cudaMemcpyAsync(siteClass + s0, a.class_out, n * sizeof(int32_t), cudaMemcpyDeviceToHost, p->stream));
     }
     CU(cudaStreamSynchronize(p->stream));
     return 0;

@@ -1464,6 +1464,23 @@ __global__ void __launch_bounds__(256) class_merge_kernel(const double *gath, co
 // sum_c w_c PT_c[j][k], components in order as mix_reduce_kernel (tree.cpp:3047-3089), before it enters the contraction:
 // the mixed matrix never goes to memory.
 // ------------------------------------------------------------------------------------------------
+// A branch's mixture as a thread forms it (prune_batch_kernel<true>, sim_cdf_kernel<true>): mix_weights loads the weights
+// of its nc <= 4 component rows; mix_entry forms an entry of the mixed matrix as w_0 P_0, then fma(w_c, P_c, .) in
+// component order -- the order of mix_reduce_kernel -- from P(c), component c's entry.
+__device__ __forceinline__ void mix_weights(double (&w)[4], const double *ws, int nc) {
+#pragma unroll
+    for (int c = 0; c < 4; c++) w[c] = c < nc ? ws[c] : 0.0;
+}
+
+template <typename Component>
+__device__ __forceinline__ double mix_entry(const double (&w)[4], int nc, Component P) {
+    double v = w[0] * P(0);
+#pragma unroll
+    for (int c = 1; c < 4; c++)
+        if (c < nc) v = fma(w[c], P(c), v);
+    return v;
+}
+
 struct BatchPruneArgs {
     const double *PT;         // [nSets][B][4096]; MIX: [nSets][R][4096]
     double *cond;             // [nSets][I][64]
@@ -1518,20 +1535,11 @@ __global__ void __launch_bounds__(64) prune_batch_kernel(BatchPruneArgs a) {
             if constexpr (MIX) {
                 const int r0 = a.row_off[child];
                 nc = a.row_off[child + 1] - r0;
-                const double *ws = a.mix_w + (size_t)s * a.R + r0;      // same address in every thread: a broadcast
-#pragma unroll
-                for (int c = 0; c < 4; c++) wc[c] = c < nc ? ws[c] : 0.0;
+                mix_weights(wc, a.mix_w + (size_t)s * a.R + r0, nc);   // same address in every thread: a broadcast
             }
             auto entry = [&](int j) {
-                if constexpr (!MIX) {
-                    return PT[j * 64 + k];
-                } else {
-                    double e = wc[0] * PT[j * 64 + k];
-#pragma unroll
-                    for (int c = 1; c < 4; c++)
-                        if (c < nc) e = fma(wc[c], PT[(size_t)c * 4096 + j * 64 + k], e);
-                    return e;
-                }
+                if constexpr (!MIX) return PT[j * 64 + k];
+                else return mix_entry(wc, nc, [&](int c) { return PT[j * 64 + k + (size_t)c * 4096]; });
             };
             double m = 0.0;
             if (child < a.L) {
@@ -1670,21 +1678,16 @@ __global__ void __launch_bounds__(64) sim_cdf_kernel(SimArgs a) {
             const int b = (int)(cb - set * a.B), r0 = a.row_off[b];
             nc = a.row_off[b + 1] - r0;
             P = a.PT + ((size_t)set * a.R + r0) * a.Dp * a.Dp + row;
-#pragma unroll
-            for (int k = 0; k < 4; k++) wc[k] = k < nc ? a.mix_w[(size_t)set * a.R + r0 + k] : 0.0;
+            mix_weights(wc, a.mix_w + (size_t)set * a.R + r0, nc);
         }
         double *c = rows + row * SIM_CDF_LD;
         double s = 0.0;
         int last = -1;
 #pragma unroll 4
         for (int j = 0; j < a.D; j++) {
-            double v = P[(size_t)j * a.Dp];
-            if constexpr (MIX) {
-                v = wc[0] * v;
-#pragma unroll
-                for (int k = 1; k < 4; k++)
-                    if (k < nc) v = fma(wc[k], P[(size_t)k * a.Dp * a.Dp + (size_t)j * a.Dp], v);
-            }
+            double v;
+            if constexpr (!MIX) v = P[(size_t)j * a.Dp];
+            else v = mix_entry(wc, nc, [&](int k) { return P[(size_t)k * a.Dp * a.Dp + (size_t)j * a.Dp]; });
             if (v > 0.0) { s = __dadd_rn(s, v); last = j; }
             c[j] = s;
         }
@@ -1700,71 +1703,61 @@ __global__ void __launch_bounds__(64) sim_cdf_kernel(SimArgs a) {
     }
 }
 
-// One thread per site of the chunk: class, root state, then every internal node from the root down (flat post-order puts
-// a parent after its children), each child's state drawn from the row of its parent's state.  Internal states are bytes
-// in shared memory ([I][blockDim]) or, for trees with too many internal nodes, in global scratch ([I][chunk]).
-__global__ void __launch_bounds__(128) simulate_kernel(SimArgs a) {
+// The walk of simulate_kernel and batch_simulate_kernel, one thread per column: the block of the table (a rate class, or
+// a set), the root state, then every internal node from the root down (flat post-order puts a parent after its children),
+// each child's state drawn from the row of its parent's state.  Internal states are bytes in shared memory
+// ([I][blockDim]) or, for trees with too many internal nodes, in global scratch ([I][chunk]).
+// hb2_simulate (PER_SET false): thread i is site g0 + i; it draws its class, the fourth counter word is 0, and outputs
+// are site-minor: leaf_out [L][chunk], node_out [I][chunk], class_out [chunk].
+// Per-set mode (hb2_batch_site_simulate): thread i is column col0 + i = set * reps + replicate, consecutive threads on
+// consecutive replicates of one set.  The set is the block and t0 + set the fourth counter word; there is no class draw.
+// Outputs are column-major: leaf_out [n][L], node_out [n][I].
+template <bool PER_SET>
+__device__ __forceinline__ void sim_walk(const SimArgs &a) {
     extern __shared__ unsigned char sim_smem[];
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= a.n) return;
-    const unsigned long long g = a.g0 + (unsigned long long)i;
+    size_t blk = 0;
+    unsigned long long g = a.g0 + (unsigned long long)i;
+    unsigned t = 0u;
+    if constexpr (PER_SET) {
+        const long long col = a.col0 + i, set = col / a.reps;
+        g = a.g0 + (unsigned long long)(col - set * a.reps);
+        t = a.t0 + (unsigned)set;
+        blk = (size_t)set;
+    }
     const int L = a.L, I = a.I;
     unsigned char *st = a.states ? a.states + i : sim_smem + threadIdx.x;
     const size_t stride = a.states ? (size_t)a.chunk : (size_t)blockDim.x;
-    const int cls = a.C == 1 ? 0 : sim_draw(a.class_cdf, a.C, a.class_last, sim_uniform(g, (unsigned)(L + I), a.key));
-    if (a.class_out) a.class_out[i] = cls;
-    int s = sim_draw(a.root_cdf, a.D, a.root_last, sim_uniform(g, (unsigned)(L + I - 1), a.key));
-    if (a.node_out) a.node_out[(size_t)(I - 1) * a.chunk + i] = s;
-    const size_t cls_rows = (size_t)cls * a.B;
+    // output index of node n (leaves: len = L, internal nodes: len = I)
+    auto out = [&](int n, int len) { return PER_SET ? (size_t)i * len + n : (size_t)n * a.chunk + i; };
+    if constexpr (!PER_SET) {
+        const int cls = a.C == 1 ? 0 : sim_draw(a.class_cdf, a.C, a.class_last, sim_uniform(g, (unsigned)(L + I), a.key));
+        if (a.class_out) a.class_out[i] = cls;
+        blk = (size_t)cls;
+    }
+    int s = sim_draw(a.root_cdf, a.D, a.root_last, sim_uniform(g, (unsigned)(L + I - 1), a.key, t));
+    if (a.node_out) a.node_out[out(I - 1, I)] = s;
+    const size_t blk_rows = blk * a.B;
     for (int n = I - 1; n >= 0; n--) {
         if (n < I - 1) s = st[(size_t)n * stride];
         const int c_end = a.tree.child_start[n + 1];
         for (int ci = a.tree.child_start[n]; ci < c_end; ci++) {
             const int ch = a.tree.child_ids[ci];
-            const size_t r = (cls_rows + ch) * a.D + s;
-            const int x = sim_draw(a.cdf + r * a.Dp, a.D, a.last + r, sim_uniform(g, (unsigned)ch, a.key));
+            const size_t r = (blk_rows + ch) * a.D + s;
+            const int x = sim_draw(a.cdf + r * a.Dp, a.D, a.last + r, sim_uniform(g, (unsigned)ch, a.key, t));
             if (ch < L) {
-                a.leaf_out[(size_t)ch * a.chunk + i] = x;
+                a.leaf_out[out(ch, L)] = x;
             } else {
                 st[(size_t)(ch - L) * stride] = (unsigned char)x;
-                if (a.node_out) a.node_out[(size_t)(ch - L) * a.chunk + i] = x;
+                if (a.node_out) a.node_out[out(ch - L, I)] = x;
             }
         }
     }
 }
 
-// Per-set mode (hb2_batch_site_simulate): one thread per column (set, replicate) of the chunk, column = set * reps +
-// replicate, consecutive threads on consecutive replicates of one set.  The set is the "class" of the table and t0 + set
-// the fourth counter word; there is no class draw.  Outputs are column-major: leaf_out [n][L], node_out [n][I].
-__global__ void __launch_bounds__(128) batch_simulate_kernel(SimArgs a) {
-    extern __shared__ unsigned char sim_smem[];
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= a.n) return;
-    const long long col = a.col0 + i, set = col / a.reps;
-    const unsigned long long g = a.g0 + (unsigned long long)(col - set * a.reps);
-    const unsigned t = a.t0 + (unsigned)set;
-    const int L = a.L, I = a.I;
-    unsigned char *st = a.states ? a.states + i : sim_smem + threadIdx.x;
-    const size_t stride = a.states ? (size_t)a.chunk : (size_t)blockDim.x;
-    int s = sim_draw(a.root_cdf, a.D, a.root_last, sim_uniform(g, (unsigned)(L + I - 1), a.key, t));
-    if (a.node_out) a.node_out[(size_t)i * I + I - 1] = s;
-    const size_t set_rows = (size_t)set * a.B;
-    for (int n = I - 1; n >= 0; n--) {
-        if (n < I - 1) s = st[(size_t)n * stride];
-        const int c_end = a.tree.child_start[n + 1];
-        for (int ci = a.tree.child_start[n]; ci < c_end; ci++) {
-            const int ch = a.tree.child_ids[ci];
-            const size_t r = (set_rows + ch) * a.D + s;
-            const int x = sim_draw(a.cdf + r * a.Dp, a.D, a.last + r, sim_uniform(g, (unsigned)ch, a.key, t));
-            if (ch < L) {
-                a.leaf_out[(size_t)i * L + ch] = x;
-            } else {
-                st[(size_t)(ch - L) * stride] = (unsigned char)x;
-                if (a.node_out) a.node_out[(size_t)i * I + ch - L] = x;
-            }
-        }
-    }
-}
+__global__ void __launch_bounds__(128) simulate_kernel(SimArgs a) { sim_walk<false>(a); }
+__global__ void __launch_bounds__(128) batch_simulate_kernel(SimArgs a) { sim_walk<true>(a); }
 
 // ------------------------------------------------------------------------------------------------
 // Peer exchange over NVLink (one process per GPU; every rank maps every other rank's exchange buffer through CUDA IPC).

@@ -264,13 +264,8 @@ class Partition:
     def batch_site_likelihoods(self, pattern_of, formula_values, root_freqs, branch_group=None, template=0):
         """formula_values: [nSets, B, nF]; returns the nSets log-likelihoods."""
         po, ppo = _i(pattern_of)
-        v, pv = _d(formula_values)
-        assert v.ndim == 3 and v.shape[0] == len(po) and v.shape[1] == self.B
+        _, _, pv, _, pbg, keep = self._batch_rows(len(po), formula_values, None, None, branch_group)
         pi, ppi = _d(root_freqs)
-        pbg = None
-        if branch_group is not None:
-            bg, pbg = _i(branch_group)
-            assert bg.shape == (self.B,)
         out = np.empty(len(po))
         _check(self._lib.hb2_batch_site_likelihoods(self._h, int(template), len(po), ppo, pv, pbg, ppi, out.ctypes.data_as(_dp)))
         return out

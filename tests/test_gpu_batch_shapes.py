@@ -321,6 +321,27 @@ def test_group_layouts():
         lf.close()
 
 
+def test_workspace_resize():
+    """Calls on one partition whose chunks need more groups per set than the last call's (no hint, then 8 groups) re-size
+    the batch workspace; each result, and a simulation after them, is bit-identical to the call on a fresh partition."""
+    for mix in (False, True):
+        case = group_case(mix)
+        lay = layouts(case)
+        calls = [(what, name) for name in ("none", "eight", "none", "tested") for what in ("patterns", "columns")]
+        lf = new_lf(case)
+        got = [run(lf, case, what, bg=lay[name]) for what, name in calls]
+        sim = simulate(lf, case, 3, seed=11)
+        lf.close()
+        for (what, name), g in zip(calls, got):
+            fresh = new_lf(case)
+            assert np.array_equal(g, run(fresh, case, what, bg=lay[name])), (mix, what, name)
+            fresh.close()
+        fresh = new_lf(case)
+        ref = simulate(fresh, case, 3, seed=11)
+        fresh.close()
+        assert np.array_equal(sim[0], ref[0]) and np.array_equal(sim[1], ref[1]), mix
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # 4. column identities
 # ---------------------------------------------------------------------------------------------------------------------
