@@ -234,6 +234,8 @@ struct Slot {
 struct BatchShape {
     std::vector<int> row_off;                 // branch b of a set owns component rows row_off[b] .. row_off[b+1]-1
     int64_t R = 0, nF = 0, gk = 0, sets = 0;  // rows per set, formula values per row, groups per set; sets per chunk
+    int64_t mat = 4096, vec = 64;             // doubles per P matrix (Dp^2) and per node vector (Dp)
+    int64_t ent = 0, in = 0;                  // rows per set through launch_expm (R; 0 for site rates) and input doubles per set
 };
 
 }  // namespace
@@ -284,13 +286,13 @@ struct hb2_partition {
         }
     };
     ExBuf ex;                                 // the partition's own hand-overs
-    // Workspace of the batch entry points (hb2_batch_*) for one chunk of `sets` sets: the chunk's expm entries are its
-    // sets' component rows in [set][row] order, and entry e goes to slot e of the chunk's P area.  The batch calls stage
-    // their own root vector, so the staged d_pi stays the evaluations'.
+    // Workspace of the batch entry points (hb2_batch_*) for one chunk of `sets` sets: the chunk's P area holds its sets'
+    // R rows in [set][row] order; the rows that go through launch_expm are its entries, entry e going to slot e.  The batch
+    // calls stage their own root vector, so the staged d_pi stays the evaluations'.
     struct BatchWorkspace {
         ExBuf ex;                             // shared-powers groups of the chunk: [set][groups per set]
-        DeviceBuffer<double> PT, V, mixw;     // P area [entries][4096], formula values [entries][nF], weights [sets][rows]
-        DeviceBuffer<double> cond, out, pi;   // node vectors [sets][I][64], log-likelihoods [sets], root vector [64]
+        DeviceBuffer<double> PT, V, mixw;     // P area [sets][R][Dp^2], inputs [sets][in] (formula values or rates), weights [sets][rows]
+        DeviceBuffer<double> cond, out, pi;   // node vectors [sets][I][Dp], log-likelihoods [sets], root vector [64]
         DeviceBuffer<int> slot, pat, node_ex; // identity slots [entries], patterns [sets], node exponents [sets][I]
         DeviceBuffer<int> row, col;           // first component row of each branch [B+1], caller columns [L][sets]
         PinnedBuffer<int> h_slot, h_pat, h_col;   // staging of slot, pat and col
@@ -298,13 +300,14 @@ struct hb2_partition {
         // after releasing it, so that memory stays at one call's chunk footprint (~8 GB) instead of adding up the largest
         // buffers of different calls' shapes.
         int fit(const BatchShape &sh, int64_t L, int64_t I, cudaStream_t stream) {
-            const int64_t sets = sh.sets, ne = sets * sh.R;
-            if (sets <= (int64_t)out.size() && ne <= (int64_t)slot.size() && sets * sh.gk <= ex.G && ne * sh.nF <= (int64_t)V.size())
+            const int64_t sets = sh.sets, nr = sets * sh.R, ne = sets * sh.ent;
+            if (sets <= (int64_t)out.size() && ne <= (int64_t)slot.size() && sets * sh.gk <= ex.G && sets * sh.in <= (int64_t)V.size() &&
+                nr * sh.mat <= (int64_t)PT.size() && sets * I * sh.vec <= (int64_t)cond.size() && sets * L <= (int64_t)col.size())
                 return 0;
             CU(cudaStreamSynchronize(stream));
             *this = BatchWorkspace();
-            if (ex.alloc((int)(sets * sh.gk), ne, stream) || PT.alloc((size_t)ne * 4096) || V.alloc((size_t)ne * sh.nF) ||
-                mixw.alloc(ne) || cond.alloc((size_t)sets * I * 64) || out.alloc(sets) || slot.alloc(ne) || pat.alloc(sets) ||
+            if (ex.alloc((int)(sets * sh.gk), ne, stream) || PT.alloc((size_t)nr * sh.mat) || V.alloc((size_t)sets * sh.in) ||
+                mixw.alloc(ne) || cond.alloc((size_t)sets * I * sh.vec) || out.alloc(sets) || slot.alloc(ne) || pat.alloc(sets) ||
                 node_ex.alloc((size_t)sets * I) || row.alloc(sh.row_off.size()) || col.alloc((size_t)sets * L) || pi.alloc(64) ||
                 h_slot.alloc(ne) || h_pat.alloc(sets) || h_col.alloc((size_t)sets * L)) {
                 *this = BatchWorkspace();     // fits nothing: the next call sizes it again
@@ -1479,6 +1482,7 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
         CU(cudaMemcpyAsync(p->d_child_ids, ci.data(), ci.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     }
     if (Dp == 32) CU(cudaFuncSetAttribute(hb2::expm_small_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hb2::expm_small_smem_bytes(32)));
+    if (Dp == 32) CU(cudaFuncSetAttribute(hb2::expm_rates_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hb2::expm_rates_smem_bytes(32)));
     if (Dp == 64) {
         { const char *env = getenv("HB2_EXPM_SHARED"); p->ex_enabled = !(env && env[0] == '0'); }
         if (p->ex.alloc(std::max((int)C + 8, HB2_MAX_TEMPLATES * (int)C), (int64_t)(C + 8) * p->B, st)) return 1;
@@ -1674,7 +1678,9 @@ int hb2_evaluate_classes(hb2_partition *p, const double *weights, int64_t nUpdat
 // weights == nullptr: one matrix per branch, row b = branch b (FEL's site model).  Otherwise branch b owns branchK[b]
 // (NULL: K) consecutive component rows and its transition matrix is the weighted sum of their exponentials, formed inside
 // prune_batch_kernel<true> or sim_cdf_kernel<true> (MEME's site model).
-enum class BatchEntry { Sites, MixtureSites, Columns, Simulate };
+// Rates: set s is pattern patternOf[s] under the resident rate matrices of class `cat`, each multiplied by rates[s]
+// (LEISR's site model); its P matrices come from expm_rates_kernel and its likelihood from prune_rates_kernel.
+enum class BatchEntry { Sites, MixtureSites, Columns, Simulate, Rates };
 struct BatchCall {
     BatchEntry entry;
     int64_t templateId, nSets, K;
@@ -1685,7 +1691,13 @@ struct BatchCall {
     int64_t nReps = 0, firstSet = 0, firstRep = 0;
     uint64_t seed = 0;
     int64_t *leafStates = nullptr, *nodeStates = nullptr;
+    int64_t cat = 0;
+    const double *rates = nullptr;
 };
+
+// Sets per chunk of hb2_batch_site_rates, whatever the memory rule allows: at 4 states and 256 taxa a chunk of this many
+// sets holds 4.2 GB of P matrices, and its pruning launch fills every SM.
+constexpr int64_t RATES_MAX_SETS = 65536;
 
 // Every refusal of the batch entry points, before anything is launched or written.
 static int check_batch(const hb2_partition *p, const BatchCall &c) {
@@ -1761,7 +1773,86 @@ static BatchShape batch_shape(const hb2_partition *p, const BatchCall &c) {
                                                 // the power tables of its groups and its node vectors
         per_set = (double)sh.R * (4096 + (double)sh.nF + 1) * 8 + (double)sh.gk * hb2::EXPM_POW_TERMS * 4096 * 8 + (double)p->I * 64 * 8;
     sh.sets = std::min<int64_t>({c.nSets, std::max<int64_t>(1, (int64_t)(8.0e9 / (per_set + sim_bytes))), 1024});
+    sh.ent = sh.R;
+    sh.in = sh.R * sh.nF;
     return sh;
+}
+
+// Refusals of hb2_batch_site_rates, before anything is launched or written.  A branch's rate matrix is resident when its
+// last hand-over, pending or flushed, was a rate matrix (dense or compiled): that is what d_Qres holds for it.
+static int check_rates(const hb2_partition *p, const BatchCall &c) {
+    if (!p) return fail("hb2_batch_site_rates: null partition");
+    if (!c.patternOf || !c.rates || !c.rootFreqs || !c.siteLnL) return fail("hb2_batch_site_rates: null argument");
+    if (c.nSets < 0) return fail("hb2_batch_site_rates: nSets=%lld is negative", (long long)c.nSets);
+    if (c.cat < 0 || c.cat >= p->C) return fail("hb2_batch_site_rates: rate class %lld out of range (C=%lld)", (long long)c.cat, (long long)p->C);
+    if (p->cg_G > 1) return fail("hb2_batch_site_rates is not available with class groups (shard the SETS across ranks instead)");
+    if (p->Dp > 32)
+        return fail("hb2_batch_site_rates supports 2..32-state partitions: for 33..64 states use hb2_batch_site_likelihoods with "
+                    "formula values multiplied by the rate");
+    for (int64_t s = 0; s < c.nSets; s++)
+        if (c.patternOf[s] < 0 || c.patternOf[s] >= p->S)
+            return fail("hb2_batch_site_rates: set %lld: patternOf=%lld out of range (0..%lld)", (long long)s, (long long)c.patternOf[s], (long long)p->S - 1);
+    for (int64_t s = 0; s < c.nSets; s++)
+        if (!(c.rates[s] >= 0.0) || std::isinf(c.rates[s]))
+            return fail("hb2_batch_site_rates: set %lld: rate %g is not a finite number >= 0", (long long)s, c.rates[s]);
+    for (int64_t b = 0; b < p->B; b++) {
+        const Slot &s = p->slots[c.cat * p->B + b];
+        const HandoverQueue *q = s.entry < 0 ? nullptr : s.queue == DENSE_QUEUE ? &p->dense : &p->tmpls[s.queue].queue;
+        if (q ? q->kind[s.entry] == Kind::Trans : s.res != Resident::DenseQ)
+            return fail("hb2_batch_site_rates: rate class %lld, branch %lld has no resident rate matrix (its last hand-over was a "
+                        "transition matrix or a mixture, or it has none)", (long long)c.cat, (long long)b);
+    }
+    return 0;
+}
+
+// hb2_batch_site_rates: one P matrix per branch and set, read from d_Qres and scaled on the device (no input but the rate),
+// and the ~8 GB chunk rule of batch_shape with Dp-sized matrices and node vectors.
+static BatchShape rates_shape(const hb2_partition *p, const BatchCall &c) {
+    BatchShape sh;
+    sh.R = p->B;
+    sh.mat = (int64_t)p->Dp * p->Dp;
+    sh.vec = p->Dp;
+    sh.in = 1;
+    // P matrices, node vectors and exponents, rate, pattern and result
+    const double per_set = (double)p->B * sh.mat * 8 + (double)p->I * (sh.vec * 8 + 4) + 20;
+    sh.sets = std::min<int64_t>({c.nSets, std::max<int64_t>(1, (int64_t)(8.0e9 / per_set)), RATES_MAX_SETS});
+    return sh;
+}
+
+extern "C++" template <int DP>
+void launch_rates(hb2_partition *p, const BatchCall &c, int64_t nb) {
+    hb2_partition::BatchWorkspace &ws = p->batch;
+    hb2::ExpmRatesArgs ea;
+    ea.Q = p->d_Qres + (size_t)c.cat * p->B * p->D * p->D; ea.rate = ws.V; ea.PT = ws.PT;
+    ea.D = (int)p->D; ea.B = (int)p->B; ea.n = (long long)nb * p->B;
+    constexpr int M = 128 / hb2::expm_rates_team(DP);
+    hb2::expm_rates_kernel<DP><<<(unsigned)((ea.n + M - 1) / M), 128, hb2::expm_rates_smem_bytes(DP), p->stream>>>(ea);
+    hb2::BatchPruneArgs ba{};
+    ba.PT = ws.PT; ba.cond = ws.cond; ba.node_ex = ws.node_ex; ba.pat = ws.pat; ba.ambig = p->d_ambig; ba.pi = ws.pi;
+    ba.leaf = p->d_leaf; ba.tree.child_start = p->d_child_start; ba.tree.child_ids = p->d_child_ids; ba.out = ws.out;
+    ba.L = (int)p->L; ba.I = (int)p->I; ba.B = (int)p->B; ba.D = (int)p->D; ba.Sp = (int)p->Sp;
+    constexpr int per_block = 128 / (DP <= 16 ? DP : 32);
+    hb2::prune_rates_kernel<DP><<<(unsigned)((nb + per_block - 1) / per_block), 128, 0, p->stream>>>(ba, (int)nb);
+}
+
+// Sets s0 .. s0+nb-1 of hb2_batch_site_rates: their rates and patterns up, their matrices and likelihoods, the results down.
+static int rates_chunk(hb2_partition *p, const BatchCall &c, int64_t s0, int64_t nb) {
+    hb2_partition::BatchWorkspace &ws = p->batch;
+    for (int64_t s = 0; s < nb; s++) ws.h_pat[s] = (int)c.patternOf[s0 + s];
+    CU(cudaMemcpyAsync(ws.pat, ws.h_pat, (size_t)nb * sizeof(int), cudaMemcpyHostToDevice, p->stream));
+    CU(cudaMemcpyAsync(ws.V, c.rates + s0, (size_t)nb * sizeof(double), cudaMemcpyHostToDevice, p->stream));
+    switch (p->Dp) {
+        case 4: launch_rates<4>(p, c, nb); break;
+        case 8: launch_rates<8>(p, c, nb); break;
+        case 16: launch_rates<16>(p, c, nb); break;
+        case 24: launch_rates<24>(p, c, nb); break;
+        case 32: launch_rates<32>(p, c, nb); break;
+        default: return fail("hb2_batch_site_rates: unsupported padded state count %d", p->Dp);
+    }
+    p->launches += 2;
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(c.siteLnL + s0, ws.out, (size_t)nb * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
+    return 0;
 }
 
 // Uploads the formula values (and weights) of sets s0 .. s0+nb-1, plans their shared-powers groups and exponentiates them
@@ -1845,20 +1936,24 @@ static int simulate_chunk(hb2_partition *p, const BatchCall &c, const BatchShape
 
 // Body of every batch entry point: per chunk of sets, the batched exponential, then the call's consumer.
 static int batch_sites(hb2_partition *p, const BatchCall &c) {
-    if (check_batch(p, c)) return 1;
-    const bool sim = c.entry == BatchEntry::Simulate;
+    const bool sim = c.entry == BatchEntry::Simulate, rates = c.entry == BatchEntry::Rates;
+    if (rates ? check_rates(p, c) : check_batch(p, c)) return 1;
     if (c.nSets == 0 || (sim && c.nReps == 0)) return 0;
     CU(cudaSetDevice(p->device));
-    const BatchShape sh = batch_shape(p, c);
-    if (p->batch.fit(sh, p->L, p->I, p->stream)) return 1;
+    if (rates && flush_matrices(p)) return 1;          // d_Qres holds every matrix handed over so far
+    const BatchShape sh = rates ? rates_shape(p, c) : batch_shape(p, c);
+    if (p->batch.fit(sh, rates ? 0 : p->L, p->I, p->stream)) return 1;     // site rates score patterns only: no column area
     CU(cudaStreamSynchronize(p->stream));
     if (stage_root(p, c.rootFreqs, nullptr, 0, p->batch.pi)) return 1;
     if (c.weights) CU(cudaMemcpyAsync(p->batch.row, sh.row_off.data(), sh.row_off.size() * sizeof(int), cudaMemcpyHostToDevice, p->stream));
     for (int64_t s0 = 0; s0 < c.nSets; s0 += sh.sets) {
         const int64_t nb = std::min(sh.sets, c.nSets - s0);
         CU(cudaStreamSynchronize(p->stream));          // previous chunk done: buffers and pinned arrays are free again
-        if (exponentiate_chunk(p, c, sh, s0, nb) || (sim ? simulate_chunk(p, c, sh, s0, nb) : score_chunk(p, c, sh, s0, nb)))
+        if (rates) {
+            if (rates_chunk(p, c, s0, nb)) return 1;
+        } else if (exponentiate_chunk(p, c, sh, s0, nb) || (sim ? simulate_chunk(p, c, sh, s0, nb) : score_chunk(p, c, sh, s0, nb))) {
             return 1;
+        }
     }
     int err = 0;
     CU(cudaMemcpyAsync(&err, p->d_err, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
@@ -1893,6 +1988,14 @@ int hb2_batch_site_simulate(hb2_partition *p, int64_t templateId, int64_t nSets,
                             int64_t *leafStates, int64_t *nodeStates) {
     return batch_sites(p, {BatchEntry::Simulate, templateId, nSets, K, branchK, branchGroup, formulaValues, weights, rootFreqs,
                            nullptr, nullptr, nullptr, nReps, firstSet, firstRep, seed, leafStates, nodeStates});
+}
+
+int hb2_batch_site_rates(hb2_partition *p, int64_t cat, int64_t nSets, const int64_t *patternOf, const double *rates,
+                         const double *rootFreqs, double *siteLnL) {
+    BatchCall c{BatchEntry::Rates, 0, nSets, 1, nullptr, nullptr, nullptr, nullptr, rootFreqs, patternOf, nullptr, siteLnL};
+    c.cat = cat < 0 ? 0 : cat;
+    c.rates = rates;
+    return batch_sites(p, c);
 }
 
 int hb2_read_conditionals(hb2_partition *p, int64_t cat, int64_t inode, double *cond, int32_t *exp2) {

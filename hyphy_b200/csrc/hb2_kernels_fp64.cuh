@@ -814,6 +814,59 @@ __global__ void __launch_bounds__(256, 3) expm_poly_kernel(ExpmArgs a, ExpmTcOut
 
 // Small state spaces (Dp <= 32): one CTA of 128 threads per matrix, plain shared-memory products.
 constexpr size_t expm_small_smem_bytes(int DP) { return (size_t)6 * DP * (DP + 1) * sizeof(double); }
+
+// The per-entry rules of the small-state exponential, shared by expm_small_kernel (one matrix per CTA) and
+// expm_rates_kernel (several per CTA).  Matrices sit in shared memory transposed, leading dimension LD: A1[j*LD + i] = A[i][j].
+// Row-sum norm of row i of A (column i of A1), in column order.
+template <int DP, int LD>
+__device__ __forceinline__ double expm_small_norm(const double *A1, int i) {
+    double s = 0.0;
+    for (int j = 0; j < DP; j++) s += fabs(A1[j * LD + i]);
+    return s;
+}
+
+// Scaling shift from the DP row norms: the binary exponent of the largest, at least 0; -1 when one is NaN or infinite.
+template <int DP>
+__device__ __forceinline__ int expm_small_shift(const double *red) {
+    double m = 0.0; bool bad = false;
+    for (int i = 0; i < DP; i++) { if (!(red[i] == red[i]) || isinf(red[i])) bad = true; m = fmax(m, red[i]); }
+    int e = 0;
+    if (m > 0.0) frexp(m, &e);
+    return bad ? -1 : max(e, 0);
+}
+
+// Entry (r, c) of X*Y, fma over k in order.
+template <int DP, int LD>
+__device__ __forceinline__ double expm_small_dot(const double *X, const double *Y, int r, int c) {
+    double s = 0.0;
+#pragma unroll
+    for (int k = 0; k < DP; k++) s = fma(X[r * LD + k], Y[k * LD + c], s);
+    return s;
+}
+
+// Entry (r, c) of the q-th Horner block c_{4q} I + c_{4q+1} A + c_{4q+2} A^2 + c_{4q+3} A^3.
+template <int LD>
+__device__ __forceinline__ double expm_small_poly(const double *A1, const double *A2, const double *A3, int q, int r, int c) {
+    int o = r * LD + c;
+    double v = taylor_c(4 * q + 1) * A1[o] + taylor_c(4 * q + 2) * A2[o] + taylor_c(4 * q + 3) * A3[o];
+    if (r == c) v += taylor_c(4 * q);
+    return v;
+}
+
+// Padding and negative entries of the result go to 0.
+__device__ __forceinline__ double expm_small_clamp(double v, int j, int k, int D) {
+    if (j >= D || k >= D) v = 0.0; else if (v < 0.0) v = 0.0;
+    return v;
+}
+
+// Diagonal repair of column c of the clamped result R (a row of P): 1 minus its other entries, at least 0.
+template <int DP, int LD>
+__device__ __forceinline__ double expm_small_diag(const double *R, int c) {
+    double s = 0.0;
+    for (int j = 0; j < DP; j++) if (j != c) s += R[j * LD + c];
+    return fmax(1.0 - s, 0.0);
+}
+
 template <int DP>
 __global__ void __launch_bounds__(128) expm_small_kernel(ExpmArgs a) {
     constexpr int LD = DP + 1;
@@ -829,19 +882,9 @@ __global__ void __launch_bounds__(128) expm_small_kernel(ExpmArgs a) {
         for (int idx = tid; idx < DP * DP; idx += 128) out[idx] = A1[(idx / DP) * LD + idx % DP];
         return;
     }
-    if (tid < DP) {
-        double s = 0.0;
-        for (int j = 0; j < DP; j++) s += fabs(A1[j * LD + tid]);
-        red[tid] = s;
-    }
+    if (tid < DP) red[tid] = expm_small_norm<DP, LD>(A1, tid);
     __syncthreads();
-    if (tid == 0) {
-        double m = 0.0; bool bad = false;
-        for (int i = 0; i < DP; i++) { if (!(red[i] == red[i]) || isinf(red[i])) bad = true; m = fmax(m, red[i]); }
-        int e = 0;
-        if (m > 0.0) frexp(m, &e);
-        s_shift = bad ? -1 : max(e, 0);
-    }
+    if (tid == 0) s_shift = expm_small_shift<DP>(red);
     __syncthreads();
     const int shift = s_shift;
     if (shift < 0 || shift > 900) {
@@ -856,25 +899,16 @@ __global__ void __launch_bounds__(128) expm_small_kernel(ExpmArgs a) {
     auto mm = [&](double *Cm, const double *X, const double *Y) {      // Cm = X*Y (Cm distinct from X,Y)
         for (int idx = tid; idx < DP * DP; idx += 128) {
             int r = idx / DP, c = idx % DP;
-            double s = 0.0;
-#pragma unroll
-            for (int k = 0; k < DP; k++) s = fma(X[r * LD + k], Y[k * LD + c], s);
-            Cm[r * LD + c] = s;
+            Cm[r * LD + c] = expm_small_dot<DP, LD>(X, Y, r, c);
         }
         __syncthreads();
     };
     mm(A2, A1, A1); mm(A3, A2, A1); mm(A4, A2, A2);
-    auto poly = [&](int q, int r, int c) -> double {
-        int o = r * LD + c;
-        double v = taylor_c(4 * q + 1) * A1[o] + taylor_c(4 * q + 2) * A2[o] + taylor_c(4 * q + 3) * A3[o];
-        if (r == c) v += taylor_c(4 * q);
-        return v;
-    };
-    for (int idx = tid; idx < DP * DP; idx += 128) R[(idx / DP) * LD + idx % DP] = poly(3, idx / DP, idx % DP);
+    for (int idx = tid; idx < DP * DP; idx += 128) R[(idx / DP) * LD + idx % DP] = expm_small_poly<LD>(A1, A2, A3, 3, idx / DP, idx % DP);
     __syncthreads();
     for (int q = 2; q >= 0; q--) {
         mm(T, R, A4);
-        for (int idx = tid; idx < DP * DP; idx += 128) { int r = idx / DP, c = idx % DP; R[r * LD + c] = T[r * LD + c] + poly(q, r, c); }
+        for (int idx = tid; idx < DP * DP; idx += 128) { int r = idx / DP, c = idx % DP; R[r * LD + c] = T[r * LD + c] + expm_small_poly<LD>(A1, A2, A3, q, r, c); }
         __syncthreads();
     }
     for (int s = 0; s < shift; s++) {
@@ -884,18 +918,107 @@ __global__ void __launch_bounds__(128) expm_small_kernel(ExpmArgs a) {
     }
     for (int idx = tid; idx < DP * DP; idx += 128) {
         int j = idx / DP, k = idx % DP;
-        double v = R[j * LD + k];
-        if (j >= D || k >= D) v = 0.0; else if (v < 0.0) v = 0.0;
-        R[j * LD + k] = v;
+        R[j * LD + k] = expm_small_clamp(R[j * LD + k], j, k, D);
     }
     __syncthreads();
-    if (tid < DP) {
-        double s = 0.0;
-        for (int j = 0; j < DP; j++) if (j != tid) s += R[j * LD + tid];
-        if (tid < D) R[tid * LD + tid] = fmax(1.0 - s, 0.0);
-    }
+    if (tid < D) R[tid * LD + tid] = expm_small_diag<DP, LD>(R, tid);
     __syncthreads();
     for (int idx = tid; idx < DP * DP; idx += 128) out[idx] = R[(idx / DP) * LD + idx % DP];
+}
+
+// ------------------------------------------------------------------------------------------------
+// expm_rates_kernel (hb2_batch_site_rates): P = exp(r_s A_b) for every (set s, branch b) of a chunk, A_b the resident rate
+// matrix of the call's class (d_Qres, row-major D*D), scaled by the set's rate while it is loaded.  A team of
+// expm_rates_team(DP) threads owns one matrix and runs expm_small_kernel's steps entry for entry (same shift, Horner
+// order, fma order, clamping and diagonal repair), so that rate 1 gives the resident path's matrices; 4 and 8
+// states pack 8 and 2 matrices into a CTA, one thread per entry.  Output: PT[s][b][DP*DP], transposed like every P.
+// ------------------------------------------------------------------------------------------------
+struct ExpmRatesArgs {
+    const double *Q;          // [B][D*D] resident rate matrices of the class
+    const double *rate;       // [sets]
+    double *PT;               // [sets][B][DP*DP]
+    int D, B;
+    long long n;              // sets * B matrices
+};
+
+__host__ __device__ constexpr int expm_rates_team(int DP) { return DP * DP < 128 ? DP * DP : 128; }
+constexpr size_t expm_rates_smem_bytes(int DP) { return (size_t)(128 / expm_rates_team(DP)) * expm_small_smem_bytes(DP); }
+
+// Barrier of one team: the CTA, a pair of warps (named barrier 1 + team), or a half-warp.
+template <int T>
+__device__ __forceinline__ void team_sync(int team) {
+    if constexpr (T == 128) __syncthreads();
+    else if constexpr (T == 64) {
+        if (team == 0) asm volatile("bar.sync 1, 64;" ::: "memory");
+        else asm volatile("bar.sync 2, 64;" ::: "memory");
+    }
+    else {
+        static_assert(T == 16, "teams of 16, 64 or 128 threads");
+        __syncwarp(0xffffu << (threadIdx.x & 16));
+    }
+}
+
+template <int DP>
+__global__ void __launch_bounds__(128) expm_rates_kernel(ExpmRatesArgs a) {
+    constexpr int LD = DP + 1, T = expm_rates_team(DP), M = 128 / T, MS = DP * LD;
+    extern __shared__ __align__(16) double sm[];          // M teams x 6 matrices of DP*LD doubles (expm_rates_smem_bytes)
+    __shared__ double red_all[M][DP];
+    __shared__ int shift_all[M];
+    const int team = threadIdx.x / T, lt = threadIdx.x % T, D = a.D;
+    const long long e = (long long)blockIdx.x * M + team;
+    if (e >= a.n) return;
+    double *A1 = sm + (size_t)team * 6 * MS, *A2 = A1 + MS, *A3 = A2 + MS, *A4 = A3 + MS, *R = A4 + MS, *Tm = R + MS;
+    double *red = red_all[team];
+    const double r = a.rate[e / a.B];
+    const double *Q = a.Q + (size_t)(e % a.B) * D * D;
+    double *out = a.PT + (size_t)e * DP * DP;
+    for (int idx = lt; idx < DP * DP; idx += T) {
+        const int i = idx / DP, j = idx - i * DP;
+        A1[j * LD + i] = (i < D && j < D) ? r * Q[(size_t)i * D + j] : 0.0;
+    }
+    team_sync<T>(team);
+    if (lt < DP) red[lt] = expm_small_norm<DP, LD>(A1, lt);
+    team_sync<T>(team);
+    if (lt == 0) shift_all[team] = expm_small_shift<DP>(red);
+    team_sync<T>(team);
+    const int shift = shift_all[team];
+    if (shift < 0 || shift > 900) {
+        for (int idx = lt; idx < DP * DP; idx += T) out[idx] = __longlong_as_double(0x7ff8000000000000LL);
+        return;
+    }
+    if (shift > 0) {
+        const double sc = exp2i(-shift);
+        for (int idx = lt; idx < DP * DP; idx += T) A1[(idx / DP) * LD + idx % DP] *= sc;
+        team_sync<T>(team);
+    }
+    auto mm = [&](double *Cm, const double *X, const double *Y) {
+        for (int idx = lt; idx < DP * DP; idx += T) {
+            int rr = idx / DP, c = idx % DP;
+            Cm[rr * LD + c] = expm_small_dot<DP, LD>(X, Y, rr, c);
+        }
+        team_sync<T>(team);
+    };
+    mm(A2, A1, A1); mm(A3, A2, A1); mm(A4, A2, A2);
+    for (int idx = lt; idx < DP * DP; idx += T) R[(idx / DP) * LD + idx % DP] = expm_small_poly<LD>(A1, A2, A3, 3, idx / DP, idx % DP);
+    team_sync<T>(team);
+    for (int q = 2; q >= 0; q--) {
+        mm(Tm, R, A4);
+        for (int idx = lt; idx < DP * DP; idx += T) { int rr = idx / DP, c = idx % DP; R[rr * LD + c] = Tm[rr * LD + c] + expm_small_poly<LD>(A1, A2, A3, q, rr, c); }
+        team_sync<T>(team);
+    }
+    for (int s = 0; s < shift; s++) {
+        mm(Tm, R, R);
+        for (int idx = lt; idx < DP * DP; idx += T) { int o = (idx / DP) * LD + idx % DP; R[o] = Tm[o]; }
+        team_sync<T>(team);
+    }
+    for (int idx = lt; idx < DP * DP; idx += T) {
+        int j = idx / DP, k = idx % DP;
+        R[j * LD + k] = expm_small_clamp(R[j * LD + k], j, k, D);
+    }
+    team_sync<T>(team);
+    if (lt < D) R[lt * LD + lt] = expm_small_diag<DP, LD>(R, lt);
+    team_sync<T>(team);
+    for (int idx = lt; idx < DP * DP; idx += T) out[idx] = R[(idx / DP) * LD + idx % DP];
 }
 
 
@@ -1572,6 +1695,77 @@ __global__ void __launch_bounds__(64) prune_batch_kernel(BatchPruneArgs a) {
             if (k == 0) a.out[s] = pattern_lnl(red[0] + red[1], ex, [] {});
         }
     }
+}
+
+// ------------------------------------------------------------------------------------------------
+// prune_rates_kernel (hb2_batch_site_rates): prune_batch_kernel<false>'s recursion for 4..32 padded states.  A group of
+// G = 4, 8, 16 or 32 lanes owns one set, lane k = parent state k, and 32/G sets share a warp (24 states take G = 32, so
+// a quarter of their lanes idle).  A child's vector is broadcast with width-G shuffles, the node maximum is a group
+// shuffle-max, and node vectors live in global scratch cond[s][I][DP] (each lane reads back only the entry it wrote).
+// Numerical rules as prune_batch_kernel: power-of-two renormalisation of every node to [0.5, 1), the wide-node rescale
+// below RESCALE_BELOW from the third child on, ambiguity sums over the allowed states in state order, pattern_lnl's
+// -inf / NaN encoding.  The root sum differs in order: one xor tree over the G lanes, where prune_batch_kernel adds the
+// totals of two 32-lane trees.
+// PT [sets][B][DP*DP], ambig [nAmb][DP], pi [DP]; n = sets of the launch.
+// ------------------------------------------------------------------------------------------------
+template <int DP>
+__global__ void __launch_bounds__(128) prune_rates_kernel(BatchPruneArgs a, int n) {
+    constexpr int G = DP <= 16 ? DP : 32;
+    const int lane = threadIdx.x & 31, k = lane % G;
+    const unsigned mask = G == 32 ? 0xffffffffu : ((1u << G) - 1) << (lane / G * G);
+    const int s = (int)((blockIdx.x * 128u + threadIdx.x) / G);
+    if (s >= n) return;                                  // whole groups
+    const bool live = k < DP;
+    const int pattern = a.pat[s];
+    const double *PTs = a.PT + (size_t)s * a.B * DP * DP;
+    double *cs = a.cond + (size_t)s * a.I * DP;
+    int *node_ex = a.node_ex + (size_t)s * a.I;
+    int ex = 0;
+    double v = 0.0;
+    for (int par = 0; par < a.I; par++) {
+        v = k < a.D ? 1.0 : 0.0;
+        ex = 0;
+        auto renorm = [&](double below) {
+            double mx = v;
+#pragma unroll
+            for (int o = G / 2; o > 0; o >>= 1) mx = fmax(mx, __shfl_xor_sync(mask, mx, o, G));
+            if (mx > 0.0 && mx < below) {
+                const int e = ilogb(mx) + 1;
+                v = v * exp2i(-(e / 2)) * exp2i(-(e - e / 2));
+                ex += e;
+            }
+        };
+        const int c_begin = a.tree.child_start[par], c_end = a.tree.child_start[par + 1];
+        for (int ci = c_begin; ci < c_end; ci++) {
+            if (ci - c_begin >= 2) renorm(RESCALE_BELOW);
+            const int child = a.tree.child_ids[ci];
+            const double *PT = PTs + (size_t)child * DP * DP;
+            auto entry = [&](int j) { return live ? PT[j * DP + k] : 0.0; };
+            double m = 0.0;
+            if (child < a.L) {
+                const int code = a.leaf[(size_t)child * a.Sp + pattern];
+                if (code >= 0) m = entry(code);
+                else {
+                    const double *amb = a.ambig + (size_t)(-code - 1) * DP;
+                    for (int j = 0; j < a.D; j++) { const double w = amb[j]; if (w != 0.0) m = fma(w, entry(j), m); }
+                }
+            } else {
+                const int cin = child - a.L;
+                const double x = live ? cs[(size_t)cin * DP + k] : 0.0;
+                for (int j = 0; j < a.D; j++) m = fma(__shfl_sync(mask, x, j, G), entry(j), m);
+                ex += node_ex[cin];
+            }
+            v *= m;
+        }
+        renorm(INFINITY);
+        if (live) cs[(size_t)par * DP + k] = v;
+        if (k == 0) node_ex[par] = ex;
+        __syncwarp(mask);                                // node_ex visible to the group before a parent reads it
+    }
+    double r = live ? v * a.pi[k] : 0.0;
+#pragma unroll
+    for (int o = G / 2; o > 0; o >>= 1) r += __shfl_xor_sync(mask, r, o, G);
+    if (k == 0) a.out[s] = pattern_lnl(r, ex, [] {});
 }
 
 // ------------------------------------------------------------------------------------------------

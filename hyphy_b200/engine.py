@@ -45,6 +45,7 @@ ABI = [
     ("hb2_batch_site_likelihoods", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, _dp, _ip, _dp, _dp]),
     ("hb2_batch_site_mixture_likelihoods", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, C.c_int64, _ip, _dp, _dp, _ip, _dp, _dp]),
     ("hb2_batch_column_likelihoods", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, C.c_int64, _ip, _dp, _dp, _ip, _dp, _dp]),
+    ("hb2_batch_site_rates", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, _dp, _dp, _dp]),
     ("hb2_read_conditionals", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _dp, _i32p]),
     ("hb2_read_transition", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _dp]),
     ("hb2_simulate", C.c_int, [C.c_void_p, _dp, _dp, C.c_int64, C.c_uint64, C.c_int64, _ip, _ip, _i32p]),
@@ -339,6 +340,18 @@ class Partition:
                                                  int(seed) & 0xFFFFFFFFFFFFFFFF, int(first_set), int(first_rep),
                                                  leaf.ctypes.data_as(_ip), nodes.ctypes.data_as(_ip) if want_nodes else None))
         return leaf, nodes
+
+    def batch_site_rates(self, pattern_of, rates, root_freqs, cat=0):
+        """LEISR's site model (hb2_batch_site_rates): set s is pattern pattern_of[s] under class `cat` of the current model
+        with every branch's rate matrix multiplied by rates[s].  Returns the nSets log-likelihoods."""
+        po, ppo = _i(pattern_of)
+        r, pr = _d(rates)
+        assert po.ndim == 1 and r.shape == po.shape
+        pi, ppi = _d(root_freqs)
+        assert pi.shape == (self.D,)
+        out = np.empty(len(po))
+        _check(self._lib.hb2_batch_site_rates(self._h, int(cat), len(po), ppo, pr, ppi, out.ctypes.data_as(_dp)))
+        return out
 
     # -- read-backs --------------------------------------------------------------------------------
     def read_conditionals(self, cat, inode):

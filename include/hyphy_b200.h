@@ -183,6 +183,27 @@ int hb2_batch_column_likelihoods(hb2_partition *p, int64_t templateId, int64_t n
                                  int64_t K, const int64_t *branchK, const double *formulaValues, const double *weights,
                                  const int64_t *branchGroup, const double *rootFreqs, double *siteLnL);
 
+/* Batched one-pattern likelihoods at site-specific relative rates, for nucleotide and protein partitions (2..32 states).
+ * LEISR (res/TemplateBatchFiles/LEISR.bf:209-266, :271-290, :420-444) and ProteinAnalyses/relative_prot_rates.bf
+ * (:160-192, :286) fit the alignment-wide model once, then one one-site likelihood function per pattern whose only free
+ * parameter scales every branch length; a constant site is evaluated at rate 0 (LEISR.bf:411-416).  Set s is the
+ * log-likelihood of pattern patternOf[s] under class `cat` (-1 means 0) of the partition's current model with every
+ * branch's rate matrix multiplied by rates[s]:  P_b(s) = exp(rates[s] * A_b), A_b the rate matrix last handed over for
+ * (cat, b) by hb2_set_matrices* with HB2_MATRIX_RATE or by hb2_set_matrices_compiled* (pending hand-overs are flushed
+ * first, as by hb2_read_transition).  Only patternOf and rates cross to the device.
+ *   rootFreqs  D values, one root vector for every set.
+ *   siteLnL    [nSets], NOT multiplied by the pattern frequency; a pattern of likelihood 0 gives -inf.  fp64 throughout.
+ * rates[s] == 0 gives identity matrices exactly (a constant column: log pi_state; any other: -inf).  A product
+ * rates[s] * ||A_b|| beyond the exponential's range (scaling shift > 900) gives NaN for that set only.
+ * Refusals before anything is launched or written (the partition stays usable): null pointers; nSets < 0; cat out of
+ * range; patternOf out of range or a rate that is negative, NaN or infinite (both name the set); class-group mode;
+ * 33..64 states (use hb2_batch_site_likelihoods with formula values multiplied by the rate: codon rows are linear in
+ * them); a branch of `cat` without a resident rate matrix -- its last hand-over a transition matrix or a mixture, or
+ * none -- named with its class.  Nothing an evaluation reads is touched: conditionals, scalers, walk plans and tags, the
+ * branch cache, the staged root vector, the P cache and the resident rate matrices. */
+int hb2_batch_site_rates(hb2_partition *p, int64_t cat, int64_t nSets, const int64_t *patternOf, const double *rates,
+                         const double *rootFreqs, double *siteLnL);
+
 /* FillInConditionals-style read-back (tree.cpp:3335): conditionals of internal node `inode` (0..I-1), class cat,
  * as S*D doubles (original pattern order) and S binary exponents: true value = cond * 2^exp2. */
 int hb2_read_conditionals(hb2_partition *p, int64_t cat, int64_t inode, double *cond, int32_t *exp2);
