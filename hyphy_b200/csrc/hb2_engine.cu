@@ -236,6 +236,7 @@ struct BatchShape {
     int64_t R = 0, nF = 0, gk = 0, sets = 0;  // rows per set, formula values per row, groups per set; sets per chunk
     int64_t mat = 4096, vec = 64;             // doubles per P matrix (Dp^2) and per node vector (Dp)
     int64_t ent = 0, in = 0;                  // rows per set through launch_expm (R; 0 for site rates) and input doubles per set
+    int64_t side = 0;                         // branches per set with outside scratch (branch rows: B; 0 for every other call)
 };
 
 }  // namespace
@@ -296,20 +297,26 @@ struct hb2_partition {
         DeviceBuffer<int> slot, pat, node_ex; // identity slots [entries], patterns [sets], node exponents [sets][I]
         DeviceBuffer<int> row, col;           // first component row of each branch [B+1], caller columns [L][sets]
         PinnedBuffer<int> h_slot, h_pat, h_col;   // staging of slot, pat and col
+        // hb2_batch_branch_component_likelihoods only (sh.side = B; empty for every other call): messages and outside
+        // vectors [sets][2][B][64], their exponents [sets][2][B], and the row log-likelihoods [sets][R]
+        DeviceBuffer<double> side, rows;
+        DeviceBuffer<int> side_ex;
         // Sizes the workspace for chunks of `sh`.  A chunk that does not fit re-sizes the whole workspace for this call,
         // after releasing it, so that memory stays at one call's chunk footprint (~8 GB) instead of adding up the largest
         // buffers of different calls' shapes.
         int fit(const BatchShape &sh, int64_t L, int64_t I, cudaStream_t stream) {
             const int64_t sets = sh.sets, nr = sets * sh.R, ne = sets * sh.ent;
             if (sets <= (int64_t)out.size() && ne <= (int64_t)slot.size() && sets * sh.gk <= ex.G && sets * sh.in <= (int64_t)V.size() &&
-                nr * sh.mat <= (int64_t)PT.size() && sets * I * sh.vec <= (int64_t)cond.size() && sets * L <= (int64_t)col.size())
+                nr * sh.mat <= (int64_t)PT.size() && sets * I * sh.vec <= (int64_t)cond.size() && sets * L <= (int64_t)col.size() &&
+                sets * sh.side * 128 <= (int64_t)side.size() && (sh.side == 0 || nr <= (int64_t)rows.size()))
                 return 0;
             CU(cudaStreamSynchronize(stream));
             *this = BatchWorkspace();
             if (ex.alloc((int)(sets * sh.gk), ne, stream) || PT.alloc((size_t)nr * sh.mat) || V.alloc((size_t)sets * sh.in) ||
                 mixw.alloc(ne) || cond.alloc((size_t)sets * I * sh.vec) || out.alloc(sets) || slot.alloc(ne) || pat.alloc(sets) ||
                 node_ex.alloc((size_t)sets * I) || row.alloc(sh.row_off.size()) || col.alloc((size_t)sets * L) || pi.alloc(64) ||
-                h_slot.alloc(ne) || h_pat.alloc(sets) || h_col.alloc((size_t)sets * L)) {
+                h_slot.alloc(ne) || h_pat.alloc(sets) || h_col.alloc((size_t)sets * L) ||
+                (sh.side && (side.alloc((size_t)sets * sh.side * 128) || side_ex.alloc((size_t)sets * sh.side * 2) || rows.alloc(nr)))) {
                 *this = BatchWorkspace();     // fits nothing: the next call sizes it again
                 return 1;
             }
@@ -1680,7 +1687,9 @@ int hb2_evaluate_classes(hb2_partition *p, const double *weights, int64_t nUpdat
 // prune_batch_kernel<true> or sim_cdf_kernel<true> (MEME's site model).
 // Rates: set s is pattern patternOf[s] under the resident rate matrices of class `cat`, each multiplied by rates[s]
 // (LEISR's site model); its P matrices come from expm_rates_kernel and its likelihood from prune_rates_kernel.
-enum class BatchEntry { Sites, MixtureSites, Columns, Simulate, Rates };
+// BranchRows: MixtureSites, and after its pruning every component row of every branch pinned alone (rowLnL [nSets][R],
+// branch_rows_kernel; MEME's branch-level empirical Bayes factors).  siteLnL is nullable there.
+enum class BatchEntry { Sites, MixtureSites, Columns, Simulate, Rates, BranchRows };
 struct BatchCall {
     BatchEntry entry;
     int64_t templateId, nSets, K;
@@ -1693,6 +1702,7 @@ struct BatchCall {
     int64_t *leafStates = nullptr, *nodeStates = nullptr;
     int64_t cat = 0;
     const double *rates = nullptr;
+    double *rowLnL = nullptr;
 };
 
 // Sets per chunk of hb2_batch_site_rates, whatever the memory rule allows: at 4 states and 256 taxa a chunk of this many
@@ -1701,13 +1711,18 @@ constexpr int64_t RATES_MAX_SETS = 65536;
 
 // Every refusal of the batch entry points, before anything is launched or written.
 static int check_batch(const hb2_partition *p, const BatchCall &c) {
-    const bool sites = c.entry == BatchEntry::Sites || c.entry == BatchEntry::MixtureSites, sim = c.entry == BatchEntry::Simulate;
+    const bool rows = c.entry == BatchEntry::BranchRows;
+    const bool sites = c.entry == BatchEntry::Sites || c.entry == BatchEntry::MixtureSites || rows, sim = c.entry == BatchEntry::Simulate;
     const char *fn = sim ? "hb2_batch_site_simulate" : "hb2_batch_column_likelihoods";
     if (!p) return fail(c.entry == BatchEntry::Sites ? "null argument" : "null partition");
     if (sites) {
+        if (rows && !c.weights)
+            return fail("hb2_batch_branch_component_likelihoods: weights must not be null (with one row per branch every row "
+                        "would equal siteLnL)");
+        if (rows && !c.rowLnL) return fail("hb2_batch_branch_component_likelihoods: rowLnL must not be null");
         if (c.entry == BatchEntry::MixtureSites && !c.weights) return fail("weights must not be null");
         if (c.entry == BatchEntry::MixtureSites && !c.formulaValues) return fail("formulaValues must not be null");
-        if (!c.formulaValues || !c.rootFreqs || !c.siteLnL || !c.patternOf) return fail("null argument");
+        if (!c.formulaValues || !c.rootFreqs || (!c.siteLnL && !rows) || !c.patternOf) return fail("null argument");
         if (c.nSets < 0) return fail("bad set count");
     } else {
         if (c.nSets < 0) return fail("%s: nSets=%lld is negative", fn, (long long)c.nSets);
@@ -1772,6 +1787,10 @@ static BatchShape batch_shape(const hb2_partition *p, const BatchCall &c) {
     else                                        // a set's R component matrices, formula values and weights,
                                                 // the power tables of its groups and its node vectors
         per_set = (double)sh.R * (4096 + (double)sh.nF + 1) * 8 + (double)sh.gk * hb2::EXPM_POW_TERMS * 4096 * 8 + (double)p->I * 64 * 8;
+    if (c.entry == BatchEntry::BranchRows) {    // messages and outside vectors with their exponents, and the row results
+        sh.side = B;
+        per_set += (double)B * 2 * (64 * 8 + 4) + (double)sh.R * 8;
+    }
     sh.sets = std::min<int64_t>({c.nSets, std::max<int64_t>(1, (int64_t)(8.0e9 / (per_set + sim_bytes))), 1024});
     sh.ent = sh.R;
     sh.in = sh.R * sh.nF;
@@ -1877,7 +1896,8 @@ static int exponentiate_chunk(hb2_partition *p, const BatchCall &c, const BatchS
     return launch_expm(p, {Kind::Compiled, (int)c.templateId}, ws.V, ws.slot, (int)ne, false, sp, 0, ws.PT);
 }
 
-// Likelihoods of sets s0 .. s0+nb-1 from the chunk's P area.
+// Likelihoods of sets s0 .. s0+nb-1 from the chunk's P area.  Branch rows: then branch_rows_kernel on the inside pass's node
+// vectors (so siteLnL stays hb2_batch_site_mixture_likelihoods' bit for bit), and the chunk's rows go down.
 static int score_chunk(hb2_partition *p, const BatchCall &c, const BatchShape &sh, int64_t s0, int64_t nb) {
     hb2_partition::BatchWorkspace &ws = p->batch;
     const int64_t L = p->L;
@@ -1899,7 +1919,15 @@ static int score_chunk(hb2_partition *p, const BatchCall &c, const BatchShape &s
     else hb2::prune_batch_kernel<false><<<(unsigned)nb, 64, 0, p->stream>>>(ba);
     p->launches++;
     CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(c.siteLnL + s0, ws.out, (size_t)nb * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
+    if (c.rowLnL) {
+        const size_t side = (size_t)nb * p->B;
+        hb2::BranchRowsArgs g{ba, ws.side, ws.side + side * 64, ws.side_ex, ws.side_ex + side, ws.rows};
+        hb2::branch_rows_kernel<<<(unsigned)nb, 64, 0, p->stream>>>(g);
+        p->launches++;
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(c.rowLnL + s0 * sh.R, ws.rows, (size_t)nb * sh.R * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
+    }
+    if (c.siteLnL) CU(cudaMemcpyAsync(c.siteLnL + s0, ws.out, (size_t)nb * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
     return 0;
 }
 
@@ -1973,6 +2001,16 @@ int hb2_batch_site_mixture_likelihoods(hb2_partition *p, int64_t templateId, int
                                        const int64_t *branchGroup, const double *rootFreqs, double *siteLnL) {
     return batch_sites(p, {BatchEntry::MixtureSites, templateId, nSets, K, branchK, branchGroup, formulaValues, weights, rootFreqs,
                            patternOf, nullptr, siteLnL});
+}
+
+int hb2_batch_branch_component_likelihoods(hb2_partition *p, int64_t templateId, int64_t nSets, const int64_t *patternOf,
+                                           int64_t K, const int64_t *branchK, const double *formulaValues,
+                                           const double *weights, const int64_t *branchGroup, const double *rootFreqs,
+                                           double *siteLnL, double *rowLnL) {
+    BatchCall c{BatchEntry::BranchRows, templateId, nSets, K, branchK, branchGroup, formulaValues, weights, rootFreqs,
+                patternOf, nullptr, siteLnL};
+    c.rowLnL = rowLnL;
+    return batch_sites(p, c);
 }
 
 int hb2_batch_column_likelihoods(hb2_partition *p, int64_t templateId, int64_t nSets, const int64_t *columns, int64_t K,

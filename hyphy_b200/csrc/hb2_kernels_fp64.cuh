@@ -1698,6 +1698,160 @@ __global__ void __launch_bounds__(64) prune_batch_kernel(BatchPruneArgs a) {
 }
 
 // ------------------------------------------------------------------------------------------------
+// branch_rows_kernel (hb2_batch_branch_component_likelihoods): the likelihood of every set with one branch pinned to one of
+// its mixture components, for MEME's branch-level empirical Bayes factors (MEME.bf:886-944).  For branch b with child node
+// c, in_c is c's subtree vector (prune_batch_kernel<true>'s cond / node_ex) and A_b the vector at the parent end of b of
+// everything outside c's subtree; row r of b then has L_{b,r} = sum_p A_b[p] (P_r in_c)[p] with P_r the row's own
+// exponential, whatever the branch's weights.  Runs after prune_batch_kernel<true> on the same chunk, one CTA of 64 threads
+// per set, thread = state.  Internal nodes are visited in reverse flat order (a pre-order); node n with outside vector O_n
+// (the root: pi, exponent 0) and children c_1..c_m:
+//   1. m_c = P_c in_c for each child, P_c the mixed matrix formed entry by entry as the inside pass forms it (mix_entry),
+//      leaves by their state or ambiguity row as there; stored in msg[c];
+//   2. the suffix products m_{c_{i+1}} ... m_{c_m}, stored in side[c_i];
+//   3. forward, with the running prefix O_n m_{c_1} ... m_{c_{i-1}}: A_{c_i} = prefix * suffix (no division, so a zero
+//      message does not poison its siblings), then every row of c_i, then for an internal c_i its outside vector
+//      O_{c_i}[j] = sum_p A_{c_i}[p] P_{c_i}[p][j], kept in side[c_i] until c_i is visited.
+// The transposed table serves the messages and rows with coalesced reads, as in the inside pass; the outside product reads
+// its rows, as bc_path_kernel does.
+// Numerical rules: every message, suffix, prefix, A and outside vector is brought to max in [0.5, 1) by an exact power of
+// two after each factor, with its binary exponent carried (so the products over the children of a wide node are rescaled
+// between factors, more often than RESCALE_BELOW requires).  A row's sum is encoded by pattern_lnl: a row likelihood of 0
+// gives -inf, and NaN propagates.  Padded states (>= D) stay 0.
+// ------------------------------------------------------------------------------------------------
+struct BranchRowsArgs {
+    BatchPruneArgs in;        // the chunk's inside pass (MIX layout): PT, cond, node_ex, pat, leaf, ambig, pi, tree, mix_w, row_off
+    double *msg, *side;       // [nSets][B][64] messages; suffix products, then A, then outside vectors
+    int *msg_ex, *side_ex;    // [nSets][B] their binary exponents
+    double *rows;             // [nSets][R] log-likelihood of each row
+};
+
+__global__ void __launch_bounds__(64) branch_rows_kernel(BranchRowsArgs g) {
+    __shared__ double xs[64];
+    __shared__ double red[2];
+    const BatchPruneArgs &a = g.in;
+    const int s = blockIdx.x, k = threadIdx.x;
+    const bool live = k < a.D;
+    const int pattern = a.pat[s];
+    const double *PTs = a.PT + (size_t)s * a.R * 4096;
+    const double *cs = a.cond + (size_t)s * a.I * 64;
+    const int *node_ex = a.node_ex + (size_t)s * a.I;
+    const double *mw = a.mix_w + (size_t)s * a.R;
+    double *msg = g.msg + (size_t)s * a.B * 64, *side = g.side + (size_t)s * a.B * 64;
+    int *msg_ex = g.msg_ex + (size_t)s * a.B, *side_ex = g.side_ex + (size_t)s * a.B;
+    double *rows = g.rows + (size_t)s * a.R;
+    // max over the 64 threads; a positive finite maximum is brought to [0.5, 1) by an exact power of two
+    auto renorm = [&](double &v, int &ex) {
+        double mx = v;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+        __syncthreads();
+        if ((k & 31) == 0) red[k >> 5] = mx;
+        __syncthreads();
+        mx = fmax(red[0], red[1]);
+        if (mx > 0.0 && mx < INFINITY) {
+            const int e = ilogb(mx) + 1;
+            v = v * exp2i(-(e / 2)) * exp2i(-(e - e / 2));
+            ex += e;
+        }
+    };
+    auto block_sum = [&](double v) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        __syncthreads();
+        if ((k & 31) == 0) red[k >> 5] = v;
+        __syncthreads();
+        return red[0] + red[1];
+    };
+    auto broadcast = [&](double v) {             // xs <- v of every thread
+        __syncthreads();
+        xs[k] = v;
+        __syncthreads();
+    };
+    // (P in_child)[k], entry(j) = P[k][j]: a leaf's state or ambiguity row, or the child's vector staged in xs
+    auto apply = [&](int child, auto entry) {
+        double m = 0.0;
+        if (!live) return m;
+        if (child < a.L) {
+            const int code = a.leaf[(size_t)child * a.Sp + pattern];
+            if (code >= 0) m = entry(code);
+            else {
+                const double *amb = a.ambig + (size_t)(-code - 1) * 64;
+                for (int j = 0; j < a.D; j++) { const double w = amb[j]; if (w != 0.0) m = fma(w, entry(j), m); }
+            }
+        } else {
+            for (int j = 0; j < a.D; j++) m = fma(xs[j], entry(j), m);
+        }
+        return m;
+    };
+    auto stage_inside = [&](int child) {        // xs <- in_child of an internal child; its exponent
+        if (child < a.L) return 0;
+        broadcast(cs[(size_t)(child - a.L) * 64 + k]);
+        return node_ex[child - a.L];
+    };
+    for (int n = a.I - 1; n >= 0; n--) {
+        const int c_begin = a.tree.child_start[n], c_end = a.tree.child_start[n + 1];
+        // 1. messages
+        for (int ci = c_begin; ci < c_end; ci++) {
+            const int child = a.tree.child_ids[ci];
+            const int r0 = a.row_off[child], nc = a.row_off[child + 1] - r0;
+            const double *PT = PTs + (size_t)r0 * 4096;
+            double wc[4];
+            mix_weights(wc, mw + r0, nc);
+            int ex = stage_inside(child);
+            double m = apply(child, [&](int j) { return mix_entry(wc, nc, [&](int c) { return PT[j * 64 + k + (size_t)c * 4096]; }); });
+            renorm(m, ex);
+            msg[(size_t)child * 64 + k] = m;
+            if (k == 0) msg_ex[child] = ex;
+        }
+        __syncthreads();                         // msg_ex visible to the block
+        // 2. suffix products
+        double v = live ? 1.0 : 0.0;
+        int ve = 0;
+        for (int ci = c_end - 1; ci >= c_begin; ci--) {
+            const int child = a.tree.child_ids[ci];
+            side[(size_t)child * 64 + k] = v;
+            if (k == 0) side_ex[child] = ve;
+            v *= msg[(size_t)child * 64 + k];
+            ve += msg_ex[child];
+            renorm(v, ve);
+        }
+        // 3. prefix, A, rows and outside vectors; O_n is the root vector or what the parent's visit left in side[L+n]
+        __syncthreads();                         // side_ex visible to the block
+        if (n == a.I - 1) { v = live ? a.pi[k] : 0.0; ve = 0; }
+        else { v = side[(size_t)(a.L + n) * 64 + k]; ve = side_ex[a.L + n]; }
+        for (int ci = c_begin; ci < c_end; ci++) {
+            const int child = a.tree.child_ids[ci];
+            const int r0 = a.row_off[child], nc = a.row_off[child + 1] - r0;
+            const double *PT = PTs + (size_t)r0 * 4096;
+            double A = v * side[(size_t)child * 64 + k];
+            int ae = ve + side_ex[child];
+            renorm(A, ae);
+            const int ie = stage_inside(child);
+            for (int c = 0; c < nc; c++) {
+                const double *Pr = PT + (size_t)c * 4096;
+                const double sum = block_sum(A * apply(child, [&](int j) { return Pr[j * 64 + k]; }));
+                if (k == 0) rows[r0 + c] = pattern_lnl(sum, ae + ie, [] {});
+            }
+            if (child >= a.L) {                  // O_child[k] = sum_p A[p] P[p][k] = sum_p A[p] PT[k][p]
+                double wc[4];
+                mix_weights(wc, mw + r0, nc);
+                broadcast(A);
+                double o = 0.0;
+                if (live)
+                    for (int p = 0; p < a.D; p++)
+                        o = fma(xs[p], mix_entry(wc, nc, [&](int c) { return PT[k * 64 + p + (size_t)c * 4096]; }), o);
+                renorm(o, ae);
+                side[(size_t)child * 64 + k] = o;
+                if (k == 0) side_ex[child] = ae;
+            }
+            v *= msg[(size_t)child * 64 + k];
+            ve += msg_ex[child];
+            renorm(v, ve);
+        }
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // prune_rates_kernel (hb2_batch_site_rates): prune_batch_kernel<false>'s recursion for 4..32 padded states.  A group of
 // G = 4, 8, 16 or 32 lanes owns one set, lane k = parent state k, and 32/G sets share a warp (24 states take G = 32, so
 // a quarter of their lanes idle).  A child's vector is broadcast with width-G shuffles, the node maximum is a group

@@ -44,6 +44,8 @@ ABI = [
     ("hb2_evaluate_classes", C.c_int, [C.c_void_p, _dp, C.c_int64, _ip, _dp, _dp, _dp, _ip]),
     ("hb2_batch_site_likelihoods", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, _dp, _ip, _dp, _dp]),
     ("hb2_batch_site_mixture_likelihoods", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, C.c_int64, _ip, _dp, _dp, _ip, _dp, _dp]),
+    ("hb2_batch_branch_component_likelihoods", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, C.c_int64, _ip, _dp, _dp, _ip,
+                                                         _dp, _dp, _dp]),
     ("hb2_batch_column_likelihoods", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, C.c_int64, _ip, _dp, _dp, _ip, _dp, _dp]),
     ("hb2_batch_site_rates", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, _dp, _dp, _dp]),
     ("hb2_read_conditionals", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _dp, _i32p]),
@@ -283,6 +285,21 @@ class Partition:
         _check(self._lib.hb2_batch_site_mixture_likelihoods(self._h, int(template), len(po), ppo, K, pbk, pv, pw, pbg, ppi,
                                                             out.ctypes.data_as(_dp)))
         return out
+
+    def batch_branch_component_likelihoods(self, pattern_of, formula_values, weights, root_freqs, branch_k=None,
+                                           branch_group=None, template=0):
+        """MEME's branch-level empirical Bayes (hb2_batch_branch_component_likelihoods): arguments as
+        batch_site_mixture_likelihoods.  Returns (site_lnl [nSets], row_lnl [nSets, R]): row r of a set is its log-likelihood
+        with that row's branch pinned to that row's component alone."""
+        po, ppo = _i(pattern_of)
+        assert weights is not None
+        K, pbk, pv, pw, pbg, keep = self._batch_rows(len(po), formula_values, weights, branch_k, branch_group)
+        pi, ppi = _d(root_freqs)
+        site = np.empty(len(po))
+        rows = np.empty((len(po), keep[1].shape[1]))
+        _check(self._lib.hb2_batch_branch_component_likelihoods(self._h, int(template), len(po), ppo, K, pbk, pv, pw, pbg, ppi,
+                                                                site.ctypes.data_as(_dp), rows.ctypes.data_as(_dp)))
+        return site, rows
 
     def _batch_rows(self, n_sets, formula_values, weights, branch_k, branch_group):
         """Checked arguments of the batch entry points that take both set layouts: weights None means one row per branch

@@ -172,6 +172,32 @@ int hb2_batch_site_mixture_likelihoods(hb2_partition *p, int64_t templateId, int
                                        const double *weights, const int64_t *branchGroup, const double *rootFreqs,
                                        double *siteLnL);
 
+/* Branch-level empirical Bayes for MEME (meme.compute_branch_EBF, MEME.bf:886-944, called for every tested branch of a
+ * site whose fitted beta+ > alpha with a positive weight above 1e-6, :1415-1431): the site's likelihood with each branch
+ * pinned to each of its mixture components, for every set in one call.  Arguments as hb2_batch_site_mixture_likelihoods
+ * (R = sum_b branchK[b] rows per set, in branch order with the components of one branch consecutive), plus:
+ *   rowLnL   [nSets][R]: row r = component k of branch b is the log-likelihood of pattern patternOf[s] under set s with
+ *            branch b's transition matrix replaced by that row's exponential alone, Exp(Q_{s,r}) with weight 1, and every
+ *            other branch keeping its mixture sum_k w_k Exp(Q_k) as the batch pruning forms it.  NOT multiplied by the
+ *            pattern frequency; it does not depend on branch b's own weights (a component of weight 0 still gets its
+ *            pinned value); a branch with one component gives the set's own likelihood up to rounding.
+ *   siteLnL  nullable [nSets]: the set's mixed log-likelihood, bit for bit what hb2_batch_site_mixture_likelihoods
+ *            returns for the same arguments (the same inside pass).
+ * MEME's posteriors are post_{b,k} = w_{s,r} exp(rowLnL[s][r] - siteLnL[s]) and the EBF of branch b is its positive
+ * component's posterior odds over its prior odds, (post / (1 - post)) / (w / (1 - w)).  The weights are neither normalised
+ * nor checked: the host maps MEME's stick-breaking mixture_aux_weight parameters to plain weights.  All values come from
+ * one inside and one outside (pre-order) pass per set, fp64, every vector renormalised by exact powers of two; a row of
+ * likelihood 0 gives -inf, and a NaN weight gives NaN for its set only.
+ * Refusals before anything is launched or written (the partition stays usable): everything
+ * hb2_batch_site_mixture_likelihoods refuses; weights == NULL (with one row per branch every row would equal siteLnL);
+ * rowLnL == NULL.  nSets == 0 after these checks does nothing.  33..64 states only; not available in class-group mode.
+ * Nothing an evaluation reads is touched: conditionals, scalers, walk plans and tags, the branch cache, the staged root
+ * vector, the P cache and the resident rate matrices. */
+int hb2_batch_branch_component_likelihoods(hb2_partition *p, int64_t templateId, int64_t nSets, const int64_t *patternOf,
+                                           int64_t K, const int64_t *branchK, const double *formulaValues,
+                                           const double *weights, const int64_t *branchGroup, const double *rootFreqs,
+                                           double *siteLnL, double *rowLnL);
+
 /* The batch likelihoods of caller-given columns instead of partition patterns (the refits of a parametric bootstrap score
  * columns simulated by hb2_batch_site_simulate, which are not patterns of the partition): set s scores
  * columns[s][0..L-1], in hb2_create's leafState codes (>= 0: a state < D; < 0: ambiguity row -(code+1) < nAmb).

@@ -5,12 +5,17 @@ Each fixture holds the reference's lnL and per-site log-likelihoods (ConstructCa
 alignment order) plus a checksum of the generated leaf states, so tests can prove they regenerated the same input.
 `--runs` writes tests/golden/reference_runs.json instead: what tests/test_host_binding.py compares the patched host
 with (the final lnL of an evaluation stream, joint ML ancestral sequences).
-Run where the reference binary was built:  python tools/make_golden.py [--runs | name ...]
+`--pinned` writes tests/golden/bsrel_12x80_k3_pinned.npz: MEME's branch-level empirical Bayes procedure
+(meme.compute_branch_EBF, MEME.bf:886-944) on every site at once -- see pinned_fixture.
+Run where the reference binary was built:  python tools/make_golden.py [--runs | --pinned | name ...]
 """
 import hashlib
 import json
 import os
+import re
+import subprocess
 import sys
+import tempfile
 
 import numpy as np
 
@@ -57,12 +62,68 @@ def reference_runs(out):
         f.write("\n")
 
 
+PINNED_CASE = "bsrel_12x80_k3"
+
+
+def pinned_script(w, path_bf, path_fas):
+    """The BS-REL script of ref_harness.write_hbl with branch-local mixture weights (as MEME's mixture_aux_weight
+    parameters are local to each tested branch), followed by, for every branch b and component k: b's weights set to
+    one-hot on k, the per-site log-likelihoods (ConstructCategoryMatrix SITE_LOG_LIKELIHOODS) printed as `PIN b k site
+    value`, b's weights restored.  A site's value in the whole-alignment function equals its one-site function's."""
+    rh.write_hbl(w, path_bf, path_fas)
+    wts = w.meta["mixture"]["weights"]
+    K, tree = len(wts), w.tree
+    lines = open(path_bf).read().splitlines()
+    glob = [i for i, line in enumerate(lines) if re.match(r"global bw\d+ = ", line)]
+    assert len(glob) == K
+    lines = [line for i, line in enumerate(lines) if i not in glob]         # bw_k: a model parameter local to each branch
+    at = max(i for i, line in enumerate(lines) if line.startswith("T.") and ".t := " in line) + 1
+    local = [f"T.{tree.names[b]}.bw{k + 1} = {rh._fmt(wts[k])};" for b in range(tree.n_branches) for k in range(K)]
+    lines[at:at] = local
+    for b in range(tree.n_branches):
+        nm = tree.names[b]
+        for k in range(K):
+            lines += [f"T.{nm}.bw{j + 1} = {1 if j == k else 0};" for j in range(K)]
+            lines.append("ConstructCategoryMatrix (sl, lf, SITE_LOG_LIKELIHOODS);")
+            lines.append(f'for (k = 0; k < Columns (sl); k += 1) {{ fprintf (stdout, "PIN {b} {k} ", k, " ", Format (sl[k], 30, 16), "\\n"); }}')
+        lines += [f"T.{nm}.bw{j + 1} = {rh._fmt(wts[j])};" for j in range(K)]
+    with open(path_bf, "w") as f:
+        f.write("\n".join(lines) + "\n")
+
+
+def pinned_fixture(out):
+    """tests/golden/bsrel_12x80_k3_pinned.npz: lnL and site_lnL of the branch-local script, and pinned [B*K][sites],
+    row b*K + k = every site with branch b (flat id) pinned to component k."""
+    w = CASES[PINNED_CASE]()
+    K, nb, n = len(w.meta["mixture"]["weights"]), w.tree.n_branches, len(w.site_to_pattern)
+    tmp = tempfile.mkdtemp(prefix="hb2ref_")
+    bf, fas = os.path.join(tmp, "job.bf"), os.path.join(tmp, "job.fas")
+    pinned_script(w, bf, fas)
+    proc = subprocess.run([rh.REF_BIN, "CPU=1", bf], cwd=tmp, stdin=subprocess.DEVNULL, capture_output=True, text=True, check=True)
+    lnL, site, pinned = None, np.full(n, np.nan), np.full((nb * K, n), np.nan)
+    for line in proc.stdout.splitlines():
+        f = line.split()
+        if line.startswith("LNL="):
+            lnL = float(line[4:])
+        elif f and f[0] == "SITE":
+            site[int(f[1])] = float(f[2])
+        elif f and f[0] == "PIN":
+            pinned[int(f[1]) * K + int(f[2]), int(f[3])] = float(f[4])
+    assert lnL is not None and not np.isnan(site).any() and not np.isnan(pinned).any(), proc.stdout[-2000:]
+    np.savez_compressed(os.path.join(out, PINNED_CASE + "_pinned.npz"), lnL=np.float64(lnL), site_lnL=site, pinned=pinned,
+                        checksum=np.array(checksum(w)), S=np.int64(w.S), sites=np.int64(n))
+    print(f"{PINNED_CASE}_pinned: lnL={lnL!r} rows={nb * K} sites={n}", flush=True)
+
+
 def main():
     out = os.path.join(ROOT, "tests", "golden")
     os.makedirs(out, exist_ok=True)
     only = sys.argv[1:]
     if only == ["--runs"]:
         reference_runs(out)
+        return
+    if only == ["--pinned"]:
+        pinned_fixture(out)
         return
     for name, make in CASES.items():
         if only and name not in only:
