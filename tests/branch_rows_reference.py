@@ -21,6 +21,9 @@ MUTATIONS = {
     "root_ones": "the root's outside vector is all ones instead of the root frequencies",
     "row_mixed": "a row is scored with the branch's mixed matrix instead of its own component",
     "drop_third_child": "the third child of a wide node is left out of its siblings' products",
+    "root_stationary": "the root's outside vector is the template's stationary vector instead of the caller's root vector",
+    "message_transposed": "the outside pass's child messages go through the transpose (m_c = P^T in_c)",
+    "outside_component0": "an internal child's outside vector goes through its branch's first component, not its mixture",
 }
 
 
@@ -46,8 +49,20 @@ def site_ld(tree, expm, V, W, branch_k, col, ambig, root):
     return br.prune_ld(tree, br.set_P(expm, V, W, branch_k), col[None, :], ambig, root)[0]
 
 
+def stationary(t):
+    """The stationary vector of a batch_reference.Template at its base rates: the column frequencies where it has them
+    (pi_i q_ij is symmetric for every alpha, beta), else the left null vector of its rate matrix."""
+    if t.cf is not None:
+        return np.asarray(t.cf, dtype=LD)
+    Q = br.dense(t, t.base)
+    vt = np.linalg.svd(Q.T)[2]
+    pi = np.abs(vt[-1])
+    return np.asarray(pi / pi.sum(), dtype=LD)
+
+
 def outside_rows(tree, expm, V, W, branch_k, col, ambig, root, mutate=()):
-    """[R] long-double log-likelihoods by one inside and one outside pass (the kernel's order, no scaling)."""
+    """[R] long-double log-likelihoods by one inside and one outside pass (the kernel's order, no scaling).  The
+    'root_stationary' mutation reads the template of `expm` (a batch_reference.ExpmCache)."""
     L, D = tree.n_leaves, len(root)
     P = br.set_P(expm, V, W, branch_k)
     off = _row_offsets(branch_k)
@@ -68,8 +83,16 @@ def outside_rows(tree, expm, V, W, branch_k, col, ambig, root, mutate=()):
             msg[c] = P[c] @ inside[c]
             v = v * msg[c]
         inside[L + i] = v
+    side_msg = msg
+    if "message_transposed" in mutate:                           # the inside pass stays right; the outside pass's copy not
+        side_msg = [None if m is None else P[c].T @ inside[c] for c, m in enumerate(msg)]
     out = np.empty(off[-1], dtype=LD)
-    outside = {L + tree.n_internal - 1: np.ones(D, dtype=LD) if "root_ones" in mutate else np.asarray(root, dtype=LD)}
+    root0 = np.asarray(root, dtype=LD)
+    if "root_ones" in mutate:
+        root0 = np.ones(D, dtype=LD)
+    elif "root_stationary" in mutate:
+        root0 = stationary(expm.t)
+    outside = {L + tree.n_internal - 1: root0}
     for i in reversed(range(tree.n_internal)):
         ch = kids[i]
         for pos, c in enumerate(ch):
@@ -79,10 +102,11 @@ def outside_rows(tree, expm, V, W, branch_k, col, ambig, root, mutate=()):
                     continue
                 if q == 2 and "drop_third_child" in mutate:
                     continue
-                A = A * msg[c2]
+                A = A * side_msg[c2]
             for r in range(off[c], off[c + 1]):
                 Pr = P[c] if "row_mixed" in mutate else expm(V[r])
                 out[r] = np.log(A @ (Pr @ inside[c]))
             if c >= L:
-                outside[c] = P[c] @ A if "outside_through_P" in mutate else A @ P[c]
+                Pc = expm(V[off[c]]) if "outside_component0" in mutate else P[c]
+                outside[c] = Pc @ A if "outside_through_P" in mutate else A @ Pc
     return out

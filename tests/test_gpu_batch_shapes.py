@@ -539,8 +539,9 @@ def test_simulation_agrees_with_scoring():
 # ---------------------------------------------------------------------------------------------------------------------
 # 6. memory-derived chunks
 # ---------------------------------------------------------------------------------------------------------------------
-def chunk_cap(case, sim):
-    """Sets per chunk as batch_sites computes them (hb2_engine.cu), with no branch-group hint."""
+def chunk_cap(case, sim, rows=False):
+    """Sets per chunk as batch_shape computes them (hb2_engine.cu), with no branch-group hint; `rows`: for
+    hb2_batch_branch_component_likelihoods, whose messages, outside vectors and rows add to a mixture set's bytes."""
     B, I, D, nF = case.w.tree.n_branches, case.w.tree.n_internal, case.w.D, case.tmpl.nF
     R = int(case.branch_k.sum()) if case.mix else B
     sim_bytes = B * D * (64 * 8 + 4) if sim else 0.0
@@ -549,6 +550,8 @@ def chunk_cap(case, sim):
     else:
         gk = int(case.branch_k.max())
         per_set = R * (4096 + nF + 1) * 8 + gk * EXPM_POW_TERMS * 4096 * 8 + I * 64 * 8
+        if rows:
+            per_set += B * 2 * (64 * 8 + 4) + R * 8
         cap = int(8.0e9 / (per_set + sim_bytes))
     return min(max(1, cap), 1024)
 
