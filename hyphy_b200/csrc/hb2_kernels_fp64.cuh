@@ -239,7 +239,9 @@ __device__ __forceinline__ float tf32_rn_dev(float x) {
 // Shared-powers path, stage 1: one small CTA per batch entry.  Measures the entry (weight = sum of |values|: formula
 // values of a compiled hand-over, matrix entries of a dense one), keeps the resident copy of the input (Vres / Qres:
 // hb2_time_resident replays from it) and decides whether the entry is a scalar multiple of its group's reference
-// direction:  |v_k[f] * w_ref - v_ref[f] * w_k| <= 1e-13 * w_k * w_ref  for every value f.  The reference is either
+// direction:  |v_k[f] * w_ref - v_ref[f] * w_k| <= 1e-13 * |v_ref[f]| * w_k  for every value f, so every value matches
+// its scaled reference value to 1e-13 of itself and a zero matches only a zero (a bound by the value's share of the weight,
+// 1e-13 * w_k * w_ref, would let a value with a small share drift by far more than 1e-13 of itself).  The reference is either
 // entry ref[k] of this batch (its powers are (re)built by expm_powers_kernel in this launch sequence) or, for small
 // batches, the direction the group's power table was last built from (refvec, kept on the device).
 // ------------------------------------------------------------------------------------------------
@@ -318,12 +320,12 @@ __global__ void __launch_bounds__(128) expm_classify_kernel(ExpmClassifyArgs a) 
     if (wr_cached >= 0.0) wr = wr_cached;
     int ok = (vr != nullptr) && (wr > 0.0) && (wk >= 0.0) && (wk < INFINITY) && (wr < INFINITY);   // NaN fails every comparison
     if (ok) {
-        const double tol = 1e-13 * wk * wr;
+        const double tol = 1e-13 * wk;
 #pragma unroll
         for (int i = 0; i < EXPM_CLASSIFY_REGS; i++)
-            if (tid + 128 * i < nV && !(fabs(xv[i] * wr - xr[i] * wk) <= tol)) ok = 0;
+            if (tid + 128 * i < nV && !(fabs(xv[i] * wr - xr[i] * wk) <= tol * fabs(xr[i]))) ok = 0;
         for (int f = tid + 128 * EXPM_CLASSIFY_REGS; f < nV; f += 128)
-            if (!(fabs(v[f] * wr - vr[f] * wk) <= tol)) ok = 0;
+            if (!(fabs(v[f] * wr - vr[f] * wk) <= tol * fabs(vr[f]))) ok = 0;
     }
     ok = __all_sync(0xffffffffu, ok);
     if ((tid & 31) == 0) bad[tid >> 5] = !ok;
@@ -359,9 +361,9 @@ __global__ void __launch_bounds__(256) expm_classify_warp_kernel(ExpmClassifyArg
     if (wr_cached >= 0.0) wr = wr_cached;
     int ok = (vr != nullptr) && (wr > 0.0) && (wk >= 0.0) && (wk < INFINITY) && (wr < INFINITY);   // NaN fails every comparison
     if (ok) {
-        const double tol = 1e-13 * wk * wr;
+        const double tol = 1e-13 * wk;
         for (int f = lane; f < a.nV; f += 32)
-            if (!(fabs(v[f] * wr - vr[f] * wk) <= tol)) ok = 0;
+            if (!(fabs(v[f] * wr - vr[f] * wk) <= tol * fabs(vr[f]))) ok = 0;
     }
     ok = __all_sync(0xffffffffu, ok);
     if (lane == 0) expm_classify_result(a, k, g, r, ok, wk);

@@ -496,7 +496,12 @@ __global__ void __launch_bounds__(256, 1) prune64_tc_walk_kernel(WalkArgs w) {
                 }
             } else if (enc & WALK_MUL) {
                 // side product of this node (its other children, multiplied up by another lane or earlier in this one):
-                // no matrix, just the element-wise product and the exponent
+                // no matrix, just the element-wise product and the exponent.  The step's (empty) ring phase is still
+                // awaited: it completes only once both warpgroups released the slot a step earlier, and that keeps this
+                // warpgroup within one step of the other.  Without it a warpgroup ran through side products ahead, its
+                // ring releases completed the other's count and restaged a slot the other was still reading, and its
+                // parity waits two phases ahead returned at once (two-tile units whose tiles run at different speeds).
+                mbar_wait(bar_full + (n_step & 1u), (n_step >> 1) & 1u, a.err);
                 const int cin = child - a.L;
                 const bool await = (enc & WALK_WAIT) != 0;
                 uint4 x4[16];

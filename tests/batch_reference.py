@@ -146,34 +146,18 @@ def set_P(expm, V, W, branch_k, mutate=()):
 
 def prune_ld(tree, P, cols, ambig, root, mutate=()):
     """log-likelihoods (long double) of columns [n, L] (leaf codes: state >= 0, ambiguity row -(r+1)) under P [B, D, D]
-    and the root vector, by the plain recursion without scaling (80-bit exponents reach 2^-16382)."""
+    and the root vector, by tests/resident_reference.py's recursion without scaling (80-bit exponents reach 2^-16382).
+    'pad_leak' adds 64 - D to every entry of every ambiguity row: each entry of the leaf's vector grows by 64 - D times
+    its matrix row sum, which is one -- the 64 - D padded states, each as a matrix entry of one."""
+    from tests import resident_reference as rr          # it builds on this module's expm_ld
     if "no_wide_rescale" in mutate:
         return _prune_fp64_node_scaled(tree, P, cols, ambig, root)
-    cols = np.atleast_2d(np.asarray(cols, dtype=np.int64))
-    n, L, D = len(cols), tree.n_leaves, P.shape[-1]
-    Pl = np.asarray(P, dtype=LD)
     amb = np.asarray(ambig, dtype=LD)
-    cond = [None] * tree.n_internal
-    for i, kids in enumerate(tree.children()):
-        v = np.ones((n, D), dtype=LD)
-        for c in kids:
-            if c < L:
-                codes = cols[:, c]
-                obs = codes >= 0
-                m = np.empty((n, D), dtype=LD)
-                m[obs] = Pl[c][:, codes[obs]].T
-                if not obs.all():
-                    rows = -codes[~obs] - 1
-                    if "amb_off_by_one" in mutate:
-                        rows = (rows + 1) % len(amb)
-                    m[~obs] = amb[rows] @ Pl[c].T
-                    if "pad_leak" in mutate:
-                        m[~obs] += 64 - D
-            else:
-                m = cond[c - L] @ Pl[c].T
-            v = v * m
-        cond[i] = v
-    return np.log(cond[-1] @ np.asarray(root, dtype=LD))
+    if "amb_off_by_one" in mutate and len(amb):
+        amb = np.roll(amb, -1, axis=0)                      # code -(r+1) reads row (r+1) mod nAmb
+    if "pad_leak" in mutate:
+        amb = amb + LD(64 - P.shape[-1])
+    return rr.class_sites(tree, P, cols, amb, root)
 
 
 def _prune_fp64_node_scaled(tree, P, cols, ambig, root):

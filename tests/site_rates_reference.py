@@ -86,7 +86,7 @@ def site_lnl(tree, A, r, cols, ambig, root, expm=None, mutate=()):
     P = rate_P(A, r, tree.n_leaves, expm, mutate)
     amb = np.asarray(ambig, dtype=np.float64)
     if "pad_leak" in mutate and len(amb):
-        amb = amb + (pad_states(D) - D) / D        # rows of P sum to 1: adds Dp - D to every ambiguity leaf's entry
+        amb = amb + (pad_states(D) - D)            # rows of P sum to 1: adds Dp - D to every ambiguity leaf's entry
     rt = np.full(D, 1.0 / D) if "root_ignored" in mutate else root
     pm = tuple(m for m in mutate if m == "amb_off_by_one")
     with np.errstate(divide="ignore"):

@@ -17,6 +17,7 @@ import scipy.linalg
 
 from hyphy_b200 import synth, LikelihoodFunction, engine
 from oracle import port
+from tests import resident_reference as rr
 
 pytestmark = pytest.mark.gpu
 
@@ -179,32 +180,11 @@ def oracle_sites(w, P):
 
 
 def longdouble_sites(w, P, forced_node=-1, forced_states=None):
-    """Per-pattern log-likelihoods of one rate class by a plain Felsenstein recursion in numpy.longdouble without any
-    scaling: its exponent range (x86-64: 80-bit extended, down to 2^-16382) covers every product in this suite.  Optionally
-    one node (flat id) pinned to a state per pattern."""
-    ld = np.longdouble
-    L, I = w.tree.n_leaves, w.tree.n_internal
-    pin = np.zeros((w.S, w.D), dtype=ld)
-    if forced_node >= 0:
-        pin[np.arange(w.S), forced_states] = 1
-    Pl = P.astype(ld)
-    amb = np.asarray(w.ambig, dtype=ld)
-    cond = [None] * I
-    for i, kids in enumerate(w.tree.children()):
-        v = np.ones((w.S, w.D), dtype=ld)
-        for c in kids:
-            if c < L:
-                codes = forced_states if c == forced_node else w.leaf_states[c]
-                obs = codes >= 0
-                m = np.empty((w.S, w.D), dtype=ld)
-                m[obs] = Pl[c][:, codes[obs]].T                         # (P x)[k] = P[k][state]
-                if not obs.all():
-                    m[~obs] = amb[-codes[~obs] - 1] @ Pl[c].T
-            else:
-                m = cond[c - L] @ Pl[c].T
-            v *= m
-        cond[i] = v * pin if L + i == forced_node else v
-    return np.log(cond[I - 1] @ w.pi.astype(ld)).astype(np.float64)
+    """Per-pattern log-likelihoods of one rate class by tests/resident_reference.py's plain recursion in numpy.longdouble
+    without any scaling: its exponent range (x86-64: 80-bit extended, down to 2^-16382) covers every product in this
+    suite.  Optionally one node (flat id) pinned to a state per pattern."""
+    pin = (forced_node, forced_states) if forced_node >= 0 else None
+    return rr.class_sites(w.tree, P, w.leaf_states.T, w.ambig, w.pi, pin).astype(np.float64)
 
 
 def depth_of(tree):
