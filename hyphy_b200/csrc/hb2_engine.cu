@@ -236,7 +236,8 @@ struct BatchShape {
     int64_t R = 0, nF = 0, gk = 0, sets = 0;  // rows per set, formula values per row, groups per set; sets per chunk
     int64_t mat = 4096, vec = 64;             // doubles per P matrix (Dp^2) and per node vector (Dp)
     int64_t ent = 0, in = 0;                  // rows per set through launch_expm (R; 0 for site rates) and input doubles per set
-    int64_t side = 0;                         // branches per set with outside scratch (branch rows: B; 0 for every other call)
+    int64_t side = 0;                         // branches per set with outside scratch (branch rows, leaf support: B; else 0)
+    int64_t rows = 0, sup = 0;                // doubles per set of row results (branch rows: R) and of support (leaf support: L*D)
 };
 
 }  // namespace
@@ -297,9 +298,10 @@ struct hb2_partition {
         DeviceBuffer<int> slot, pat, node_ex; // identity slots [entries], patterns [sets], node exponents [sets][I]
         DeviceBuffer<int> row, col;           // first component row of each branch [B+1], caller columns [L][sets]
         PinnedBuffer<int> h_slot, h_pat, h_col;   // staging of slot, pat and col
-        // hb2_batch_branch_component_likelihoods only (sh.side = B; empty for every other call): messages and outside
-        // vectors [sets][2][B][64], their exponents [sets][2][B], and the row log-likelihoods [sets][R]
-        DeviceBuffer<double> side, rows;
+        // hb2_batch_branch_component_likelihoods and hb2_batch_leaf_support only (sh.side = B; empty for every other call):
+        // messages and outside vectors [sets][2][B][64] and their exponents [sets][2][B]; then the row log-likelihoods
+        // [sets][R] (branch rows) or the leaf support [sets][L][D] (leaf support)
+        DeviceBuffer<double> side, rows, sup;
         DeviceBuffer<int> side_ex;
         // Sizes the workspace for chunks of `sh`.  A chunk that does not fit re-sizes the whole workspace for this call,
         // after releasing it, so that memory stays at one call's chunk footprint (~8 GB) instead of adding up the largest
@@ -308,7 +310,8 @@ struct hb2_partition {
             const int64_t sets = sh.sets, nr = sets * sh.R, ne = sets * sh.ent;
             if (sets <= (int64_t)out.size() && ne <= (int64_t)slot.size() && sets * sh.gk <= ex.G && sets * sh.in <= (int64_t)V.size() &&
                 nr * sh.mat <= (int64_t)PT.size() && sets * I * sh.vec <= (int64_t)cond.size() && sets * L <= (int64_t)col.size() &&
-                sets * sh.side * 128 <= (int64_t)side.size() && (sh.side == 0 || nr <= (int64_t)rows.size()))
+                sets * sh.side * 128 <= (int64_t)side.size() && sets * sh.rows <= (int64_t)rows.size() &&
+                sets * sh.sup <= (int64_t)sup.size())
                 return 0;
             CU(cudaStreamSynchronize(stream));
             *this = BatchWorkspace();
@@ -316,7 +319,8 @@ struct hb2_partition {
                 mixw.alloc(ne) || cond.alloc((size_t)sets * I * sh.vec) || out.alloc(sets) || slot.alloc(ne) || pat.alloc(sets) ||
                 node_ex.alloc((size_t)sets * I) || row.alloc(sh.row_off.size()) || col.alloc((size_t)sets * L) || pi.alloc(64) ||
                 h_slot.alloc(ne) || h_pat.alloc(sets) || h_col.alloc((size_t)sets * L) ||
-                (sh.side && (side.alloc((size_t)sets * sh.side * 128) || side_ex.alloc((size_t)sets * sh.side * 2) || rows.alloc(nr)))) {
+                (sh.side && (side.alloc((size_t)sets * sh.side * 128) || side_ex.alloc((size_t)sets * sh.side * 2))) ||
+                (sh.rows && rows.alloc((size_t)sets * sh.rows)) || (sh.sup && sup.alloc((size_t)sets * sh.sup))) {
                 *this = BatchWorkspace();     // fits nothing: the next call sizes it again
                 return 1;
             }
@@ -1689,7 +1693,9 @@ int hb2_evaluate_classes(hb2_partition *p, const double *weights, int64_t nUpdat
 // (LEISR's site model); its P matrices come from expm_rates_kernel and its likelihood from prune_rates_kernel.
 // BranchRows: MixtureSites, and after its pruning every component row of every branch pinned alone (rowLnL [nSets][R],
 // branch_rows_kernel; MEME's branch-level empirical Bayes factors).  siteLnL is nullable there.
-enum class BatchEntry { Sites, MixtureSites, Columns, Simulate, Rates, BranchRows };
+// LeafSupport: Sites (weights == nullptr) or MixtureSites, and after its pruning every leaf's support [nSets][L][D]
+// (leaf_support_kernel; MEME's and PRIME's --impute-states).  siteLnL is nullable there.
+enum class BatchEntry { Sites, MixtureSites, Columns, Simulate, Rates, BranchRows, LeafSupport };
 struct BatchCall {
     BatchEntry entry;
     int64_t templateId, nSets, K;
@@ -1703,6 +1709,7 @@ struct BatchCall {
     int64_t cat = 0;
     const double *rates = nullptr;
     double *rowLnL = nullptr;
+    double *support = nullptr;
 };
 
 // Sets per chunk of hb2_batch_site_rates, whatever the memory rule allows: at 4 states and 256 taxa a chunk of this many
@@ -1711,8 +1718,9 @@ constexpr int64_t RATES_MAX_SETS = 65536;
 
 // Every refusal of the batch entry points, before anything is launched or written.
 static int check_batch(const hb2_partition *p, const BatchCall &c) {
-    const bool rows = c.entry == BatchEntry::BranchRows;
-    const bool sites = c.entry == BatchEntry::Sites || c.entry == BatchEntry::MixtureSites || rows, sim = c.entry == BatchEntry::Simulate;
+    const bool rows = c.entry == BatchEntry::BranchRows, leaves = c.entry == BatchEntry::LeafSupport;
+    const bool sites = c.entry == BatchEntry::Sites || c.entry == BatchEntry::MixtureSites || rows || leaves;
+    const bool sim = c.entry == BatchEntry::Simulate;
     const char *fn = sim ? "hb2_batch_site_simulate" : "hb2_batch_column_likelihoods";
     if (!p) return fail(c.entry == BatchEntry::Sites ? "null argument" : "null partition");
     if (sites) {
@@ -1720,9 +1728,10 @@ static int check_batch(const hb2_partition *p, const BatchCall &c) {
             return fail("hb2_batch_branch_component_likelihoods: weights must not be null (with one row per branch every row "
                         "would equal siteLnL)");
         if (rows && !c.rowLnL) return fail("hb2_batch_branch_component_likelihoods: rowLnL must not be null");
+        if (leaves && !c.support) return fail("hb2_batch_leaf_support: support must not be null");
         if (c.entry == BatchEntry::MixtureSites && !c.weights) return fail("weights must not be null");
         if (c.entry == BatchEntry::MixtureSites && !c.formulaValues) return fail("formulaValues must not be null");
-        if (!c.formulaValues || !c.rootFreqs || (!c.siteLnL && !rows) || !c.patternOf) return fail("null argument");
+        if (!c.formulaValues || !c.rootFreqs || (!c.siteLnL && !rows && !leaves) || !c.patternOf) return fail("null argument");
         if (c.nSets < 0) return fail("bad set count");
     } else {
         if (c.nSets < 0) return fail("%s: nSets=%lld is negative", fn, (long long)c.nSets);
@@ -1790,6 +1799,12 @@ static BatchShape batch_shape(const hb2_partition *p, const BatchCall &c) {
     if (c.entry == BatchEntry::BranchRows) {    // messages and outside vectors with their exponents, and the row results
         sh.side = B;
         per_set += (double)B * 2 * (64 * 8 + 4) + (double)sh.R * 8;
+        sh.rows = sh.R;
+    }
+    if (c.entry == BatchEntry::LeafSupport) {   // messages and outside vectors with their exponents, and the support rows
+        sh.side = B;
+        sh.sup = p->L * D;
+        per_set += (double)B * 2 * (64 * 8 + 4) + (double)sh.sup * 8;
     }
     sh.sets = std::min<int64_t>({c.nSets, std::max<int64_t>(1, (int64_t)(8.0e9 / (per_set + sim_bytes))), 1024});
     sh.ent = sh.R;
@@ -1896,8 +1911,9 @@ static int exponentiate_chunk(hb2_partition *p, const BatchCall &c, const BatchS
     return launch_expm(p, {Kind::Compiled, (int)c.templateId}, ws.V, ws.slot, (int)ne, false, sp, 0, ws.PT);
 }
 
-// Likelihoods of sets s0 .. s0+nb-1 from the chunk's P area.  Branch rows: then branch_rows_kernel on the inside pass's node
-// vectors (so siteLnL stays hb2_batch_site_mixture_likelihoods' bit for bit), and the chunk's rows go down.
+// Likelihoods of sets s0 .. s0+nb-1 from the chunk's P area.  Branch rows and leaf support: then branch_rows_kernel or
+// leaf_support_kernel on the inside pass's node vectors (so siteLnL stays the likelihood entry point's bit for bit), and the
+// chunk's rows or support go down.
 static int score_chunk(hb2_partition *p, const BatchCall &c, const BatchShape &sh, int64_t s0, int64_t nb) {
     hb2_partition::BatchWorkspace &ws = p->batch;
     const int64_t L = p->L;
@@ -1919,13 +1935,18 @@ static int score_chunk(hb2_partition *p, const BatchCall &c, const BatchShape &s
     else hb2::prune_batch_kernel<false><<<(unsigned)nb, 64, 0, p->stream>>>(ba);
     p->launches++;
     CU(cudaGetLastError());
-    if (c.rowLnL) {
+    if (c.rowLnL || c.support) {
         const size_t side = (size_t)nb * p->B;
-        hb2::BranchRowsArgs g{ba, ws.side, ws.side + side * 64, ws.side_ex, ws.side_ex + side, ws.rows};
-        hb2::branch_rows_kernel<<<(unsigned)nb, 64, 0, p->stream>>>(g);
+        hb2::OutsideArgs g{ba, ws.side, ws.side + side * 64, ws.side_ex, ws.side_ex + side, ws.rows, ws.sup};
+        if (c.rowLnL) hb2::branch_rows_kernel<<<(unsigned)nb, 64, 0, p->stream>>>(g);
+        else if (c.weights) hb2::leaf_support_kernel<true><<<(unsigned)nb, 64, 0, p->stream>>>(g);
+        else hb2::leaf_support_kernel<false><<<(unsigned)nb, 64, 0, p->stream>>>(g);
         p->launches++;
         CU(cudaGetLastError());
-        CU(cudaMemcpyAsync(c.rowLnL + s0 * sh.R, ws.rows, (size_t)nb * sh.R * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
+        if (c.rowLnL)
+            CU(cudaMemcpyAsync(c.rowLnL + s0 * sh.R, ws.rows, (size_t)nb * sh.R * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
+        else
+            CU(cudaMemcpyAsync(c.support + s0 * sh.sup, ws.sup, (size_t)nb * sh.sup * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
     }
     if (c.siteLnL) CU(cudaMemcpyAsync(c.siteLnL + s0, ws.out, (size_t)nb * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
     return 0;
@@ -2010,6 +2031,15 @@ int hb2_batch_branch_component_likelihoods(hb2_partition *p, int64_t templateId,
     BatchCall c{BatchEntry::BranchRows, templateId, nSets, K, branchK, branchGroup, formulaValues, weights, rootFreqs,
                 patternOf, nullptr, siteLnL};
     c.rowLnL = rowLnL;
+    return batch_sites(p, c);
+}
+
+int hb2_batch_leaf_support(hb2_partition *p, int64_t templateId, int64_t nSets, const int64_t *patternOf, int64_t K,
+                           const int64_t *branchK, const double *formulaValues, const double *weights,
+                           const int64_t *branchGroup, const double *rootFreqs, double *siteLnL, double *support) {
+    BatchCall c{BatchEntry::LeafSupport, templateId, nSets, K, branchK, branchGroup, formulaValues, weights, rootFreqs,
+                patternOf, nullptr, siteLnL};
+    c.support = support;
     return batch_sites(p, c);
 }
 

@@ -1700,19 +1700,25 @@ __global__ void __launch_bounds__(64) prune_batch_kernel(BatchPruneArgs a) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// branch_rows_kernel (hb2_batch_branch_component_likelihoods): the likelihood of every set with one branch pinned to one of
-// its mixture components, for MEME's branch-level empirical Bayes factors (MEME.bf:886-944).  For branch b with child node
-// c, in_c is c's subtree vector (prune_batch_kernel<true>'s cond / node_ex) and A_b the vector at the parent end of b of
-// everything outside c's subtree; row r of b then has L_{b,r} = sum_p A_b[p] (P_r in_c)[p] with P_r the row's own
-// exponential, whatever the branch's weights.  Runs after prune_batch_kernel<true> on the same chunk, one CTA of 64 threads
-// per set, thread = state.  Internal nodes are visited in reverse flat order (a pre-order); node n with outside vector O_n
-// (the root: pi, exponent 0) and children c_1..c_m:
-//   1. m_c = P_c in_c for each child, P_c the mixed matrix formed entry by entry as the inside pass forms it (mix_entry),
-//      leaves by their state or ambiguity row as there; stored in msg[c];
+// The batch outside pass (outside_pass), behind two kernels that run after prune_batch_kernel on the same chunk, one CTA
+// of 64 threads per set, thread = state.  For branch b with child node c, in_c is c's subtree vector (the inside pass's
+// cond / node_ex) and A_b the vector at the parent end of b of everything outside c's subtree.
+//   branch_rows_kernel (hb2_batch_branch_component_likelihoods, MIX layout only): the likelihood of every set with one
+//     branch pinned to one of its mixture components, for MEME's branch-level empirical Bayes factors (MEME.bf:886-944):
+//     row r of b has L_{b,r} = sum_p A_b[p] (P_r in_c)[p] with P_r the row's own exponential, whatever the branch's weights.
+//   leaf_support_kernel<MIX> (hb2_batch_leaf_support, both layouts): for every leaf l, the predictive distribution of its
+//     state given every other leaf (ReconstructAncestors(MARGINAL, DOLEAVES), likefunc2.cpp:974-1006 and :1083-1093):
+//     u[k] = sum_p A_l[p] P_l[p][k], written as u[k] / sum_j u[j], or NaN in every entry when that total is 0 or not
+//     finite.  A_l leaves out l's own message, so the row does not read l's code.
+// Internal nodes are visited in reverse flat order (a pre-order); node n with outside vector O_n (the root: pi, exponent 0)
+// and children c_1..c_m:
+//   1. m_c = P_c in_c for each child, P_c the branch's matrix (MIX: mixed entry by entry as the inside pass mixes it,
+//      mix_entry), leaves by their state or ambiguity row as there; stored in msg[c];
 //   2. the suffix products m_{c_{i+1}} ... m_{c_m}, stored in side[c_i];
 //   3. forward, with the running prefix O_n m_{c_1} ... m_{c_{i-1}}: A_{c_i} = prefix * suffix (no division, so a zero
-//      message does not poison its siblings), then every row of c_i, then for an internal c_i its outside vector
-//      O_{c_i}[j] = sum_p A_{c_i}[p] P_{c_i}[p][j], kept in side[c_i] until c_i is visited.
+//      message does not poison its siblings), then what the kernel emits at c_i (every row of c_i, or for a leaf c_i its
+//      support row), then for an internal c_i its outside vector O_{c_i}[j] = sum_p A_{c_i}[p] P_{c_i}[p][j], kept in
+//      side[c_i] until c_i is visited.  A leaf's u is the same product.
 // The transposed table serves the messages and rows with coalesced reads, as in the inside pass; the outside product reads
 // its rows, as bc_path_kernel does.
 // Numerical rules: every message, suffix, prefix, A and outside vector is brought to max in [0.5, 1) by an exact power of
@@ -1720,27 +1726,31 @@ __global__ void __launch_bounds__(64) prune_batch_kernel(BatchPruneArgs a) {
 // between factors, more often than RESCALE_BELOW requires).  A row's sum is encoded by pattern_lnl: a row likelihood of 0
 // gives -inf, and NaN propagates.  Padded states (>= D) stay 0.
 // ------------------------------------------------------------------------------------------------
-struct BranchRowsArgs {
-    BatchPruneArgs in;        // the chunk's inside pass (MIX layout): PT, cond, node_ex, pat, leaf, ambig, pi, tree, mix_w, row_off
+struct OutsideArgs {
+    BatchPruneArgs in;        // the chunk's inside pass: PT, cond, node_ex, pat, leaf, ambig, pi, tree (MIX: mix_w, row_off)
     double *msg, *side;       // [nSets][B][64] messages; suffix products, then A, then outside vectors
     int *msg_ex, *side_ex;    // [nSets][B] their binary exponents
-    double *rows;             // [nSets][R] log-likelihood of each row
+    double *rows;             // branch_rows_kernel: [nSets][R] log-likelihood of each row
+    double *support;          // leaf_support_kernel: [nSets][L][D] support of each leaf's states
 };
 
-__global__ void __launch_bounds__(64) branch_rows_kernel(BranchRowsArgs g) {
+enum class OutsideEmit { BranchRows, LeafSupport };
+
+template <OutsideEmit EMIT, bool MIX>
+__device__ __forceinline__ void outside_pass(const OutsideArgs &g) {
     __shared__ double xs[64];
     __shared__ double red[2];
     const BatchPruneArgs &a = g.in;
     const int s = blockIdx.x, k = threadIdx.x;
     const bool live = k < a.D;
     const int pattern = a.pat[s];
-    const double *PTs = a.PT + (size_t)s * a.R * 4096;
+    const double *PTs = a.PT + (size_t)s * (MIX ? a.R : a.B) * 4096;
     const double *cs = a.cond + (size_t)s * a.I * 64;
     const int *node_ex = a.node_ex + (size_t)s * a.I;
-    const double *mw = a.mix_w + (size_t)s * a.R;
+    const double *mw = MIX ? a.mix_w + (size_t)s * a.R : nullptr;
     double *msg = g.msg + (size_t)s * a.B * 64, *side = g.side + (size_t)s * a.B * 64;
     int *msg_ex = g.msg_ex + (size_t)s * a.B, *side_ex = g.side_ex + (size_t)s * a.B;
-    double *rows = g.rows + (size_t)s * a.R;
+    double *rows = EMIT == OutsideEmit::BranchRows ? g.rows + (size_t)s * a.R : nullptr;
     // max over the 64 threads; a positive finite maximum is brought to [0.5, 1) by an exact power of two
     auto renorm = [&](double &v, int &ex) {
         double mx = v;
@@ -1790,17 +1800,28 @@ __global__ void __launch_bounds__(64) branch_rows_kernel(BranchRowsArgs g) {
         broadcast(cs[(size_t)(child - a.L) * 64 + k]);
         return node_ex[child - a.L];
     };
+    // the component rows of a child's branch: its first row of the set's P area and their count
+    auto branch_rows = [&](int child, int &nc) {
+        if constexpr (!MIX) { nc = 1; return child; }
+        else { const int r0 = a.row_off[child]; nc = a.row_off[child + 1] - r0; return r0; }
+    };
+    auto load_weights = [&](double (&wc)[4], int r0, int nc) {
+        if constexpr (MIX) mix_weights(wc, mw + r0, nc);
+    };
     for (int n = a.I - 1; n >= 0; n--) {
         const int c_begin = a.tree.child_start[n], c_end = a.tree.child_start[n + 1];
         // 1. messages
         for (int ci = c_begin; ci < c_end; ci++) {
             const int child = a.tree.child_ids[ci];
-            const int r0 = a.row_off[child], nc = a.row_off[child + 1] - r0;
+            int nc;
+            const int r0 = branch_rows(child, nc);
             const double *PT = PTs + (size_t)r0 * 4096;
             double wc[4];
-            mix_weights(wc, mw + r0, nc);
+            load_weights(wc, r0, nc);
             int ex = stage_inside(child);
-            double m = apply(child, [&](int j) { return mix_entry(wc, nc, [&](int c) { return PT[j * 64 + k + (size_t)c * 4096]; }); });
+            double m;
+            if constexpr (MIX) m = apply(child, [&](int j) { return mix_entry(wc, nc, [&](int c) { return PT[j * 64 + k + (size_t)c * 4096]; }); });
+            else m = apply(child, [&](int j) { return PT[j * 64 + k]; });
             renorm(m, ex);
             msg[(size_t)child * 64 + k] = m;
             if (k == 0) msg_ex[child] = ex;
@@ -1817,34 +1838,47 @@ __global__ void __launch_bounds__(64) branch_rows_kernel(BranchRowsArgs g) {
             ve += msg_ex[child];
             renorm(v, ve);
         }
-        // 3. prefix, A, rows and outside vectors; O_n is the root vector or what the parent's visit left in side[L+n]
+        // 3. prefix, A, what is emitted and outside vectors; O_n is the root vector or what the parent's visit left in side[L+n]
         __syncthreads();                         // side_ex visible to the block
         if (n == a.I - 1) { v = live ? a.pi[k] : 0.0; ve = 0; }
         else { v = side[(size_t)(a.L + n) * 64 + k]; ve = side_ex[a.L + n]; }
         for (int ci = c_begin; ci < c_end; ci++) {
             const int child = a.tree.child_ids[ci];
-            const int r0 = a.row_off[child], nc = a.row_off[child + 1] - r0;
+            int nc;
+            const int r0 = branch_rows(child, nc);
             const double *PT = PTs + (size_t)r0 * 4096;
             double A = v * side[(size_t)child * 64 + k];
             int ae = ve + side_ex[child];
             renorm(A, ae);
-            const int ie = stage_inside(child);
-            for (int c = 0; c < nc; c++) {
-                const double *Pr = PT + (size_t)c * 4096;
-                const double sum = block_sum(A * apply(child, [&](int j) { return Pr[j * 64 + k]; }));
-                if (k == 0) rows[r0 + c] = pattern_lnl(sum, ae + ie, [] {});
+            if constexpr (EMIT == OutsideEmit::BranchRows) {
+                const int ie = stage_inside(child);
+                for (int c = 0; c < nc; c++) {
+                    const double *Pr = PT + (size_t)c * 4096;
+                    const double sum = block_sum(A * apply(child, [&](int j) { return Pr[j * 64 + k]; }));
+                    if (k == 0) rows[r0 + c] = pattern_lnl(sum, ae + ie, [] {});
+                }
             }
-            if (child >= a.L) {                  // O_child[k] = sum_p A[p] P[p][k] = sum_p A[p] PT[k][p]
+            // sum_p A[p] P[p][k] = sum_p A[p] PT[k][p]: an internal child's outside vector, a leaf child's u
+            auto through = [&]() {
                 double wc[4];
-                mix_weights(wc, mw + r0, nc);
+                load_weights(wc, r0, nc);
                 broadcast(A);
                 double o = 0.0;
                 if (live)
-                    for (int p = 0; p < a.D; p++)
-                        o = fma(xs[p], mix_entry(wc, nc, [&](int c) { return PT[k * 64 + p + (size_t)c * 4096]; }), o);
+                    for (int p = 0; p < a.D; p++) {
+                        if constexpr (MIX) o = fma(xs[p], mix_entry(wc, nc, [&](int c) { return PT[k * 64 + p + (size_t)c * 4096]; }), o);
+                        else o = fma(xs[p], PT[k * 64 + p], o);
+                    }
+                return o;
+            };
+            if (child >= a.L) {
+                double o = through();
                 renorm(o, ae);
                 side[(size_t)child * 64 + k] = o;
                 if (k == 0) side_ex[child] = ae;
+            } else if constexpr (EMIT == OutsideEmit::LeafSupport) {
+                const double u = through(), total = block_sum(u);
+                if (live) g.support[((size_t)s * a.L + child) * a.D + k] = total != 0.0 && isfinite(total) ? u / total : nan("");
             }
             v *= msg[(size_t)child * 64 + k];
             ve += msg_ex[child];
@@ -1852,6 +1886,14 @@ __global__ void __launch_bounds__(64) branch_rows_kernel(BranchRowsArgs g) {
         }
     }
 }
+
+__global__ void __launch_bounds__(64) branch_rows_kernel(OutsideArgs g) { outside_pass<OutsideEmit::BranchRows, true>(g); }
+
+// A minimum of 8 CTAs per SM (a chunk of at most 1024 sets puts no more on any of the 132 SMs) lets ptxas use 79-88
+// registers instead of 44-46; on one H100 at 700 W the kernel then took 22 / 60 / 38 ms instead of 29 / 79 / 52 ms on the
+// north-star FEL / MEME-all / MEME-third shapes (tools/bench_leaf_support.py, alternating runs, identical output).
+template <bool MIX>
+__global__ void __launch_bounds__(64, 8) leaf_support_kernel(OutsideArgs g) { outside_pass<OutsideEmit::LeafSupport, MIX>(g); }
 
 // ------------------------------------------------------------------------------------------------
 // prune_rates_kernel (hb2_batch_site_rates): prune_batch_kernel<false>'s recursion for 4..32 padded states.  A group of

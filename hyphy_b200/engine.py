@@ -46,6 +46,7 @@ ABI = [
     ("hb2_batch_site_mixture_likelihoods", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, C.c_int64, _ip, _dp, _dp, _ip, _dp, _dp]),
     ("hb2_batch_branch_component_likelihoods", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, C.c_int64, _ip, _dp, _dp, _ip,
                                                          _dp, _dp, _dp]),
+    ("hb2_batch_leaf_support", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, C.c_int64, _ip, _dp, _dp, _ip, _dp, _dp, _dp]),
     ("hb2_batch_column_likelihoods", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, C.c_int64, _ip, _dp, _dp, _ip, _dp, _dp]),
     ("hb2_batch_site_rates", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, _dp, _dp, _dp]),
     ("hb2_read_conditionals", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _dp, _i32p]),
@@ -300,6 +301,20 @@ class Partition:
         _check(self._lib.hb2_batch_branch_component_likelihoods(self._h, int(template), len(po), ppo, K, pbk, pv, pw, pbg, ppi,
                                                                 site.ctypes.data_as(_dp), rows.ctypes.data_as(_dp)))
         return site, rows
+
+    def batch_leaf_support(self, pattern_of, formula_values, root_freqs, weights=None, branch_k=None, branch_group=None,
+                           template=0, want_site=False):
+        """Leaf state imputation (hb2_batch_leaf_support): sets as batch_column_likelihoods on partition patterns.  Returns
+        support [nSets, L, D], row l of a set being the distribution of leaf l's state given every other leaf; with
+        want_site also the nSets site log-likelihoods, as (support, site_lnl)."""
+        po, ppo = _i(pattern_of)
+        K, pbk, pv, pw, pbg, keep = self._batch_rows(len(po), formula_values, weights, branch_k, branch_group)
+        pi, ppi = _d(root_freqs)
+        site = np.empty(len(po)) if want_site else None
+        sup = np.empty((len(po), self.L, self.D))
+        _check(self._lib.hb2_batch_leaf_support(self._h, int(template), len(po), ppo, K, pbk, pv, pw, pbg, ppi,
+                                                site.ctypes.data_as(_dp) if want_site else None, sup.ctypes.data_as(_dp)))
+        return (sup, site) if want_site else sup
 
     def _batch_rows(self, n_sets, formula_values, weights, branch_k, branch_group):
         """Checked arguments of the batch entry points that take both set layouts: weights None means one row per branch

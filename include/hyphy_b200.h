@@ -198,6 +198,35 @@ int hb2_batch_branch_component_likelihoods(hb2_partition *p, int64_t templateId,
                                            const double *weights, const int64_t *branchGroup, const double *rootFreqs,
                                            double *siteLnL, double *rowLnL);
 
+/* Leaf state imputation for MEME and PRIME (--impute-states, MEME.bf:1382-1412, PRIME.bf:940-960): what
+ * ReconstructAncestors(lf_site, {{0}}, MARGINAL, DOLEAVES) reports for every leaf of a site, for every set in one call.
+ * The reference evaluates the site with leaf l forced to each state k (setBranchTo replaces the leaf's observation, so its
+ * state or ambiguity is not used, tree_evaluator.cpp:173-181), divides by the site likelihood and normalises over k
+ * (_LikelihoodFunction::RecoverAncestralSequencesMarginal, likefunc2.cpp:974-1006 and :1083-1093): the row of leaf l is the
+ * predictive distribution of l's state given every other leaf, not the posterior given all the data.
+ * Sets as hb2_batch_column_likelihoods, on partition patterns: weights == NULL gives one row per branch, formulaValues
+ * [nSets][B][nFormulas] as hb2_batch_site_likelihoods (K must be 1 and branchK NULL; PRIME's and FEL's site models);
+ * otherwise rows, weights, K and branchK as hb2_batch_site_mixture_likelihoods (MEME's lf_bsrel).  Outputs:
+ *   support  [nSets][L][D]: support[s][l][k] = u[k] / sum_j u[j] with u[k] = sum_p A_l[p] P_l[p][k], A_l the vector at the
+ *            parent end of leaf l's branch of everything outside l (the batch outside pass of
+ *            hb2_batch_branch_component_likelihoods) and P_l l's transition matrix, mixed as the batch pruning mixes it.
+ *            Flat leaf ids, states 0..D-1 (not padded).  A leaf's row does not depend on that leaf's own code; rows sum
+ *            to 1 up to rounding; a row whose total sum_j u[j] is 0 or not finite is NaN in every entry (the reference
+ *            gives NaN there too, likefunc2.cpp:1084-1086).
+ *   siteLnL  nullable [nSets]: bit for bit what hb2_batch_site_likelihoods (weights == NULL) or
+ *            hb2_batch_site_mixture_likelihoods returns for the same arguments (the same inside pass).
+ * Plain sets give, bit for bit, the support of the mixture layout with one component of weight 1.0 per branch.  A NaN
+ * weight or formula value gives NaN for its own set only.  fp64 throughout, every outside vector renormalised by exact
+ * powers of two.
+ * Refusals before anything is launched or written (the partition stays usable): everything the corresponding likelihood
+ * entry point refuses; support == NULL; K != 1 or a non-NULL branchK without weights.  nSets == 0 after these checks does
+ * nothing.  33..64 states only; not available in class-group mode.
+ * Nothing an evaluation reads is touched: conditionals, scalers, walk plans and tags, the branch cache, the staged root
+ * vector, the P cache and the resident rate matrices. */
+int hb2_batch_leaf_support(hb2_partition *p, int64_t templateId, int64_t nSets, const int64_t *patternOf,
+                           int64_t K, const int64_t *branchK, const double *formulaValues, const double *weights,
+                           const int64_t *branchGroup, const double *rootFreqs, double *siteLnL, double *support);
+
 /* The batch likelihoods of caller-given columns instead of partition patterns (the refits of a parametric bootstrap score
  * columns simulated by hb2_batch_site_simulate, which are not patterns of the partition): set s scores
  * columns[s][0..L-1], in hb2_create's leafState codes (>= 0: a state < D; < 0: ambiguity row -(code+1) < nAmb).

@@ -7,7 +7,9 @@ alignment order) plus a checksum of the generated leaf states, so tests can prov
 with (the final lnL of an evaluation stream, joint ML ancestral sequences).
 `--pinned` writes tests/golden/bsrel_12x80_k3_pinned.npz: MEME's branch-level empirical Bayes procedure
 (meme.compute_branch_EBF, MEME.bf:886-944) on every site at once -- see pinned_fixture.
-Run where the reference binary was built:  python tools/make_golden.py [--runs | --pinned | name ...]
+`--impute` writes tests/golden/<case>_impute.npz for IMPUTE_CASES: leaf state imputation
+(ReconstructAncestors(MARGINAL, DOLEAVES), MEME's and PRIME's --impute-states) on every site -- see impute_fixture.
+Run where the reference binary was built:  python tools/make_golden.py [--runs | --pinned | --impute | name ...]
 """
 import hashlib
 import json
@@ -115,6 +117,67 @@ def pinned_fixture(out):
     print(f"{PINNED_CASE}_pinned: lnL={lnL!r} rows={nb * K} sites={n}", flush=True)
 
 
+IMPUTE_CASES = ["bsrel_12x80_k3", "mg94_8x60_c1"]     # mixture layout (K = 3 on every branch), plain layout
+
+
+def impute_script(w, path_bf, path_fas):
+    """The case's script of ref_harness.write_hbl, followed by the marginal reconstruction of the leaves and its support
+    matrix: `NAMES` the reconstructed data set's sequence names (the matrix's row order), `DUP` the filter's
+    site-to-pattern map, then one `SUP leaf` line per matrix row with its patterns x D entries (pattern-major)."""
+    rh.write_hbl(w, path_bf, path_fas, per_site=False)
+    lines = ["DataSet anc = ReconstructAncestors (lf, {{0}}, MARGINAL, DOLEAVES);",
+             "sm = anc.marginal_support_matrix;",
+             "GetString (nms, anc, -1);",
+             'for (k = 0; k < Columns (nms); k += 1) { fprintf (stdout, "NAMES ", k, " ", nms[k], "\n"); }',
+             "GetDataInfo (dup, flt);",
+             'fprintf (stdout, "DUP");',
+             'for (k = 0; k < Columns (dup); k += 1) { fprintf (stdout, " ", dup[k]); }',
+             'fprintf (stdout, "\n");',
+             "for (r = 0; r < Rows (sm); r += 1) {",
+             '  fprintf (stdout, "SUP ", r);',
+             '  for (c = 0; c < Columns (sm); c += 1) { fprintf (stdout, " ", Format (sm[r][c], 50, 30)); }',
+             '  fprintf (stdout, "\n");',
+             "}"]
+    with open(path_bf, "a") as f:
+        f.write("\n".join(lines) + "\n")
+
+
+def impute_fixture(out, name):
+    """tests/golden/<name>_impute.npz: lnL, and support [sites][L][D] -- row l of a site is the reference's support of
+    leaf l (flat id, mapped by name) at that site's pattern of the filter (mapped by the filter's site-to-pattern map)."""
+    w = CASES[name]()
+    L, D, n = w.tree.n_leaves, w.D, len(w.site_to_pattern)
+    tmp = tempfile.mkdtemp(prefix="hb2ref_")
+    bf, fas = os.path.join(tmp, "job.bf"), os.path.join(tmp, "job.fas")
+    impute_script(w, bf, fas)
+    proc = subprocess.run([rh.REF_BIN, "CPU=1", bf], cwd=tmp, stdin=subprocess.DEVNULL, capture_output=True, text=True, check=True)
+    lnL, names, dup, rows = None, {}, None, {}
+    for line in proc.stdout.splitlines():
+        f = line.split()
+        if line.startswith("LNL="):
+            lnL = float(line[4:])
+        elif f and f[0] == "NAMES":
+            names[int(f[1])] = f[2]
+        elif f and f[0] == "DUP":
+            dup = np.array([int(x) for x in f[1:]], dtype=np.int64)
+        elif f and f[0] == "SUP":
+            rows[int(f[1])] = np.array([float(x) for x in f[2:]])
+    assert lnL is not None and dup is not None and len(dup) == n and len(rows) == L == len(names), proc.stdout[-2000:]
+    n_pat = int(dup.max()) + 1
+    leaf_of = {nm: l for l, nm in enumerate(w.tree.names[:L])}
+    support = np.full((n, L, D), np.nan)
+    for r, row in rows.items():
+        assert row.shape == (n_pat * D,)
+        support[:, leaf_of[names[r]], :] = row.reshape(n_pat, D)[dup]
+    assert not np.isnan(support).any()
+    for p in range(w.S):                        # sites of one pattern of the engine's compression share their rows
+        sites = np.nonzero(w.site_to_pattern == p)[0]
+        assert np.all(support[sites] == support[sites[:1]]), p
+    np.savez_compressed(os.path.join(out, name + "_impute.npz"), lnL=np.float64(lnL), support=support,
+                        checksum=np.array(checksum(w)), S=np.int64(w.S), sites=np.int64(n))
+    print(f"{name}_impute: lnL={lnL!r} leaves={L} sites={n} filter patterns={n_pat}", flush=True)
+
+
 def main():
     out = os.path.join(ROOT, "tests", "golden")
     os.makedirs(out, exist_ok=True)
@@ -124,6 +187,10 @@ def main():
         return
     if only == ["--pinned"]:
         pinned_fixture(out)
+        return
+    if only == ["--impute"]:
+        for name in IMPUTE_CASES:
+            impute_fixture(out, name)
         return
     for name, make in CASES.items():
         if only and name not in only:
