@@ -1403,6 +1403,10 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
     if (nAmb > 0 && !ambig) return fail("nAmb > 0 but ambig is null");
     const int Dp = pad_states(D);
     if (Dp < 0) return fail("state count %lld not supported (max 64)", (long long)D);
+    // the kernels sum an ambiguity row's allowed states with the row's weight, which is the reference's only for 0/1 rows
+    for (int64_t i = 0; i < nAmb * D; i++)
+        if (ambig[i] != 0.0 && ambig[i] != 1.0)
+            return fail("ambiguity row %lld, state %lld: weight %g is neither 0 nor 1", (long long)(i / D), (long long)(i % D), ambig[i]);
     int ndev = hb2_device_count();
     if (ndev <= 0) return fail("no CUDA device visible: the engine has no CPU fallback");
     if (device < 0 || device >= ndev) return fail("device %d out of range (%d visible)", device, ndev);
@@ -1853,6 +1857,18 @@ static BatchShape rates_shape(const hb2_partition *p, const BatchCall &c) {
     return sh;
 }
 
+// The chunk's inside-pass arguments over the batch workspace: set s prunes pattern pat[s] of leaf[L][Sp]; R component rows
+// per set (mixtures only).
+static hb2::BatchPruneArgs batch_prune_args(const hb2_partition *p, const int *leaf, int Sp, int R) {
+    const hb2_partition::BatchWorkspace &ws = p->batch;
+    hb2::BatchPruneArgs ba{};
+    ba.PT = ws.PT; ba.cond = ws.cond; ba.node_ex = ws.node_ex; ba.pat = ws.pat; ba.leaf = leaf; ba.ambig = p->d_ambig;
+    ba.pi = ws.pi; ba.tree.child_start = p->d_child_start; ba.tree.child_ids = p->d_child_ids; ba.out = ws.out;
+    ba.L = (int)p->L; ba.I = (int)p->I; ba.B = (int)p->B; ba.D = (int)p->D; ba.Sp = Sp;
+    ba.mix_w = ws.mixw; ba.row_off = ws.row; ba.R = R;
+    return ba;
+}
+
 extern "C++" template <int DP>
 void launch_rates(hb2_partition *p, const BatchCall &c, int64_t nb) {
     hb2_partition::BatchWorkspace &ws = p->batch;
@@ -1861,10 +1877,7 @@ void launch_rates(hb2_partition *p, const BatchCall &c, int64_t nb) {
     ea.D = (int)p->D; ea.B = (int)p->B; ea.n = (long long)nb * p->B;
     constexpr int M = 128 / hb2::expm_rates_team(DP);
     hb2::expm_rates_kernel<DP><<<(unsigned)((ea.n + M - 1) / M), 128, hb2::expm_rates_smem_bytes(DP), p->stream>>>(ea);
-    hb2::BatchPruneArgs ba{};
-    ba.PT = ws.PT; ba.cond = ws.cond; ba.node_ex = ws.node_ex; ba.pat = ws.pat; ba.ambig = p->d_ambig; ba.pi = ws.pi;
-    ba.leaf = p->d_leaf; ba.tree.child_start = p->d_child_start; ba.tree.child_ids = p->d_child_ids; ba.out = ws.out;
-    ba.L = (int)p->L; ba.I = (int)p->I; ba.B = (int)p->B; ba.D = (int)p->D; ba.Sp = (int)p->Sp;
+    const hb2::BatchPruneArgs ba = batch_prune_args(p, p->d_leaf, (int)p->Sp, 0);
     constexpr int per_block = 128 / (DP <= 16 ? DP : 32);
     hb2::prune_rates_kernel<DP><<<(unsigned)((nb + per_block - 1) / per_block), 128, 0, p->stream>>>(ba, (int)nb);
 }
@@ -1925,12 +1938,8 @@ static int score_chunk(hb2_partition *p, const BatchCall &c, const BatchShape &s
             for (int64_t l = 0; l < L; l++) ws.h_col[l * nb + s] = (int)c.columns[(s0 + s) * L + l];
         CU(cudaMemcpyAsync(ws.col, ws.h_col, (size_t)L * nb * sizeof(int), cudaMemcpyHostToDevice, p->stream));
     }
-    hb2::BatchPruneArgs ba;
-    ba.PT = ws.PT; ba.cond = ws.cond; ba.node_ex = ws.node_ex; ba.pat = ws.pat; ba.ambig = p->d_ambig; ba.pi = ws.pi;
-    ba.leaf = c.columns ? (const int *)ws.col : (const int *)p->d_leaf;
-    ba.tree.child_start = p->d_child_start; ba.tree.child_ids = p->d_child_ids; ba.out = ws.out;
-    ba.L = (int)L; ba.I = (int)p->I; ba.B = (int)p->B; ba.D = (int)p->D; ba.Sp = c.columns ? (int)nb : (int)p->Sp;
-    ba.mix_w = ws.mixw; ba.row_off = ws.row; ba.R = (int)sh.R;
+    const hb2::BatchPruneArgs ba = batch_prune_args(p, c.columns ? (const int *)ws.col : (const int *)p->d_leaf,
+                                                    c.columns ? (int)nb : (int)p->Sp, (int)sh.R);
     if (c.weights) hb2::prune_batch_kernel<true><<<(unsigned)nb, 64, 0, p->stream>>>(ba);
     else hb2::prune_batch_kernel<false><<<(unsigned)nb, 64, 0, p->stream>>>(ba);
     p->launches++;

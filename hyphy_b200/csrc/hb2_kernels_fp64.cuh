@@ -1357,6 +1357,104 @@ __global__ void __launch_bounds__(256) combine_kernel(CombineArgs a) {
 }
 
 // ------------------------------------------------------------------------------------------------
+// Group toolkit of the state-per-thread fp64 kernels (bc_path_kernel, prune_batch_kernel, outside_pass, prune_rates_kernel):
+// a group of G = 4, 8, 16, 32 or 64 threads owns one pattern and thread k owns state k.  G = 64 is a CTA of two warps and
+// exchanges through the kernel's shared scratch xs[64] and red[2]; G <= 32 is the lanes `mask` of one warp and exchanges
+// with width-G shuffles.  Every member is called by the whole group.
+// Numerical rules of these kernels:
+//   - Renormalisation: a vector whose group maximum m is positive and below `below` is multiplied by 2^-e, e = ilogb(m) + 1,
+//     which brings m to [0.5, 1), and e is added to its binary exponent.  The multiply is split in two exact halves so that
+//     neither factor overflows when m is subnormal.  A pruned node renormalises at its end (below = INFINITY) and, from its
+//     third child on, before each child with below = RESCALE_BELOW (the wide-node rescale); the outside passes renormalise
+//     after every factor.
+//   - Child message m[k] = sum_j P[k][j] x_j = sum_j x_j PT[j][k] over the states j < D in order, one fma per state (dot):
+//     x is an internal child's vector staged to the group.  A leaf gives m = PT[code][k] for a state, or for a 0/1
+//     ambiguity row the fma of the row's weight over its nonzero states in order (leaf_message; hb2_create refuses any
+//     other weight, so this equals the sum of those entries).  The outside product o[k] = sum_p A_p P[p][k] is the same
+//     dot over a row of the transposed table, PT[k][p].  Entries are read through the caller's entry(j): plain, mixed by
+//     mix_entry (BranchP), or a Dp-strided table.
+//   - Padded states (k >= D) stay 0: their table entries are 0, or the kernel masks them (dot's `live`).
+//   - The group sum is one fixed-order xor tree of width G; G = 64 adds the totals of its two warps, red[0] + red[1].  A
+//     pattern's sum * 2^ex goes out through pattern_lnl: a likelihood of 0 gives -inf and NaN stays NaN.
+// ------------------------------------------------------------------------------------------------
+template <int G>
+struct Group {
+    static_assert(G == 4 || G == 8 || G == 16 || G == 32 || G == 64, "a group is 4, 8, 16, 32 or 64 threads");
+    static constexpr int W = G < 32 ? G : 32;    // shuffle width
+    double *xs, *red;                            // G = 64: the kernel's shared xs[64] and red[2]
+    unsigned mask;                               // the group's lanes (G >= 32: every lane)
+    int k;                                       // this thread's state
+
+    __device__ __forceinline__ double max(double v) const {
+#pragma unroll
+        for (int o = W / 2; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(mask, v, o, W));
+        if constexpr (G == 64) {
+            __syncthreads();
+            if ((k & 31) == 0) red[k >> 5] = v;
+            __syncthreads();
+            v = fmax(red[0], red[1]);
+        }
+        return v;
+    }
+    __device__ __forceinline__ double sum(double v) const {
+#pragma unroll
+        for (int o = W / 2; o > 0; o >>= 1) v += __shfl_xor_sync(mask, v, o, W);
+        if constexpr (G == 64) {
+            __syncthreads();
+            if ((k & 31) == 0) red[k >> 5] = v;
+            __syncthreads();
+            v = red[0] + red[1];
+        }
+        return v;
+    }
+    __device__ __forceinline__ void renorm(double &v, int &ex, double below = INFINITY) const {
+        const double m = max(v);
+        if (m > 0.0 && m < below) {
+            const int e = ilogb(m) + 1;
+            v = v * exp2i(-(e / 2)) * exp2i(-(e - e / 2));
+            ex += e;
+        }
+    }
+    // Makes this thread's x readable by the group as x_j = at(staged, j).
+    __device__ __forceinline__ double stage(double x) const {
+        if constexpr (G == 64) {
+            __syncthreads();                     // xs free
+            xs[k] = x;
+            __syncthreads();
+        }
+        return x;
+    }
+    __device__ __forceinline__ double at(double staged, int j) const {
+        if constexpr (G == 64) return xs[j];
+        else return __shfl_sync(mask, staged, j, G);
+    }
+    // sum_j x_j entry(j) over j < D for a staged x: an internal child's message, or the outside product.  A thread that is
+    // not `live` reads no entry and returns 0 (or NaN for a non-finite x when G <= 32: its lanes take part in the shuffles).
+    template <typename Entry>
+    __device__ __forceinline__ double dot(double staged, int D, bool live, Entry entry) const {
+        double m = 0.0;
+        if constexpr (G == 64) {
+            if (live)
+                for (int j = 0; j < D; j++) m = fma(at(staged, j), entry(j), m);
+        } else {
+            for (int j = 0; j < D; j++) m = fma(at(staged, j), live ? entry(j) : 0.0, m);
+        }
+        return m;
+    }
+    // the message of a leaf child with state code `code`: a state (>= 0) or row -code - 1 of ambig[][stride]
+    template <typename Entry>
+    __device__ __forceinline__ double leaf_message(int code, const double *ambig, int stride, int D, Entry entry) const {
+        double m = 0.0;
+        if (code >= 0) m = entry(code);
+        else {
+            const double *amb = ambig + (size_t)(-code - 1) * stride;
+            for (int j = 0; j < D; j++) { const double w = amb[j]; if (w != 0.0) m = fma(w, entry(j), m); }
+        }
+        return m;
+    }
+};
+
+// ------------------------------------------------------------------------------------------------
 // Single-branch shortcut (reference: ComputeBranchCache tree_evaluator.cpp:4286, ComputeLLWithBranchCache tree.cpp:3383).
 // For a branch b with parent u the likelihood factorises as  L_s = sum_a rest_b[s][a] * (P_b * below_b[s])[a]  where
 // below_b = conditionals of b's subtree (already resident) and rest_b[s][a] = everything else, seen from state a at u:
@@ -1420,24 +1518,10 @@ __device__ __forceinline__ void bc_message(const BranchCacheArgs &a, int cat, in
     }
 }
 
-__device__ __forceinline__ void bc_renorm(double *v, int D, int &e) {
-    double m = 0.0;
-    for (int q = 0; q < D; q++) m = fmax(m, v[q]);
-    if (m > 0.0 && m < INFINITY) {
-        int ex;
-        frexp(m, &ex);
-        if (ex != 0) {
-            const double sc = exp2i(-ex);
-            for (int q = 0; q < D; q++) v[q] *= sc;
-            e += ex;
-        }
-    }
-}
-
-// The whole root -> parent(b) path in ONE launch: one CTA of Dp' = 64 (or 32) threads per (class, pattern), thread q owns
-// state q; vectors are exchanged through shared memory and a matrix column / row is read with consecutive threads on
-// consecutive addresses (the transposed table serves messages, its rows serve the outside propagation).  Replaces one
-// launch of bc_step_kernel per path node with a serial thread per pattern.
+// The whole root -> parent(b) path in ONE launch: one CTA of Dp' = 64 (or 32) threads per (class, pattern), a Group of
+// thread q = state q; a matrix column / row is read with consecutive threads on consecutive addresses (the transposed table
+// serves messages, its rows serve the outside propagation).  The rules are the group toolkit's, every factor
+// renormalised.  Replaces one launch of bc_step_kernel per path node with a serial thread per pattern.
 //   path[i]      internal index of the i-th path node (root first), npath nodes
 //   sib_off[i]   range of its non-path children in sib[]
 //   down[i]      flat id of the path child below path[i] (the next path node), -1 for the last (whose child is the branch b)
@@ -1451,60 +1535,30 @@ __global__ void __launch_bounds__(NT) bc_path_kernel(BranchCacheArgs a, BranchPa
     __shared__ double xs[64];
     __shared__ double red[2];
     const int s = blockIdx.x, cat = a.cat0 + blockIdx.y, q = threadIdx.x;
+    const Group<NT> grp{xs, red, 0xffffffffu, q};
     const bool live = q < a.D;
     double r = live ? a.pi[q] : 0.0;             // out_root = pi
     int e = 0;
-    auto block_max = [&](double v) -> double {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
-        if (NT > 32) {
-            __syncthreads();
-            if ((q & 31) == 0) red[q >> 5] = v;
-            __syncthreads();
-            v = fmax(red[0], red[1]);
-        }
-        return v;
-    };
-    auto renorm = [&](double &v) {
-        const double m = block_max(v);
-        if (m > 0.0 && m < INFINITY) {
-            int ex;
-            frexp(m, &ex);
-            if (ex != 0) { v *= exp2i(-(ex / 2)) * exp2i(-(ex - ex / 2)); e += ex; }
-        }
-    };
     for (int i = 0; i < bp.npath; i++) {
         for (int ci = bp.sib_off[i]; ci < bp.sib_off[i + 1]; ci++) {          // rest = out_u * prod over siblings (P_c L_c)
             const int ch = bp.sib[ci];
             const double *PTc = a.PT + ((size_t)cat * a.B + ch) * a.Dp * a.Dp;
+            auto entry = [&](int k) { return PTc[(size_t)k * a.Dp + q]; };
             double m = 0.0;
             if (ch < a.L) {
-                const int code = a.leaf[(size_t)ch * a.Sp + s];
-                if (code >= 0) m = live ? PTc[(size_t)code * a.Dp + q] : 0.0;
-                else {
-                    const double *amb = a.ambig + (size_t)(-code - 1) * a.Dp;
-                    for (int k = 0; k < a.D; k++) if (amb[k] != 0.0 && live) m += PTc[(size_t)k * a.Dp + q];
-                }
+                if (live) m = grp.leaf_message(a.leaf[(size_t)ch * a.Sp + s], a.ambig, a.Dp, a.D, entry);
             } else {
                 const int cin = ch - a.L;
-                __syncthreads();
-                if (q < a.Dp) xs[q] = live ? cond_at(a.cv, cat, cin, s, q) : 0.0;
-                __syncthreads();
-                if (live) for (int k = 0; k < a.D; k++) m = fma(xs[k], PTc[(size_t)k * a.Dp + q], m);
+                m = grp.dot(grp.stage(live ? cond_at(a.cv, cat, cin, s, q) : 0.0), a.D, live, entry);
                 e += exp_at(a.cv, cat, cin, s);
             }
             r *= m;
-            renorm(r);
+            grp.renorm(r, e);
         }
         if (bp.down[i] >= 0) {                                                  // out'[q] = sum_k rest[k] * P_down[k][q] = sum_k r[k] PT[q][k]
             const double *PTd = a.PT + ((size_t)cat * a.B + bp.down[i]) * a.Dp * a.Dp;
-            __syncthreads();
-            if (q < a.Dp) xs[q] = r;
-            __syncthreads();
-            double acc = 0.0;
-            if (live) for (int k = 0; k < a.D; k++) acc = fma(xs[k], PTd[(size_t)q * a.Dp + k], acc);
-            r = acc;
-            renorm(r);
+            r = grp.dot(grp.stage(r), a.D, live, [&](int k) { return PTd[(size_t)q * a.Dp + k]; });
+            grp.renorm(r, e);
         }
     }
     if (q < a.Dp) a.out[((size_t)cat * a.Sp + s) * a.Dp + q] = r;
@@ -1582,7 +1636,7 @@ __global__ void __launch_bounds__(256) class_merge_kernel(const double *gath, co
 // functions on the same tree, FEL.bf:1180-1233, MEME.bf:699-746).  Set s prunes pattern pat[s] with ITS OWN transition
 // matrices PT[s][b] (64-padded, transposed, as the expm kernels write them).  One CTA of 64 threads per set: thread k owns
 // parent state k; a child's vector is broadcast from shared memory and column k of P is read from PT[.][j][k] -- 64
-// consecutive doubles per j, coalesced.  fp64 throughout; per-node power-of-two renormalisation like the main kernels.
+// consecutive doubles per j, coalesced.  fp64 throughout, a Group<64> under the group toolkit's rules.
 // Internal-node vectors live in global scratch cond[s][I][64] (L1/L2 resident: 512 bytes per node).
 // MIX (explicit-form mixtures, MEME's tested branches, MEME.bf:381-386): set s holds R component matrices PT[s][row];
 // branch b mixes rows row_off[b] .. row_off[b+1]-1 (at most 4).  The thread of parent state k forms each entry as
@@ -1622,79 +1676,68 @@ struct BatchPruneArgs {
     int R;                    // MIX: component rows per set
 };
 
+// The transition matrix of a child's branch in a set's P area PTs, as prune_batch_kernel and outside_pass read it: P is
+// the branch's first row, nc its component rows from row r0 (one without MIX), w their weights once load_weights() ran.
+// Entry (j, k), at offset j * 64 + k of the table, is the row's entry, or with MIX the rows' mix_entry.
+template <bool MIX>
+struct BranchP {
+    const double *P;
+    int r0, nc;
+    double w[4];
+    __device__ __forceinline__ BranchP(const BatchPruneArgs &a, const double *PTs, int child) {
+        if constexpr (MIX) { r0 = a.row_off[child]; nc = a.row_off[child + 1] - r0; }
+        else { r0 = child; nc = 1; }
+        P = PTs + (size_t)r0 * 4096;
+    }
+    // mw: the set's weights; the same address in every thread, a broadcast
+    __device__ __forceinline__ void load_weights(const double *mw) {
+        if constexpr (MIX) mix_weights(w, mw + r0, nc);
+    }
+    __device__ __forceinline__ double operator()(int off) const {
+        if constexpr (!MIX) return P[off];
+        else return mix_entry(w, nc, [&](int c) { return P[off + (size_t)c * 4096]; });
+    }
+};
+
+// Each node follows the group toolkit's rules; the root sum is Group<64>::sum.
 template <bool MIX>
 __global__ void __launch_bounds__(64) prune_batch_kernel(BatchPruneArgs a) {
     __shared__ double xs[64];
     __shared__ double red[2];
     const int s = blockIdx.x, k = threadIdx.x;
+    const Group<64> grp{xs, red, 0xffffffffu, k};
     const int pattern = a.pat[s];
     const double *PTs = a.PT + (size_t)s * (MIX ? a.R : a.B) * 4096;
+    const double *mw = MIX ? a.mix_w + (size_t)s * a.R : nullptr;
     double *cs = a.cond + (size_t)s * a.I * 64;
     int *node_ex = a.node_ex + (size_t)s * a.I;
     for (int par = 0; par < a.I; par++) {
         double v = k < a.D ? 1.0 : 0.0;
         int ex = 0;
-        // max over the 64 threads; if it lies below `below`, an exact power of two brings it to [0.5, 1)
-        auto renorm = [&](double below) {
-            double mx = v;
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-            __syncthreads();
-            if ((k & 31) == 0) red[k >> 5] = mx;
-            __syncthreads();
-            mx = fmax(red[0], red[1]);
-            if (mx > 0.0 && mx < below) {
-                const int e = ilogb(mx) + 1;
-                v = v * exp2i(-(e / 2)) * exp2i(-(e - e / 2));
-                ex += e;
-            }
-        };
         const int c_begin = a.tree.child_start[par], c_end = a.tree.child_start[par + 1];
         for (int ci = c_begin; ci < c_end; ci++) {
-            if (ci - c_begin >= 2) renorm(RESCALE_BELOW);       // wide node: keep the running product normal
+            if (ci - c_begin >= 2) grp.renorm(v, ex, RESCALE_BELOW);
             const int child = a.tree.child_ids[ci];
-            const double *PT = PTs + (size_t)(MIX ? a.row_off[child] : child) * 4096;
-            // entry (j, k) of the branch's transition matrix
-            double wc[4];
-            int nc = 1;
-            if constexpr (MIX) {
-                const int r0 = a.row_off[child];
-                nc = a.row_off[child + 1] - r0;
-                mix_weights(wc, a.mix_w + (size_t)s * a.R + r0, nc);   // same address in every thread: a broadcast
-            }
-            auto entry = [&](int j) {
-                if constexpr (!MIX) return PT[j * 64 + k];
-                else return mix_entry(wc, nc, [&](int c) { return PT[j * 64 + k + (size_t)c * 4096]; });
-            };
-            double m = 0.0;
-            if (child < a.L) {
-                const int code = a.leaf[(size_t)child * a.Sp + pattern];
-                if (code >= 0) m = entry(code);
-                else {
-                    const double *amb = a.ambig + (size_t)(-code - 1) * 64;
-                    for (int j = 0; j < a.D; j++) { const double w = amb[j]; if (w != 0.0) m = fma(w, entry(j), m); }
-                }
-            } else {
+            BranchP<MIX> P(a, PTs, child);
+            P.load_weights(mw);
+            auto entry = [&](int j) { return P(j * 64 + k); };
+            double m;
+            if (child < a.L) m = grp.leaf_message(a.leaf[(size_t)child * a.Sp + pattern], a.ambig, 64, a.D, entry);
+            else {
                 const int cin = child - a.L;
-                __syncthreads();                 // xs free
-                xs[k] = cs[(size_t)cin * 64 + k];
-                __syncthreads();
-                for (int j = 0; j < a.D; j++) m = fma(xs[j], entry(j), m);
+                m = grp.dot(grp.stage(cs[(size_t)cin * 64 + k]), a.D, true, entry);
                 ex += node_ex[cin];
             }
             v *= m;
         }
-        renorm(INFINITY);                        // end of the node: max -> [0.5, 1)
+        grp.renorm(v, ex);
         cs[(size_t)par * 64 + k] = v;
         if (k == 0) node_ex[par] = ex;
-        __syncthreads();                         // node_ex / cond of this node visible to the block before a parent reads them
         if (par == a.I - 1) {
-            double r = v * a.pi[k];
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) r += __shfl_xor_sync(0xffffffffu, r, o);
-            if ((k & 31) == 0) red[k >> 5] = r;
-            __syncthreads();
-            if (k == 0) a.out[s] = pattern_lnl(red[0] + red[1], ex, [] {});
+            const double r = grp.sum(v * a.pi[k]);
+            if (k == 0) a.out[s] = pattern_lnl(r, ex, [] {});
+        } else {
+            __syncthreads();                     // node_ex of this node visible to the block before a parent reads it
         }
     }
 }
@@ -1721,10 +1764,8 @@ __global__ void __launch_bounds__(64) prune_batch_kernel(BatchPruneArgs a) {
 //      side[c_i] until c_i is visited.  A leaf's u is the same product.
 // The transposed table serves the messages and rows with coalesced reads, as in the inside pass; the outside product reads
 // its rows, as bc_path_kernel does.
-// Numerical rules: every message, suffix, prefix, A and outside vector is brought to max in [0.5, 1) by an exact power of
-// two after each factor, with its binary exponent carried (so the products over the children of a wide node are rescaled
-// between factors, more often than RESCALE_BELOW requires).  A row's sum is encoded by pattern_lnl: a row likelihood of 0
-// gives -inf, and NaN propagates.  Padded states (>= D) stay 0.
+// Numerical rules: the group toolkit's, with every message, suffix, prefix, A and outside vector renormalised after each
+// factor (more often than RESCALE_BELOW requires) and each row's sum encoded by pattern_lnl.
 // ------------------------------------------------------------------------------------------------
 struct OutsideArgs {
     BatchPruneArgs in;        // the chunk's inside pass: PT, cond, node_ex, pat, leaf, ambig, pi, tree (MIX: mix_w, row_off)
@@ -1742,6 +1783,7 @@ __device__ __forceinline__ void outside_pass(const OutsideArgs &g) {
     __shared__ double red[2];
     const BatchPruneArgs &a = g.in;
     const int s = blockIdx.x, k = threadIdx.x;
+    const Group<64> grp{xs, red, 0xffffffffu, k};
     const bool live = k < a.D;
     const int pattern = a.pat[s];
     const double *PTs = a.PT + (size_t)s * (MIX ? a.R : a.B) * 4096;
@@ -1751,78 +1793,22 @@ __device__ __forceinline__ void outside_pass(const OutsideArgs &g) {
     double *msg = g.msg + (size_t)s * a.B * 64, *side = g.side + (size_t)s * a.B * 64;
     int *msg_ex = g.msg_ex + (size_t)s * a.B, *side_ex = g.side_ex + (size_t)s * a.B;
     double *rows = EMIT == OutsideEmit::BranchRows ? g.rows + (size_t)s * a.R : nullptr;
-    // max over the 64 threads; a positive finite maximum is brought to [0.5, 1) by an exact power of two
-    auto renorm = [&](double &v, int &ex) {
-        double mx = v;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-        __syncthreads();
-        if ((k & 31) == 0) red[k >> 5] = mx;
-        __syncthreads();
-        mx = fmax(red[0], red[1]);
-        if (mx > 0.0 && mx < INFINITY) {
-            const int e = ilogb(mx) + 1;
-            v = v * exp2i(-(e / 2)) * exp2i(-(e - e / 2));
-            ex += e;
-        }
-    };
-    auto block_sum = [&](double v) {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        __syncthreads();
-        if ((k & 31) == 0) red[k >> 5] = v;
-        __syncthreads();
-        return red[0] + red[1];
-    };
-    auto broadcast = [&](double v) {             // xs <- v of every thread
-        __syncthreads();
-        xs[k] = v;
-        __syncthreads();
-    };
-    // (P in_child)[k], entry(j) = P[k][j]: a leaf's state or ambiguity row, or the child's vector staged in xs
-    auto apply = [&](int child, auto entry) {
-        double m = 0.0;
-        if (!live) return m;
-        if (child < a.L) {
-            const int code = a.leaf[(size_t)child * a.Sp + pattern];
-            if (code >= 0) m = entry(code);
-            else {
-                const double *amb = a.ambig + (size_t)(-code - 1) * 64;
-                for (int j = 0; j < a.D; j++) { const double w = amb[j]; if (w != 0.0) m = fma(w, entry(j), m); }
-            }
-        } else {
-            for (int j = 0; j < a.D; j++) m = fma(xs[j], entry(j), m);
-        }
-        return m;
-    };
-    auto stage_inside = [&](int child) {        // xs <- in_child of an internal child; its exponent
-        if (child < a.L) return 0;
-        broadcast(cs[(size_t)(child - a.L) * 64 + k]);
-        return node_ex[child - a.L];
-    };
-    // the component rows of a child's branch: its first row of the set's P area and their count
-    auto branch_rows = [&](int child, int &nc) {
-        if constexpr (!MIX) { nc = 1; return child; }
-        else { const int r0 = a.row_off[child]; nc = a.row_off[child + 1] - r0; return r0; }
-    };
-    auto load_weights = [&](double (&wc)[4], int r0, int nc) {
-        if constexpr (MIX) mix_weights(wc, mw + r0, nc);
-    };
     for (int n = a.I - 1; n >= 0; n--) {
         const int c_begin = a.tree.child_start[n], c_end = a.tree.child_start[n + 1];
         // 1. messages
         for (int ci = c_begin; ci < c_end; ci++) {
             const int child = a.tree.child_ids[ci];
-            int nc;
-            const int r0 = branch_rows(child, nc);
-            const double *PT = PTs + (size_t)r0 * 4096;
-            double wc[4];
-            load_weights(wc, r0, nc);
-            int ex = stage_inside(child);
-            double m;
-            if constexpr (MIX) m = apply(child, [&](int j) { return mix_entry(wc, nc, [&](int c) { return PT[j * 64 + k + (size_t)c * 4096]; }); });
-            else m = apply(child, [&](int j) { return PT[j * 64 + k]; });
-            renorm(m, ex);
+            BranchP<MIX> P(a, PTs, child);
+            P.load_weights(mw);
+            const bool leaf = child < a.L;
+            int ex = 0;
+            double x = 0.0;
+            if (!leaf) { x = grp.stage(cs[(size_t)(child - a.L) * 64 + k]); ex = node_ex[child - a.L]; }
+            auto entry = [&](int j) { return P(j * 64 + k); };
+            double m = 0.0;
+            if (!leaf) m = grp.dot(x, a.D, live, entry);
+            else if (live) m = grp.leaf_message(a.leaf[(size_t)child * a.Sp + pattern], a.ambig, 64, a.D, entry);
+            grp.renorm(m, ex);
             msg[(size_t)child * 64 + k] = m;
             if (k == 0) msg_ex[child] = ex;
         }
@@ -1836,7 +1822,7 @@ __device__ __forceinline__ void outside_pass(const OutsideArgs &g) {
             if (k == 0) side_ex[child] = ve;
             v *= msg[(size_t)child * 64 + k];
             ve += msg_ex[child];
-            renorm(v, ve);
+            grp.renorm(v, ve);
         }
         // 3. prefix, A, what is emitted and outside vectors; O_n is the root vector or what the parent's visit left in side[L+n]
         __syncthreads();                         // side_ex visible to the block
@@ -1844,52 +1830,48 @@ __device__ __forceinline__ void outside_pass(const OutsideArgs &g) {
         else { v = side[(size_t)(a.L + n) * 64 + k]; ve = side_ex[a.L + n]; }
         for (int ci = c_begin; ci < c_end; ci++) {
             const int child = a.tree.child_ids[ci];
-            int nc;
-            const int r0 = branch_rows(child, nc);
-            const double *PT = PTs + (size_t)r0 * 4096;
+            BranchP<MIX> P(a, PTs, child);
+            const bool leaf = child < a.L;
             double A = v * side[(size_t)child * 64 + k];
             int ae = ve + side_ex[child];
-            renorm(A, ae);
+            grp.renorm(A, ae);
             if constexpr (EMIT == OutsideEmit::BranchRows) {
-                const int ie = stage_inside(child);
-                for (int c = 0; c < nc; c++) {
-                    const double *Pr = PT + (size_t)c * 4096;
-                    const double sum = block_sum(A * apply(child, [&](int j) { return Pr[j * 64 + k]; }));
-                    if (k == 0) rows[r0 + c] = pattern_lnl(sum, ae + ie, [] {});
+                int ie = 0;
+                double x = 0.0;
+                if (!leaf) { x = grp.stage(cs[(size_t)(child - a.L) * 64 + k]); ie = node_ex[child - a.L]; }
+                for (int c = 0; c < P.nc; c++) {
+                    const double *Pr = P.P + (size_t)c * 4096;
+                    auto entry = [&](int j) { return Pr[j * 64 + k]; };
+                    double m = 0.0;
+                    if (!leaf) m = grp.dot(x, a.D, live, entry);
+                    else if (live) m = grp.leaf_message(a.leaf[(size_t)child * a.Sp + pattern], a.ambig, 64, a.D, entry);
+                    const double sum = grp.sum(A * m);
+                    if (k == 0) rows[P.r0 + c] = pattern_lnl(sum, ae + ie, [] {});
                 }
             }
-            // sum_p A[p] P[p][k] = sum_p A[p] PT[k][p]: an internal child's outside vector, a leaf child's u
-            auto through = [&]() {
-                double wc[4];
-                load_weights(wc, r0, nc);
-                broadcast(A);
-                double o = 0.0;
-                if (live)
-                    for (int p = 0; p < a.D; p++) {
-                        if constexpr (MIX) o = fma(xs[p], mix_entry(wc, nc, [&](int c) { return PT[k * 64 + p + (size_t)c * 4096]; }), o);
-                        else o = fma(xs[p], PT[k * 64 + p], o);
-                    }
-                return o;
-            };
-            if (child >= a.L) {
-                double o = through();
-                renorm(o, ae);
-                side[(size_t)child * 64 + k] = o;
-                if (k == 0) side_ex[child] = ae;
-            } else if constexpr (EMIT == OutsideEmit::LeafSupport) {
-                const double u = through(), total = block_sum(u);
-                if (live) g.support[((size_t)s * a.L + child) * a.D + k] = total != 0.0 && isfinite(total) ? u / total : nan("");
+            if (!leaf || EMIT == OutsideEmit::LeafSupport) {   // the outside product: O_child, or a leaf child's u
+                P.load_weights(mw);
+                const double x = grp.stage(A);
+                double o = grp.dot(x, a.D, live, [&](int p) { return P(k * 64 + p); });
+                if (!leaf) {
+                    grp.renorm(o, ae);
+                    side[(size_t)child * 64 + k] = o;
+                    if (k == 0) side_ex[child] = ae;
+                } else {
+                    const double total = grp.sum(o);
+                    if (live) g.support[((size_t)s * a.L + child) * a.D + k] = total != 0.0 && isfinite(total) ? o / total : nan("");
+                }
             }
             v *= msg[(size_t)child * 64 + k];
             ve += msg_ex[child];
-            renorm(v, ve);
+            grp.renorm(v, ve);
         }
     }
 }
 
 __global__ void __launch_bounds__(64) branch_rows_kernel(OutsideArgs g) { outside_pass<OutsideEmit::BranchRows, true>(g); }
 
-// A minimum of 8 CTAs per SM (a chunk of at most 1024 sets puts no more on any of the 132 SMs) lets ptxas use 79-88
+// A minimum of 8 CTAs per SM (a chunk of at most 1024 sets puts no more on any of the 132 SMs) lets ptxas use 78-80
 // registers instead of 44-46; on one H100 at 700 W the kernel then took 22 / 60 / 38 ms instead of 29 / 79 / 52 ms on the
 // north-star FEL / MEME-all / MEME-third shapes (tools/bench_leaf_support.py, alternating runs, identical output).
 template <bool MIX>
@@ -1900,10 +1882,8 @@ __global__ void __launch_bounds__(64, 8) leaf_support_kernel(OutsideArgs g) { ou
 // G = 4, 8, 16 or 32 lanes owns one set, lane k = parent state k, and 32/G sets share a warp (24 states take G = 32, so
 // a quarter of their lanes idle).  A child's vector is broadcast with width-G shuffles, the node maximum is a group
 // shuffle-max, and node vectors live in global scratch cond[s][I][DP] (each lane reads back only the entry it wrote).
-// Numerical rules as prune_batch_kernel: power-of-two renormalisation of every node to [0.5, 1), the wide-node rescale
-// below RESCALE_BELOW from the third child on, ambiguity sums over the allowed states in state order, pattern_lnl's
-// -inf / NaN encoding.  The root sum differs in order: one xor tree over the G lanes, where prune_batch_kernel adds the
-// totals of two 32-lane trees.
+// Numerical rules: the group toolkit's, as prune_batch_kernel, but its root sum is Group<G>::sum, one xor tree over the G
+// lanes.
 // PT [sets][B][DP*DP], ambig [nAmb][DP], pi [DP]; n = sets of the launch.
 // ------------------------------------------------------------------------------------------------
 template <int DP>
@@ -1913,6 +1893,7 @@ __global__ void __launch_bounds__(128) prune_rates_kernel(BatchPruneArgs a, int 
     const unsigned mask = G == 32 ? 0xffffffffu : ((1u << G) - 1) << (lane / G * G);
     const int s = (int)((blockIdx.x * 128u + threadIdx.x) / G);
     if (s >= n) return;                                  // whole groups
+    const Group<G> grp{nullptr, nullptr, mask, k};
     const bool live = k < DP;
     const int pattern = a.pat[s];
     const double *PTs = a.PT + (size_t)s * a.B * DP * DP;
@@ -1923,46 +1904,27 @@ __global__ void __launch_bounds__(128) prune_rates_kernel(BatchPruneArgs a, int 
     for (int par = 0; par < a.I; par++) {
         v = k < a.D ? 1.0 : 0.0;
         ex = 0;
-        auto renorm = [&](double below) {
-            double mx = v;
-#pragma unroll
-            for (int o = G / 2; o > 0; o >>= 1) mx = fmax(mx, __shfl_xor_sync(mask, mx, o, G));
-            if (mx > 0.0 && mx < below) {
-                const int e = ilogb(mx) + 1;
-                v = v * exp2i(-(e / 2)) * exp2i(-(e - e / 2));
-                ex += e;
-            }
-        };
         const int c_begin = a.tree.child_start[par], c_end = a.tree.child_start[par + 1];
         for (int ci = c_begin; ci < c_end; ci++) {
-            if (ci - c_begin >= 2) renorm(RESCALE_BELOW);
+            if (ci - c_begin >= 2) grp.renorm(v, ex, RESCALE_BELOW);
             const int child = a.tree.child_ids[ci];
             const double *PT = PTs + (size_t)child * DP * DP;
             auto entry = [&](int j) { return live ? PT[j * DP + k] : 0.0; };
-            double m = 0.0;
-            if (child < a.L) {
-                const int code = a.leaf[(size_t)child * a.Sp + pattern];
-                if (code >= 0) m = entry(code);
-                else {
-                    const double *amb = a.ambig + (size_t)(-code - 1) * DP;
-                    for (int j = 0; j < a.D; j++) { const double w = amb[j]; if (w != 0.0) m = fma(w, entry(j), m); }
-                }
-            } else {
+            double m;
+            if (child < a.L) m = grp.leaf_message(a.leaf[(size_t)child * a.Sp + pattern], a.ambig, DP, a.D, entry);
+            else {
                 const int cin = child - a.L;
-                const double x = live ? cs[(size_t)cin * DP + k] : 0.0;
-                for (int j = 0; j < a.D; j++) m = fma(__shfl_sync(mask, x, j, G), entry(j), m);
+                m = grp.dot(grp.stage(live ? cs[(size_t)cin * DP + k] : 0.0), a.D, live, entry);
                 ex += node_ex[cin];
             }
             v *= m;
         }
-        renorm(INFINITY);
+        grp.renorm(v, ex);
         if (live) cs[(size_t)par * DP + k] = v;
         if (k == 0) node_ex[par] = ex;
         __syncwarp(mask);                                // node_ex visible to the group before a parent reads it
     }
-    double r = live ? v * a.pi[k] : 0.0;
-#pragma unroll
-    for (int o = G / 2; o > 0; o >>= 1) r += __shfl_xor_sync(mask, r, o, G);
+    const double r = grp.sum(live ? v * a.pi[k] : 0.0);
     if (k == 0) a.out[s] = pattern_lnl(r, ex, [] {});
 }
 

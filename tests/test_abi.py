@@ -37,6 +37,19 @@ def test_no_cpu_fallback(engine_lib):
         LikelihoodFunction(synth.nucleotide_workload(4, 10))
 
 
+def test_create_refuses_fractional_ambiguity(engine_lib):
+    """Ambiguity rows are 0/1 (the reference's resolution vectors); create refuses any other weight, GPU or not."""
+    import dataclasses
+    import numpy as np
+    from hyphy_b200 import synth, LikelihoodFunction, EngineError
+    w = synth.nucleotide_workload(4, 10)
+    ambig = np.array([[1.0, 1.0, 0.0, 0.0], [1.0, 0.5, 0.0, 1.0]])
+    leaf_states = w.leaf_states.copy()
+    leaf_states[0, 0], leaf_states[1, 0] = -1, -2
+    with pytest.raises(EngineError, match=r"ambiguity row 1, state 1: weight 0.5 is neither 0 nor 1"):
+        LikelihoodFunction(dataclasses.replace(w, ambig=ambig, leaf_states=leaf_states))
+
+
 def test_product_does_not_import_oracle():
     """The oracle is test infrastructure: nothing under hyphy_b200/ may reference it."""
     for dirpath, _, files in os.walk(os.path.join(ROOT, "hyphy_b200")):
