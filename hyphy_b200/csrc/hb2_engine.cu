@@ -22,6 +22,7 @@
 #include <memory>
 #include <mutex>
 #include <unordered_map>
+#include <type_traits>
 #include <utility>
 
 #include <nccl.h>
@@ -45,6 +46,16 @@ int fail(const char *fmt, ...) {
         cudaError_t e_ = (x);                                                                         \
         if (e_ != cudaSuccess) return fail("%s failed: %s (%s:%d)", #x, cudaGetErrorString(e_), __FILE__, __LINE__); \
     } while (0)
+
+// The error of a device-side wait that timed out, from the code it left in the partition's error flag (hb2::WaitCode).
+int wait_timeout(int code) {
+    const char *what = code == hb2::WAIT_TC_STAGING ? "operand staging / tensor pipe"
+                       : code == hb2::WAIT_LANE ? "another lane's conditionals"
+                       : code == hb2::WAIT_PEER ? "a peer rank's partials"
+                       : code == hb2::WAIT_EXPM_POWERS ? "a coefficient matrix of the shared-powers exponential"
+                       : "unknown wait";
+    return fail("a device-side wait timed out (code %d: %s)", code, what);
+}
 
 // ---- Block pool for device and pinned-host memory ----------------------------------------------------------------------
 // The site phases of FEL / MEME create and destroy one small likelihood function per site (SURVEY 8f row 3): through the
@@ -490,6 +501,55 @@ int void_template_cache(hb2_partition *p, int tmpl) {
     return 0;
 }
 
+constexpr int EXPM64_SMEM = 3 * 64 * hb2::LD64 * sizeof(double);    // expm64_dmma_kernel and expm_powers_kernel
+
+// Launch configuration of expm_poly_kernel: `chunks` clusters of EXPM_POLY_CLUSTER row slices (a non-portable size) that
+// share their column sums.
+struct PolyLaunch {
+    cudaLaunchAttribute attr{};
+    cudaLaunchConfig_t cfg{};
+    PolyLaunch(unsigned chunks, cudaStream_t stream) {
+        attr.id = cudaLaunchAttributeClusterDimension;
+        attr.val.clusterDim = {(unsigned)hb2::EXPM_POLY_CLUSTER, 1, 1};
+        cfg.gridDim = dim3(hb2::EXPM_POLY_CLUSTER, chunks); cfg.blockDim = dim3(256); cfg.stream = stream;
+        cfg.attrs = &attr; cfg.numAttrs = 1;
+    }
+    PolyLaunch(const PolyLaunch &) = delete;               // cfg points into the object
+    PolyLaunch &operator=(const PolyLaunch &) = delete;
+};
+
+// Function attributes of the exponential's kernels for padded state count Dp, and the check that one cluster of
+// expm_poly_kernel can be resident on the device.
+int expm_setup(int Dp, int device) {
+    if (Dp == 32) {
+        CU(cudaFuncSetAttribute(hb2::expm_small_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hb2::expm_small_smem_bytes(32)));
+        CU(cudaFuncSetAttribute(hb2::expm_rates_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hb2::expm_rates_smem_bytes(32)));
+    }
+    if (Dp != 64) return 0;
+    CU(cudaFuncSetAttribute(hb2::expm_powers_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, EXPM64_SMEM));
+    CU(cudaFuncSetAttribute(hb2::expm64_dmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, EXPM64_SMEM));
+    CU(cudaFuncSetAttribute(hb2::expm64_dmma_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    CU(cudaFuncSetAttribute(hb2::expm_poly_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    const PolyLaunch one(1, 0);
+    int clusters = 0;
+    CU(cudaOccupancyMaxActiveClusters(&clusters, hb2::expm_poly_kernel, &one.cfg));
+    if (clusters < 1) return fail("expm_poly_kernel: no cluster of %d CTAs can be resident on device %d", hb2::EXPM_POLY_CLUSTER, device);
+    return 0;
+}
+
+// Calls f(std::integral_constant<int, DP>{}) for the small-state padded count DP = Dp (4, 8, 16, 24, 32); false otherwise.
+template <class F>
+bool small_states(int Dp, F &&f) {
+    switch (Dp) {
+        case 4: f(std::integral_constant<int, 4>{}); return true;
+        case 8: f(std::integral_constant<int, 8>{}); return true;
+        case 16: f(std::integral_constant<int, 16>{}); return true;
+        case 24: f(std::integral_constant<int, 24>{}); return true;
+        case 32: f(std::integral_constant<int, 32>{}); return true;
+        default: return false;
+    }
+}
+
 // One CTA per listed matrix of `in` (rows of D*D matrix entries, or of the template's formula values).  The results go to
 // the P cache, with the tensor-path operands when use_tc, or, when scratch is given, to scratch alone (mixture components
 // and batched site sets).  keep_resident: leave the resident copy of each entry's rate matrix (dense Q, or formula values
@@ -507,60 +567,48 @@ int launch_expm(hb2_partition *p, Source src, const double *in, const int *d_dst
         a.Q = nullptr; a.V = in; a.tmpl_index = t->d_index; a.tmpl_formula = t->d_formula;
         a.tmpl_colfreq = t->has_colfreq ? t->d_colfreq : (double *)nullptr; a.tmpl_nnz = (int)t->nnz; a.nF = (int)t->nF;
     }
-    switch (p->Dp) {
-        case 64: {
-            const size_t smem = 3 * 64 * hb2::LD64 * sizeof(double);
-            hb2::ExpmTcOut tc{nullptr, nullptr};
-            if (p->use_tc && !scratch) { tc.PB = p->d_PB; tc.PTf = p->d_PTf; }
-            if (sp.use && src.kind != Kind::Trans) {
-                hb2_partition::ExBuf &x = *sp.x;
-                const int nV = t ? (int)t->nF : (int)(p->D * p->D);
-                // references index the whole batch: classification has to see it in one piece (off == 0 for compiled batches
-                // and for dense batches that consist of a single run; mixed dense batches fall back below)
-                a.group = x.d_int + off; a.flag = x.d_flag + off; a.weight = x.d_weight + off; a.groups = x.d_groups;
-                a.pow = x.d_pow;
-                a.Qres = nullptr;                    // the classification stage keeps the resident copy
-                // the power tables are built on the side stream while the classification runs (plan_shared keeps the two
-                // from touching the same group)
-                if (sp.n_refs > 0) {
-                    hb2::ExpmPowersArgs pa{};
-                    pa.a = a; pa.refs = x.d_int + 2 * x.cap; pa.groups = x.d_groups;
-                    pa.pow = x.d_pow; pa.refvec = x.d_refvec; pa.refvec_stride = x.stride; pa.nV = nV; pa.kind = sp.kind; pa.Vin = in;
-                    pa.flags = x.d_flags; pa.gen = ++x.gen; pa.err = p->d_err;
-                    CU(cudaEventRecord(p->ev_fork, p->stream));
-                    CU(cudaStreamWaitEvent(p->side, p->ev_fork, 0));
-                    hb2::expm_powers_kernel<<<dim3(hb2::EXPM_POW_TERMS - 1, (unsigned)sp.n_refs), 256, smem, p->side>>>(pa);
-                    p->launches++;
-                    CU(cudaEventRecord(p->ev_join, p->side));
-                }
-                hb2::ExpmClassifyArgs ca{};
-                ca.V = in; ca.nV = nV; ca.kind = sp.kind; ca.dst = d_dst; ca.group = x.d_int + off;
-                ca.ref = x.d_int + x.cap + off; ca.groups = x.d_groups; ca.refvec = x.d_refvec; ca.refvec_stride = x.stride;
-                ca.weight = x.d_weight + off; ca.flag = x.d_flag + off;
-                ca.res = !keep_resident ? nullptr : t ? (double *)t->d_Vres : (double *)p->d_Qres;
-                if (nV <= 256) hb2::expm_classify_warp_kernel<<<(n + 7) / 8, 256, 0, p->stream>>>(ca, n);
-                else hb2::expm_classify_kernel<<<n, 128, 0, p->stream>>>(ca);
-                if (sp.n_refs > 0) CU(cudaStreamWaitEvent(p->stream, p->ev_join, 0));
-                cudaLaunchConfig_t cfg{};
-                cfg.gridDim = dim3(hb2::EXPM_POLY_CLUSTER, (unsigned)((n + hb2::EXPM_POLY_CHUNK - 1) / hb2::EXPM_POLY_CHUNK));
-                cfg.blockDim = dim3(256);
-                cfg.stream = p->stream;
-                cudaLaunchAttribute attr{};
-                attr.id = cudaLaunchAttributeClusterDimension;
-                attr.val.clusterDim.x = hb2::EXPM_POLY_CLUSTER; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
-                cfg.attrs = &attr; cfg.numAttrs = 1;
-                CU(cudaLaunchKernelEx(&cfg, hb2::expm_poly_kernel, a, tc, n));
-                p->launches += 2;
+    if (p->Dp == 64) {
+        hb2::ExpmTcOut tc{nullptr, nullptr};
+        if (p->use_tc && !scratch) { tc.PB = p->d_PB; tc.PTf = p->d_PTf; }
+        if (sp.use && src.kind != Kind::Trans) {
+            hb2_partition::ExBuf &x = *sp.x;
+            const int nV = t ? (int)t->nF : (int)(p->D * p->D);
+            // references index the whole batch: classification has to see it in one piece (off == 0 for compiled batches
+            // and for dense batches that consist of a single run; mixed dense batches fall back below)
+            a.group = x.d_int + off; a.flag = x.d_flag + off; a.weight = x.d_weight + off; a.groups = x.d_groups;
+            a.pow = x.d_pow;
+            a.Qres = nullptr;                    // the classification stage keeps the resident copy
+            // the power tables are built on the side stream while the classification runs (plan_shared keeps the two
+            // from touching the same group)
+            if (sp.n_refs > 0) {
+                hb2::ExpmPowersArgs pa{};
+                pa.a = a; pa.refs = x.d_int + 2 * x.cap; pa.groups = x.d_groups;
+                pa.pow = x.d_pow; pa.refvec = x.d_refvec; pa.refvec_stride = x.stride; pa.nV = nV; pa.kind = sp.kind; pa.Vin = in;
+                pa.flags = x.d_flags; pa.gen = ++x.gen; pa.err = p->d_err;
+                CU(cudaEventRecord(p->ev_fork, p->stream));
+                CU(cudaStreamWaitEvent(p->side, p->ev_fork, 0));
+                hb2::expm_powers_kernel<<<dim3(hb2::EXPM_POW_TERMS - 1, (unsigned)sp.n_refs), 256, EXPM64_SMEM, p->side>>>(pa);
+                p->launches++;
+                CU(cudaEventRecord(p->ev_join, p->side));
             }
-            hb2::expm64_dmma_kernel<<<std::min(n, 2 * p->sm_count), 256, smem, p->stream>>>(a, tc, n);
-            break;
+            hb2::ExpmClassifyArgs ca{};
+            ca.V = in; ca.nV = nV; ca.kind = sp.kind; ca.dst = d_dst; ca.group = x.d_int + off;
+            ca.ref = x.d_int + x.cap + off; ca.groups = x.d_groups; ca.refvec = x.d_refvec; ca.refvec_stride = x.stride;
+            ca.weight = x.d_weight + off; ca.flag = x.d_flag + off;
+            ca.res = !keep_resident ? nullptr : t ? (double *)t->d_Vres : (double *)p->d_Qres;
+            if (nV <= 256) hb2::expm_classify_warp_kernel<<<(n + 7) / 8, 256, 0, p->stream>>>(ca, n);
+            else hb2::expm_classify_kernel<<<n, 128, 0, p->stream>>>(ca);
+            if (sp.n_refs > 0) CU(cudaStreamWaitEvent(p->stream, p->ev_join, 0));
+            const PolyLaunch pl((unsigned)((n + hb2::EXPM_POLY_CHUNK - 1) / hb2::EXPM_POLY_CHUNK), p->stream);
+            CU(cudaLaunchKernelEx(&pl.cfg, hb2::expm_poly_kernel, a, tc, n));
+            p->launches += 2;
         }
-        case 4: hb2::expm_small_kernel<4><<<n, 128, hb2::expm_small_smem_bytes(4), p->stream>>>(a); break;
-        case 8: hb2::expm_small_kernel<8><<<n, 128, hb2::expm_small_smem_bytes(8), p->stream>>>(a); break;
-        case 16: hb2::expm_small_kernel<16><<<n, 128, hb2::expm_small_smem_bytes(16), p->stream>>>(a); break;
-        case 24: hb2::expm_small_kernel<24><<<n, 128, hb2::expm_small_smem_bytes(24), p->stream>>>(a); break;
-        case 32: hb2::expm_small_kernel<32><<<n, 128, hb2::expm_small_smem_bytes(32), p->stream>>>(a); break;
-        default: return fail("unsupported padded state count %d", p->Dp);
+        hb2::expm64_dmma_kernel<<<std::min(n, 2 * p->sm_count), 256, EXPM64_SMEM, p->stream>>>(a, tc, n);
+    } else if (!small_states(p->Dp, [&](auto dp) {
+                   constexpr int DP = decltype(dp)::value;
+                   hb2::expm_small_kernel<DP><<<n, 128, hb2::expm_small_smem_bytes(DP), p->stream>>>(a);
+               })) {
+        return fail("unsupported padded state count %d", p->Dp);
     }
     p->launches++;
     CU(cudaGetLastError());
@@ -1285,8 +1333,7 @@ int evaluate_impl(hb2_partition *p, int c0, int nc, const double *weights, int64
         p->walk_reset = p->use_tc;          // tags are inconsistent: the next pass starts from scratch
         cudaMemsetAsync(p->d_err, 0, sizeof(int), p->stream);   // on every path, or each later evaluation would fail too
         std::fill(p->evaluated_cat.begin(), p->evaluated_cat.end(), 0);
-        return fail("a device-side wait timed out (code %d: 1 = operand staging / tensor pipe, 2 = another lane's conditionals, 3 = a peer "
-                    "rank's partials, 4 = a coefficient matrix of the shared-powers exponential)", code);
+        return wait_timeout(code);
     }
     *lnL = hs[p->Dp + p->C];
     for (int c = c0; c < c0 + nc; c++) p->evaluated_cat[c] = 1;
@@ -1368,7 +1415,7 @@ int sim_tables(hb2_partition *p, hb2::SimArgs &a, int64_t nblk, int64_t chunk, u
     CU(cudaMemcpyAsync(&chk[0], a.bad, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
     CU(cudaMemcpyAsync(&chk[1], p->d_err, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
     CU(cudaStreamSynchronize(p->stream));
-    if (chk[1]) { cudaMemsetAsync(p->d_err, 0, sizeof(int), p->stream); return fail("a device-side wait timed out in the batched exponential (code %d)", chk[1]); }
+    if (chk[1]) { cudaMemsetAsync(p->d_err, 0, sizeof(int), p->stream); return wait_timeout(chk[1]); }
     if (chk[0] != INT_MAX) {
         const long long row = chk[0] % D, cb = chk[0] / D;
         const std::string msg = std::string(fn) + ": row %lld of the transition matrix of " + block + " does not have a finite positive total";
@@ -1496,27 +1543,10 @@ int hb2_create(hb2_partition **out, int64_t S, int64_t D, int64_t L, int64_t I, 
         CU(cudaMemcpyAsync(p->d_child_start, cs.data(), cs.size() * sizeof(int), cudaMemcpyHostToDevice, st));
         CU(cudaMemcpyAsync(p->d_child_ids, ci.data(), ci.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     }
-    if (Dp == 32) CU(cudaFuncSetAttribute(hb2::expm_small_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hb2::expm_small_smem_bytes(32)));
-    if (Dp == 32) CU(cudaFuncSetAttribute(hb2::expm_rates_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hb2::expm_rates_smem_bytes(32)));
+    if (expm_setup(Dp, device)) return 1;
     if (Dp == 64) {
         { const char *env = getenv("HB2_EXPM_SHARED"); p->ex_enabled = !(env && env[0] == '0'); }
         if (p->ex.alloc(std::max((int)C + 8, HB2_MAX_TEMPLATES * (int)C), (int64_t)(C + 8) * p->B, st)) return 1;
-        CU(cudaFuncSetAttribute(hb2::expm_powers_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(3 * 64 * hb2::LD64 * sizeof(double))));
-        CU(cudaFuncSetAttribute(hb2::expm64_dmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(3 * 64 * hb2::LD64 * sizeof(double))));
-        CU(cudaFuncSetAttribute(hb2::expm64_dmma_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-        // the polynomial kernel's 16 row slices of a chunk share their column sums as one cluster (a non-portable size)
-        CU(cudaFuncSetAttribute(hb2::expm_poly_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-        cudaLaunchConfig_t cfg{};
-        cfg.gridDim = dim3(hb2::EXPM_POLY_CLUSTER);
-        cfg.blockDim = dim3(256);
-        cudaLaunchAttribute attr{};
-        attr.id = cudaLaunchAttributeClusterDimension;
-        attr.val.clusterDim.x = hb2::EXPM_POLY_CLUSTER; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
-        cfg.attrs = &attr; cfg.numAttrs = 1;
-        int clusters = 0;
-        CU(cudaOccupancyMaxActiveClusters(&clusters, hb2::expm_poly_kernel, &cfg));
-        if (clusters < 1)
-            return fail("expm_poly_kernel: no cluster of %d CTAs can be resident on device %d", hb2::EXPM_POLY_CLUSTER, device);
     }
     if (Dp == 4) {
         if (const char *env = getenv("HB2_SMALL_ILP")) p->small_ilp = atoi(env);
@@ -1888,14 +1918,8 @@ static int rates_chunk(hb2_partition *p, const BatchCall &c, int64_t s0, int64_t
     for (int64_t s = 0; s < nb; s++) ws.h_pat[s] = (int)c.patternOf[s0 + s];
     CU(cudaMemcpyAsync(ws.pat, ws.h_pat, (size_t)nb * sizeof(int), cudaMemcpyHostToDevice, p->stream));
     CU(cudaMemcpyAsync(ws.V, c.rates + s0, (size_t)nb * sizeof(double), cudaMemcpyHostToDevice, p->stream));
-    switch (p->Dp) {
-        case 4: launch_rates<4>(p, c, nb); break;
-        case 8: launch_rates<8>(p, c, nb); break;
-        case 16: launch_rates<16>(p, c, nb); break;
-        case 24: launch_rates<24>(p, c, nb); break;
-        case 32: launch_rates<32>(p, c, nb); break;
-        default: return fail("hb2_batch_site_rates: unsupported padded state count %d", p->Dp);
-    }
+    if (!small_states(p->Dp, [&](auto dp) { launch_rates<decltype(dp)::value>(p, c, nb); }))
+        return fail("hb2_batch_site_rates: unsupported padded state count %d", p->Dp);
     p->launches += 2;
     CU(cudaGetLastError());
     CU(cudaMemcpyAsync(c.siteLnL + s0, ws.out, (size_t)nb * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
@@ -2016,7 +2040,7 @@ static int batch_sites(hb2_partition *p, const BatchCall &c) {
     int err = 0;
     CU(cudaMemcpyAsync(&err, p->d_err, sizeof(int), cudaMemcpyDeviceToHost, p->stream));
     CU(cudaStreamSynchronize(p->stream));
-    if (err) { cudaMemsetAsync(p->d_err, 0, sizeof(int), p->stream); return fail("a device-side wait timed out in the batched exponential (code %d)", err); }
+    if (err) { cudaMemsetAsync(p->d_err, 0, sizeof(int), p->stream); return wait_timeout(err); }
     return 0;
 }
 

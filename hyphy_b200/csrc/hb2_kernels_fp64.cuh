@@ -27,6 +27,41 @@ namespace hb2 {
 
 constexpr int LD64 = 66;            // smem leading dimension (doubles) for 64x64 operands: conflict-free row pairs
 
+// Tensor-path operands of one 64-state transition matrix (written by the expm stage, read by hb2_kernels_tc.cuh).
+constexpr int TC_PB_FLOATS = 2 * 4096;         // per (class, branch): Ph tile + Pl tile in canonical layout
+constexpr int TC_PTF_ROW = 68;                 // floats per row of the fp32 P^T table (64 + 4 padding: 272-byte rows)
+constexpr int TC_PTF_FLOATS = 64 * TC_PTF_ROW; // per (class, branch)
+
+// Two different roundings to tf32 (round to nearest, ties away from zero); call sites keep the one they use.
+// tf32_rn: integer add-and-mask, two full-rate instructions; a NaN with bits above 0x7fffe000 comes out as -0.0.
+__device__ __forceinline__ float tf32_rn(float x) {
+    return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
+}
+// tf32_rn_cvt: the conversion instruction cvt.rna.tf32.f32 (a quarter of the ALU rate); NaN stays NaN.
+__device__ __forceinline__ float tf32_rn_cvt(float x) {
+    uint32_t r;
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+    return __uint_as_float(r);
+}
+
+// Device-side waits are bounded by TIME (globaltimer), not by an iteration count: a slow producer (another partition or
+// process sharing the GPU, fewer co-resident CTAs than planned) only makes the pass slower; a protocol bug still surfaces
+// as an error code in the partition's error flag (the host returns an error, see wait_timeout), never as a hung GPU.
+__device__ __forceinline__ unsigned long long globaltimer_ns() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+constexpr unsigned long long HB2_WAIT_LIMIT_NS = 4000000000ull;         // waits within one device
+constexpr unsigned long long HB2_PEER_WAIT_LIMIT_NS = 20000000000ull;   // waits for another rank: longer, a rank is gone
+// What a timed-out wait was waiting for: the value it leaves in the error flag.
+enum WaitCode : int {
+    WAIT_TC_STAGING = 1,      // operand staging / the tensor pipe (mbarrier)
+    WAIT_LANE = 2,            // another lane's conditionals
+    WAIT_PEER = 3,            // a peer rank's partials
+    WAIT_EXPM_POWERS = 4,     // a coefficient matrix of the shared-powers exponential
+};
+
 struct TreeDev {
     const int *child_start;         // [I+1]
     const int *child_ids;           // flat node ids of the children of each internal node
@@ -183,10 +218,11 @@ __device__ __forceinline__ void load_rate_matrix(const ExpmArgs &a, double *A1, 
     __syncthreads();
 }
 
-__constant__ double c_taylor[16] = {1.0, 1.0, 0.5, 1.0 / 6, 1.0 / 24, 1.0 / 120, 1.0 / 720, 1.0 / 5040, 1.0 / 40320,
+// Taylor coefficients 1/k!, k = 0..17: the small-state polynomial uses 16 of them, expm64_dmma_kernel's up to 18.
+__constant__ double c_taylor[18] = {1.0, 1.0, 0.5, 1.0 / 6, 1.0 / 24, 1.0 / 120, 1.0 / 720, 1.0 / 5040, 1.0 / 40320,
                                     1.0 / 362880, 1.0 / 3628800, 1.0 / 39916800, 1.0 / 479001600, 1.0 / 6227020800.0,
-                                    1.0 / 87178291200.0, 1.0 / 1307674368000.0};
-__device__ __forceinline__ double taylor_c(int k) { return c_taylor[k]; }
+                                    1.0 / 87178291200.0, 1.0 / 1307674368000.0, 1.0 / 20922789888000.0,
+                                    1.0 / 355687428096000.0};
 
 // ------------------------------------------------------------------------------------------------
 // expm64_dmma_kernel: 64 padded states, products on the FP64 tensor pipe (mma.sync.m8n8k4.f64, DMMA)
@@ -197,11 +233,6 @@ __device__ __forceinline__ double taylor_c(int k) { return c_taylor[k]; }
 // (g = lane/4, q = lane%4) holds element (row 16wr+8i+g, col 32wc+8j+2q+e) in acc[i][j][e].
 // Optional fused epilogue for the tensor-core pruning path: PB (hi/lo canonical tiles of P) and PTf (fp32 PT).
 // ------------------------------------------------------------------------------------------------
-__constant__ double c_taylor18[18] = {1.0, 1.0, 0.5, 1.0 / 6, 1.0 / 24, 1.0 / 120, 1.0 / 720, 1.0 / 5040, 1.0 / 40320,
-                                      1.0 / 362880, 1.0 / 3628800, 1.0 / 39916800, 1.0 / 479001600, 1.0 / 6227020800.0,
-                                      1.0 / 87178291200.0, 1.0 / 1307674368000.0, 1.0 / 20922789888000.0,
-                                      1.0 / 355687428096000.0};
-
 __device__ __forceinline__ void dmma884(double (&c)[2], double a, double b) {
     asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
                  : "+d"(c[0]), "+d"(c[1]) : "d"(a), "d"(b));
@@ -228,10 +259,61 @@ struct ExpmTcOut {
     float *PTf;     // [slots][64 rows][68 floats] (rows padded: conflict-free shared-memory gathers after a flat bulk copy)
 };
 
-__device__ __forceinline__ float tf32_rn_dev(float x) {
-    uint32_t r;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-    return __uint_as_float(r);
+// ---- Finishing rules of a 64-state matrix (expm64_dmma_kernel, expm_powers_kernel, expm_poly_kernel, mix_reduce_kernel)
+// A NaN or infinite input or absurd rates: the whole slot is NaN, tensor-path operands included (the host sees NaN lnL).
+__device__ __forceinline__ void expm64_poison(double *out, const ExpmTcOut &tc, size_t slot, int tid) {
+    for (int idx = tid; idx < 4096; idx += 256) out[idx] = __longlong_as_double(0x7ff8000000000000LL);
+    if (tc.PB) {
+        for (int idx = tid; idx < TC_PB_FLOATS; idx += 256) tc.PB[slot * TC_PB_FLOATS + idx] = __int_as_float(0x7fc00000);
+        for (int idx = tid; idx < TC_PTF_FLOATS; idx += 256) tc.PTf[slot * TC_PTF_FLOATS + idx] = __int_as_float(0x7fc00000);
+    }
+}
+
+// Index maps of the tensor-path operands for element (r, c) of PT (r = child state, c = parent state): row r of the
+// padded fp32 table, and chunk r/4, offset 4c + r%4 of the canonical tiles (hb2_kernels_tc.cuh).
+__device__ __forceinline__ int tc_ptf_index(int r, int c) { return r * TC_PTF_ROW + c; }
+__device__ __forceinline__ int tc_pb_index(int r, int c) { return (r >> 2) * 256 + c * 4 + (r & 3); }
+
+// The hi/lo split of P element p into position o of the slot's tiles pb (Ph, then Pl): CVT rounds with tf32_rn_cvt, else
+// with tf32_rn.
+template <bool CVT>
+__device__ __forceinline__ void tc_split_store(float *pb, int o, double p) {
+    const float hi = CVT ? tf32_rn_cvt((float)p) : tf32_rn((float)p);
+    const float lo = (float)(p - (double)hi);
+    pb[o] = hi;
+    pb[TC_PB_FLOATS / 2 + o] = CVT ? tf32_rn_cvt(lo) : tf32_rn(lo);
+}
+
+// Both tensor-path operands of a finished PT (leading dimension ld) in the tiles' order, 256 threads.
+template <bool CVT>
+__device__ __forceinline__ void tc_store_operands(const double *PT, int ld, float *pb, float *pf, int tid) {
+    for (int o = tid; o < 4096; o += 256) {
+        const int r = (o >> 8) * 4 + (o & 3), c = (o >> 2) & 63;       // tc_pb_index(r, c) == o
+        tc_split_store<CVT>(pb, o, PT[r * ld + c]);
+        pf[tc_ptf_index(o >> 6, o & 63)] = (float)PT[(o >> 6) * ld + (o & 63)];
+    }
+}
+
+// Row-sum norm of a 64x64 matrix A held transposed in X (leading dimension LD64): the 64 sums by threads 0..63 into red,
+// then their maximum and a NaN / inf scan by warp 0 (fmax is exact).  Called by every thread of the CTA; the result and
+// `bad` are valid in warp 0.
+__device__ __forceinline__ double expm64_norm(const double *X, double *red, int tid, bool &bad) {
+    if (tid < 64) {
+        double s = 0.0;
+        for (int j = 0; j < 64; j++) s += fabs(X[j * LD64 + tid]);
+        red[tid] = s;
+    }
+    __syncthreads();
+    double m = 0.0;
+    bad = false;
+    if (tid < 32) {
+        m = fmax(red[tid], red[tid + 32]);
+        bad = !(red[tid] == red[tid]) || !(red[tid + 32] == red[tid + 32]) || isinf(red[tid]) || isinf(red[tid + 32]);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
+        bad = __any_sync(0xffffffffu, bad);
+    }
+    return m;
 }
 
 
@@ -269,6 +351,26 @@ __device__ __forceinline__ void expm_classify_result(const ExpmClassifyArgs &a, 
     if (g >= 0 && r == k) a.groups[g].weight = wk;
 }
 
+// The reference of an entry of group g (g < 0: none): entry r of this batch, or for r < 0 the direction the group's
+// table was last built from, if it holds this kind of input; then wr_cached is that table's weight, otherwise -1.
+__device__ __forceinline__ const double *expm_classify_ref(const ExpmClassifyArgs &a, int g, int r, double &wr_cached) {
+    wr_cached = -1.0;
+    if (g < 0) return nullptr;
+    if (r >= 0) return a.V + (size_t)r * a.nV;
+    if (a.groups[g].kind != a.kind) return nullptr;
+    wr_cached = a.groups[g].weight;
+    return a.refvec + (size_t)g * a.refvec_stride;
+}
+
+// The acceptance test: a reference and two finite weights, the reference's positive (NaN fails every comparison) ...
+__device__ __forceinline__ bool expm_classify_usable(const double *vr, double wk, double wr) {
+    return (vr != nullptr) && (wr > 0.0) && (wk >= 0.0) && (wk < INFINITY) && (wr < INFINITY);
+}
+// ... and every value x matching its reference value xr scaled by wk / wr to tol = 1e-13 * wk of |xr|.
+__device__ __forceinline__ bool expm_classify_match(double x, double xr, double wk, double wr, double tol) {
+    return fabs(x * wr - xr * wk) <= tol * fabs(xr);
+}
+
 // Inputs of more than 256 values (dense: nV = D*D <= 4096): each thread holds its up to EXPM_CLASSIFY_REGS values of the
 // entry and of the reference in registers, all loads issued before any sum, so the entry is read from memory once and the
 // proportionality check runs from registers.  Values f = tid + 128 i are summed in increasing i, as a plain strided loop
@@ -279,15 +381,11 @@ __global__ void __launch_bounds__(128) expm_classify_kernel(ExpmClassifyArgs a) 
     __shared__ int bad[4];
     const int k = blockIdx.x, tid = threadIdx.x, nV = a.nV;
     const int slot = a.dst[k];
-    if (slot < 0) { if (tid == 0) { a.flag[k] = 0; a.weight[k] = 0.0; } return; }
+    if (slot < 0) { if (tid == 0) expm_classify_result(a, k, -1, -1, 0, 0.0); return; }
     const double *v = a.V + (size_t)k * nV;
     const int g = a.group[k], r = a.ref[k];
-    const double *vr = nullptr;
-    double wr_cached = -1.0;
-    if (g >= 0) {
-        if (r >= 0) vr = a.V + (size_t)r * nV;
-        else if (a.groups[g].kind == a.kind) { vr = a.refvec + (size_t)g * a.refvec_stride; wr_cached = a.groups[g].weight; }
-    }
+    double wr_cached;
+    const double *vr = expm_classify_ref(a, g, r, wr_cached);
     double xv[EXPM_CLASSIFY_REGS], xr[EXPM_CLASSIFY_REGS];
 #pragma unroll
     for (int i = 0; i < EXPM_CLASSIFY_REGS; i++) {
@@ -318,14 +416,14 @@ __global__ void __launch_bounds__(128) expm_classify_kernel(ExpmClassifyArgs a) 
     wk = red[0][0] + red[0][1] + red[0][2] + red[0][3];
     wr = red[1][0] + red[1][1] + red[1][2] + red[1][3];
     if (wr_cached >= 0.0) wr = wr_cached;
-    int ok = (vr != nullptr) && (wr > 0.0) && (wk >= 0.0) && (wk < INFINITY) && (wr < INFINITY);   // NaN fails every comparison
+    int ok = expm_classify_usable(vr, wk, wr);
     if (ok) {
         const double tol = 1e-13 * wk;
 #pragma unroll
         for (int i = 0; i < EXPM_CLASSIFY_REGS; i++)
-            if (tid + 128 * i < nV && !(fabs(xv[i] * wr - xr[i] * wk) <= tol * fabs(xr[i]))) ok = 0;
+            if (tid + 128 * i < nV && !expm_classify_match(xv[i], xr[i], wk, wr, tol)) ok = 0;
         for (int f = tid + 128 * EXPM_CLASSIFY_REGS; f < nV; f += 128)
-            if (!(fabs(v[f] * wr - vr[f] * wk) <= tol * fabs(vr[f]))) ok = 0;
+            if (!expm_classify_match(v[f], vr[f], wk, wr, tol)) ok = 0;
     }
     ok = __all_sync(0xffffffffu, ok);
     if ((tid & 31) == 0) bad[tid >> 5] = !ok;
@@ -340,15 +438,11 @@ __global__ void __launch_bounds__(256) expm_classify_warp_kernel(ExpmClassifyArg
     const int lane = threadIdx.x & 31, k = blockIdx.x * 8 + (threadIdx.x >> 5);
     if (k >= n) return;
     const int slot = a.dst[k];
-    if (slot < 0) { if (lane == 0) { a.flag[k] = 0; a.weight[k] = 0.0; } return; }
+    if (slot < 0) { if (lane == 0) expm_classify_result(a, k, -1, -1, 0, 0.0); return; }
     const double *v = a.V + (size_t)k * a.nV;
     const int g = a.group[k], r = a.ref[k];
-    const double *vr = nullptr;
-    double wr_cached = -1.0;
-    if (g >= 0) {
-        if (r >= 0) vr = a.V + (size_t)r * a.nV;
-        else if (a.groups[g].kind == a.kind) { vr = a.refvec + (size_t)g * a.refvec_stride; wr_cached = a.groups[g].weight; }
-    }
+    double wr_cached;
+    const double *vr = expm_classify_ref(a, g, r, wr_cached);
     double wk = 0.0, wr = 0.0;
     for (int f = lane; f < a.nV; f += 32) {
         const double x = v[f];
@@ -359,32 +453,44 @@ __global__ void __launch_bounds__(256) expm_classify_warp_kernel(ExpmClassifyArg
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) { wk += __shfl_xor_sync(0xffffffffu, wk, o); wr += __shfl_xor_sync(0xffffffffu, wr, o); }
     if (wr_cached >= 0.0) wr = wr_cached;
-    int ok = (vr != nullptr) && (wr > 0.0) && (wk >= 0.0) && (wk < INFINITY) && (wr < INFINITY);   // NaN fails every comparison
+    int ok = expm_classify_usable(vr, wk, wr);
     if (ok) {
         const double tol = 1e-13 * wk;
         for (int f = lane; f < a.nV; f += 32)
-            if (!(fabs(v[f] * wr - vr[f] * wk) <= tol * fabs(vr[f]))) ok = 0;
+            if (!expm_classify_match(v[f], vr[f], wk, wr, tol)) ok = 0;
     }
     ok = __all_sync(0xffffffffu, ok);
     if (lane == 0) expm_classify_result(a, k, g, r, ok, wk);
 }
 
-// Shared-powers entry k: rho = ||A_k||_inf estimated from its weight, and the squarings expm_poly_kernel chose for it.
-// shift == 0 with rho not NaN: that kernel has finished the entry.
-__device__ __forceinline__ int expm_poly_shift(const ExpmArgs &a, int k, double &rho) {
-    const ExpmGroup gi = a.groups[a.group[k]];
-    rho = gi.nu * (a.weight[k] / gi.weight);
+// Shared-powers entry: rho = ||A||_inf estimated from the entry's weight w and its group's reference (nu, wref), and the
+// squarings that bring it to rho / 2^shift <= EXPM_POLY_THETA.  expm_poly_kernel evaluates the polynomial there;
+// expm64_dmma_kernel squares it, or writes NaN (expm_poly_nan).
+__device__ __forceinline__ int expm_poly_shift(double nu, double wref, double w, double &rho) {
+    rho = nu * (w / wref);
     int shift = 0;
     if (rho > EXPM_POLY_THETA) { int e = 0; frexp(rho / EXPM_POLY_THETA, &e); shift = max(e, 0); }
     return shift;
 }
+__device__ __forceinline__ int expm_poly_shift(const ExpmArgs &a, int k, double &rho) {
+    const ExpmGroup gi = a.groups[a.group[k]];
+    return expm_poly_shift(gi.nu, gi.weight, a.weight[k], rho);
+}
+// NaN input or absurd rates: the entry's matrix is NaN.
+__device__ __forceinline__ bool expm_poly_nan(int shift, double rho) { return !(rho == rho) || shift > 900; }
+// Live entry k has been finished by expm_poly_kernel: shared powers, no squaring and a usable rate.
+__device__ __forceinline__ bool expm_poly_finished(const ExpmArgs &a, int k) {
+    double rho;
+    return a.flag && a.flag[k] && expm_poly_shift(a, k, rho) == 0 && rho == rho;
+}
 
-// One entry of expm64_dmma_kernel.  Three shared 64x64 fp64 buffers (101 KB) so that TWO CTAs share an SM and one CTA's
-// load/norm/epilogue phases overlap the other's DMMA products:  X0 = A -> later R,  X1 = A^2,  X2 = A^3.  The polynomial
-// blocks need A at the thread's own output positions after X0 has become R: those values are parked in the (not yet
-// written) output slot PT[slot] in global memory (L2 resident, same [row][col] layout) and re-read per Horner step.
-// Every exit is CTA-uniform; the caller separates entries with a barrier.  Kept out of line: inlined into the kernel's
-// entry loop, the body no longer fits the 128 registers of two CTAs per SM and spills.
+// One entry of expm64_dmma_kernel, listed by it as live and not finished by expm_poly_kernel.  Three shared 64x64 fp64
+// buffers (101 KB) so that TWO CTAs share an SM and one CTA's load/norm/epilogue phases overlap the other's DMMA
+// products:  X0 = A -> later R,  X1 = A^2,  X2 = A^3.  The polynomial blocks need A at the thread's own output positions
+// after X0 has become R: those values are parked in the (not yet written) output slot PT[slot] in global memory (L2
+// resident, same [row][col] layout) and re-read per Horner step.  Every exit is CTA-uniform; the caller separates entries
+// with a barrier.  Kept out of line: inlined into the kernel's entry loop, the body no longer fits the 128 registers of two
+// CTAs per SM and spills.
 __device__ __noinline__ void expm64_dmma_entry(const ExpmArgs a, const ExpmTcOut tc, int entry, double *sm) {
     double *X0 = sm, *X1 = X0 + 64 * LD64, *X2 = X1 + 64 * LD64;
     __shared__ double red[64];
@@ -392,7 +498,6 @@ __device__ __noinline__ void expm64_dmma_entry(const ExpmArgs a, const ExpmTcOut
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int wr = warp >> 1, wc = warp & 1, g = lane >> 2, q4 = lane & 3;
     const int D = a.D;
-    if (a.dst[entry] < 0) return;
     const size_t slot = a.dst[entry];
     double *out = a.PT + slot * 4096;
     double *park = out;
@@ -404,15 +509,7 @@ __device__ __noinline__ void expm64_dmma_entry(const ExpmArgs a, const ExpmTcOut
         // (clamp, row repair, tensor-path operands) remain.  shift is recomputed exactly as the polynomial stage chose it.
         double rho;
         const int shift = expm_poly_shift(a, entry, rho);
-        if (shift == 0 && rho == rho) return;    // finished by expm_poly_kernel
-        if (!(rho == rho) || shift > 900) {
-            for (int idx = tid; idx < 4096; idx += 256) out[idx] = __longlong_as_double(0x7ff8000000000000LL);
-            if (tc.PB) {
-                for (int idx = tid; idx < 8192; idx += 256) tc.PB[slot * 8192 + idx] = __int_as_float(0x7fc00000);
-                for (int idx = tid; idx < 4352; idx += 256) tc.PTf[slot * 4352 + idx] = __int_as_float(0x7fc00000);
-            }
-            return;
-        }
+        if (expm_poly_nan(shift, rho)) { expm64_poison(out, tc, slot, tid); return; }
         for (int idx = tid; idx < 4096; idx += 256) R[(idx >> 6) * LD64 + (idx & 63)] = __ldcg(out + idx);
         if (tid == 0) s_shift = shift;
         __syncthreads();
@@ -435,40 +532,22 @@ __device__ __noinline__ void expm64_dmma_entry(const ExpmArgs a, const ExpmTcOut
               for (int j = 0; j < 4; j++) *reinterpret_cast<double2 *>(M + off(i, j)) = make_double2(acc[i][j][0], acc[i][j][1]);
       };
       if (!shared_powers) {
-        if (tid < 64) {
-            double s = 0.0;
-            for (int j = 0; j < 64; j++) s += fabs(X0[j * LD64 + tid]);
-            red[tid] = s;
-        }
-        __syncthreads();
-        if (tid < 32) {                      // warp-parallel max / NaN scan of the 64 row sums
-            double m = fmax(red[tid], red[tid + 32]);
-            bool bad = !(red[tid] == red[tid]) || !(red[tid + 32] == red[tid + 32]) || isinf(red[tid]) || isinf(red[tid + 32]);
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
-            bad = __any_sync(0xffffffffu, bad);
-            if (tid == 0) {
-                int shift = 0;
-                if (!bad && m > 0.975) {
-                    int e = 0;
-                    frexp(m / 0.975, &e);          // m/0.975 = f*2^e, f in [0.5,1)  ->  m/2^e <= 0.975
-                    shift = max(e, 0);
-                }
-                const double theta = bad ? 0.0 : ldexp(m, -shift);
-                s_Q = theta <= 0.0064 ? 1 : theta <= 0.069 ? 2 : theta <= 0.245 ? 3 : theta <= 0.55 ? 4 : 5;
-                s_shift = bad ? -1 : shift;
+        bool bad;
+        const double m = expm64_norm(X0, red, tid, bad);
+        if (tid == 0) {
+            int shift = 0;
+            if (!bad && m > 0.975) {
+                int e = 0;
+                frexp(m / 0.975, &e);          // m/0.975 = f*2^e, f in [0.5,1)  ->  m/2^e <= 0.975
+                shift = max(e, 0);
             }
+            const double theta = bad ? 0.0 : ldexp(m, -shift);
+            s_Q = theta <= 0.0064 ? 1 : theta <= 0.069 ? 2 : theta <= 0.245 ? 3 : theta <= 0.55 ? 4 : 5;
+            s_shift = bad ? -1 : shift;
         }
         __syncthreads();
         const int shift = s_shift, Q = s_Q;
-        if (shift < 0 || shift > 900) {           // NaN/inf or absurd rates: propagate NaN (host sees NaN lnL)
-            for (int idx = tid; idx < 4096; idx += 256) out[idx] = __longlong_as_double(0x7ff8000000000000LL);
-            if (tc.PB) {
-                for (int idx = tid; idx < 8192; idx += 256) tc.PB[slot * 8192 + idx] = __int_as_float(0x7fc00000);
-                for (int idx = tid; idx < 4352; idx += 256) tc.PTf[slot * 4352 + idx] = __int_as_float(0x7fc00000);
-            }
-            return;
-        }
+        if (shift < 0 || shift > 900) { expm64_poison(out, tc, slot, tid); return; }   // NaN/inf or absurd rates
         {   // scale A in place and park a copy in the output slot (coalesced)
             const double sc = exp2i(-shift);
             for (int idx = tid; idx < 64 * 64; idx += 256) {
@@ -488,10 +567,10 @@ __device__ __noinline__ void expm64_dmma_entry(const ExpmArgs a, const ExpmTcOut
             const int r = 16 * wr + 8 * i + g, c = 32 * wc + 8 * j + 2 * q4;
             const double2 a1 = __ldcg(reinterpret_cast<const double2 *>(park + goff(i, j)));
             const double2 a2 = *reinterpret_cast<const double2 *>(X1 + off(i, j));
-            double2 v = make_double2(c_taylor18[3 * qq + 1] * a1.x + c_taylor18[3 * qq + 2] * a2.x,
-                                     c_taylor18[3 * qq + 1] * a1.y + c_taylor18[3 * qq + 2] * a2.y);
-            if (r == c) v.x += c_taylor18[3 * qq];
-            if (r == c + 1) v.y += c_taylor18[3 * qq];
+            double2 v = make_double2(c_taylor[3 * qq + 1] * a1.x + c_taylor[3 * qq + 2] * a2.x,
+                                     c_taylor[3 * qq + 1] * a1.y + c_taylor[3 * qq + 2] * a2.y);
+            if (r == c) v.x += c_taylor[3 * qq];
+            if (r == c + 1) v.y += c_taylor[3 * qq];
             return v;
         };
 #pragma unroll
@@ -537,21 +616,8 @@ __device__ __noinline__ void expm64_dmma_entry(const ExpmArgs a, const ExpmTcOut
         if (tid < D) R[tid * LD64 + tid] = fmax(1.0 - (X1[tid] + X1[64 + tid] + X1[128 + tid] + X1[192 + tid]), 0.0);
         __syncthreads();
     }
-    {
-        for (int idx = tid; idx < 4096; idx += 256) out[idx] = R[(idx >> 6) * LD64 + (idx & 63)];
-        if (tc.PB) {
-            float *pb = tc.PB + slot * 8192;
-            float *pf = tc.PTf + slot * 4352;           // rows padded to 68 floats (TC_PTF_ROW)
-            for (int o = tid; o < 4096; o += 256) {
-                const int chunk = o >> 8, n = (o >> 2) & 63, kk = chunk * 4 + (o & 3);
-                const double pv = R[kk * LD64 + n];          // P[n][kk] = PT[kk][n]
-                const float hi = tf32_rn_dev((float)pv);
-                pb[o] = hi;
-                pb[4096 + o] = tf32_rn_dev((float)(pv - (double)hi));
-                pf[(o >> 6) * 68 + (o & 63)] = (float)R[(o >> 6) * LD64 + (o & 63)];
-            }
-        }
-    }
+    for (int idx = tid; idx < 4096; idx += 256) out[idx] = R[(idx >> 6) * LD64 + (idx & 63)];
+    if (tc.PB) tc_store_operands<true>(R, LD64, tc.PB + slot * TC_PB_FLOATS, tc.PTf + slot * TC_PTF_FLOATS, tid);
 }
 
 // One wave of CTAs (gridDim.x <= 2 per SM) striding over the n entries of a batch.  Per round of up to 256 entries of
@@ -564,11 +630,7 @@ __global__ void __launch_bounds__(256, 2) expm64_dmma_kernel(ExpmArgs a, ExpmTcO
         if (threadIdx.x == 0) s_count = 0;
         __syncthreads();
         const int k = base + threadIdx.x * gridDim.x;
-        if (k < n && a.dst[k] >= 0) {
-            double rho;
-            const bool finished = a.flag && a.flag[k] && expm_poly_shift(a, k, rho) == 0 && rho == rho;
-            if (!finished) s_list[atomicAdd(&s_count, 1)] = k;
-        }
+        if (k < n && a.dst[k] >= 0 && !expm_poly_finished(a, k)) s_list[atomicAdd(&s_count, 1)] = k;
         __syncthreads();
         const int count = s_count;
         for (int j = 0; j < count; j++) {
@@ -612,10 +674,9 @@ __device__ __forceinline__ bool expm_await_flag(const unsigned long long *f, uns
         asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(f) : "memory");
         if (v == gen) return true;
         if ((it & 255) == 255) {
-            unsigned long long now;
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
+            const unsigned long long now = globaltimer_ns();
             if (t0 == 0) t0 = now;
-            else if (now - t0 > 4000000000ull) { atomicExch(err, 4); return false; }
+            else if (now - t0 > HB2_WAIT_LIMIT_NS) { atomicExch(err, WAIT_EXPM_POWERS); return false; }
         }
     }
 }
@@ -635,20 +696,9 @@ __global__ void __launch_bounds__(256, 1) expm_powers_kernel(ExpmPowersArgs pa) 
     unsigned long long *flags = pa.flags + (size_t)grp * EXPM_POW_TERMS;
     if (m == 1) {
         load_rate_matrix<64, LD64, 256>(pa.a, X0, tid, entry);        // X0 = A_ref^T, zero padded
-        if (tid < 64) {
-            double s = 0.0;
-            for (int j = 0; j < 64; j++) s += fabs(X0[j * LD64 + tid]);   // column sums of A^T = row sums of A
-            red[tid] = s;
-        }
-        __syncthreads();
-        if (tid < 32) {                      // max and NaN / inf scan of the 64 row sums, one warp (fmax is exact)
-            double mx = fmax(0.0, fmax(red[tid], red[tid + 32]));
-            bool bad = !(red[tid] == red[tid]) || !(red[tid + 32] == red[tid + 32]) || isinf(red[tid]) || isinf(red[tid + 32]);
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-            bad = __any_sync(0xffffffffu, bad);
-            if (tid == 0) s_nu = (bad || !(mx > 0.0)) ? 0.0 : mx;
-        }
+        bool bad;
+        const double mx = expm64_norm(X0, red, tid, bad);
+        if (tid == 0) s_nu = (bad || !(mx > 0.0)) ? 0.0 : mx;
         __syncthreads();
         const double nu = s_nu;
         if (tid == 0) {                      // the weight is the classification's (expm_classify_result), written beside this
@@ -741,7 +791,7 @@ __global__ void __launch_bounds__(256, 3) expm_poly_kernel(ExpmArgs a, ExpmTcOut
     double c[EXPM_POW_TERMS];
     int cur = -1;
     double nu = 0.0, wref = 1.0;
-    const size_t out_pt = (size_t)e, out_ptf = (size_t)row * 68 + col, out_pb = (size_t)sl * 256 + tid;
+    const int out_pt = e, out_ptf = tc_ptf_index(row, col), out_pb = tc_pb_index(row, col);   // out_pb = 256 sl + tid
     for (int i = 0; i < EXPM_POLY_CHUNK; i++) {
         const int slot = s_slot[i];
         if (slot < 0) continue;
@@ -752,15 +802,10 @@ __global__ void __launch_bounds__(256, 3) expm_poly_kernel(ExpmArgs a, ExpmTcOut
             for (int m = 1; m < EXPM_POW_TERMS; m++) c[m] = __ldcg(pw + (size_t)m * 4096);
             nu = a.groups[cur].nu; wref = a.groups[cur].weight;
         }
-        const double rho = nu * (s_wgt[i] / wref);
-        double x = rho;
-        int shift = 0;
-        if (rho > EXPM_POLY_THETA) {
-            frexp(rho / EXPM_POLY_THETA, &shift);
-            if (shift > 900) continue;                                // the finishing kernel writes NaN for absurd rates
-            shift = max(shift, 0);
-            x = ldexp(rho, -shift);
-        }
+        double rho;
+        const int shift = expm_poly_shift(nu, wref, s_wgt[i], rho);
+        if (expm_poly_nan(shift, rho)) continue;                      // the finishing kernel writes NaN
+        const double x = shift > 0 ? ldexp(rho, -shift) : rho;
         // p(x) = 1 + x (c1 + c3 x^2 + .. + c23 x^22) + x^2 (c2 + c4 x^2 + .. + c24 x^22): two interleaved Horner chains in
         // x^2 halve the dependent-FMA depth
         static_assert(EXPM_POW_TERMS == 25, "the even/odd split below assumes degree 24");
@@ -771,7 +816,6 @@ __global__ void __launch_bounds__(256, 3) expm_poly_kernel(ExpmArgs a, ExpmTcOut
         double v = fma(vo, x, fma(ve, x2, unit));
         const size_t sidx = (size_t)slot;
         if (shift > 0) { __stcg(a.PT + sidx * 4096 + out_pt, v); continue; }
-        if (!(rho == rho)) continue;                                  // NaN input: the finishing kernel writes NaN
         v = (pad || v < 0.0) ? 0.0 : v;
         // column sums over this slice's 4 rows (lanes t, t^1, t^2, t^3 share a column), diagonal element excluded
         double part = (row == col) ? 0.0 : v;
@@ -782,12 +826,8 @@ __global__ void __launch_bounds__(256, 3) expm_poly_kernel(ExpmArgs a, ExpmTcOut
         if (row != col) {                                             // the diagonal is written after the cluster barrier
             __stcg(a.PT + sidx * 4096 + out_pt, v);
             if (tc.PB) {
-                const float vf = (float)v;
-                tc.PTf[sidx * 4352 + out_ptf] = vf;
-                const float hi = tf32_rn_dev(vf);
-                float *pb = tc.PB + sidx * 8192 + out_pb;             // canonical tile: chunk = row/4 = sl, offset col*4 + row%4 = tid
-                pb[0] = hi;
-                pb[4096] = tf32_rn_dev((float)(v - (double)hi));
+                tc.PTf[sidx * TC_PTF_FLOATS + out_ptf] = (float)v;
+                tc_split_store<true>(tc.PB + sidx * TC_PB_FLOATS, out_pb, v);
             }
         }
     }
@@ -804,14 +844,34 @@ __global__ void __launch_bounds__(256, 3) expm_poly_kernel(ExpmArgs a, ExpmTcOut
         const size_t sidx = (size_t)s_slot[i];
         a.PT[sidx * 4096 + c * 64 + c] = d;
         if (tc.PB) {
-            tc.PTf[sidx * 4352 + c * 68 + c] = (float)d;
-            const float hi = tf32_rn_dev((float)d);
-            float *pb = tc.PB + sidx * 8192 + (c >> 2) * 256 + c * 4 + (c & 3);
-            pb[0] = hi;
-            pb[4096] = tf32_rn_dev((float)(d - (double)hi));
+            tc.PTf[sidx * TC_PTF_FLOATS + tc_ptf_index(c, c)] = (float)d;
+            tc_split_store<true>(tc.PB + sidx * TC_PB_FLOATS, tc_pb_index(c, c), d);
         }
     }
     cluster.sync();                                                   // peers may still be reading this slice's partials
+}
+
+// Explicit-form mixtures (BS-REL, reference tree.cpp:3047-3089): PT[slot_i] = sum_k w[i][k] * comp[i*K + k], components
+// added in order k = 0..K-1 (deterministic); 64-state tensor partitions also get the split tiles and the fp32 table, the
+// split rounded by tf32_rn (unlike the exponential's epilogues).
+// One CTA per node; comp = scratch matrices [n*K][Dp*Dp] in the PT layout (transposed).
+__global__ void __launch_bounds__(256) mix_reduce_kernel(const double *__restrict__ comp, const double *__restrict__ w,
+                                                          const int *__restrict__ slots, int K, int Dp, double *__restrict__ PT,
+                                                          float *__restrict__ PB, float *__restrict__ PTf) {
+    const size_t slot = slots[blockIdx.x];
+    const int dpdp = Dp * Dp;
+    double *dst = PT + slot * dpdp;
+    const double *src = comp + (size_t)blockIdx.x * K * dpdp;
+    const double *wk = w + (size_t)blockIdx.x * K;
+    for (int o = threadIdx.x; o < dpdp; o += 256) {
+        double s = 0.0;
+        for (int k = 0; k < K; k++) s += wk[k] * src[(size_t)k * dpdp + o];
+        dst[o] = s;
+    }
+    if (PB && Dp == 64) {
+        __syncthreads();                         // this CTA's own global writes are visible to it after the barrier
+        tc_store_operands<false>(dst, 64, PB + slot * TC_PB_FLOATS, PTf + slot * TC_PTF_FLOATS, threadIdx.x);
+    }
 }
 
 // Small state spaces (Dp <= 32): one CTA of 128 threads per matrix, plain shared-memory products.
@@ -850,8 +910,8 @@ __device__ __forceinline__ double expm_small_dot(const double *X, const double *
 template <int LD>
 __device__ __forceinline__ double expm_small_poly(const double *A1, const double *A2, const double *A3, int q, int r, int c) {
     int o = r * LD + c;
-    double v = taylor_c(4 * q + 1) * A1[o] + taylor_c(4 * q + 2) * A2[o] + taylor_c(4 * q + 3) * A3[o];
-    if (r == c) v += taylor_c(4 * q);
+    double v = c_taylor[4 * q + 1] * A1[o] + c_taylor[4 * q + 2] * A2[o] + c_taylor[4 * q + 3] * A3[o];
+    if (r == c) v += c_taylor[4 * q];
     return v;
 }
 
@@ -869,83 +929,6 @@ __device__ __forceinline__ double expm_small_diag(const double *R, int c) {
     return fmax(1.0 - s, 0.0);
 }
 
-template <int DP>
-__global__ void __launch_bounds__(128) expm_small_kernel(ExpmArgs a) {
-    constexpr int LD = DP + 1;
-    extern __shared__ __align__(16) double sm[];          // 6 matrices of DP*LD doubles (expm_small_smem_bytes)
-    double *A1 = sm, *A2 = A1 + DP * LD, *A3 = A2 + DP * LD, *A4 = A3 + DP * LD, *R = A4 + DP * LD, *T = R + DP * LD;
-    __shared__ double red[DP];
-    __shared__ int s_shift;
-    const int tid = threadIdx.x, D = a.D;
-    if (a.dst[blockIdx.x] < 0) return;
-    double *out = a.PT + (size_t)a.dst[blockIdx.x] * DP * DP;
-    load_rate_matrix<DP, LD, 128>(a, A1, tid);
-    if (a.is_trans) {
-        for (int idx = tid; idx < DP * DP; idx += 128) out[idx] = A1[(idx / DP) * LD + idx % DP];
-        return;
-    }
-    if (tid < DP) red[tid] = expm_small_norm<DP, LD>(A1, tid);
-    __syncthreads();
-    if (tid == 0) s_shift = expm_small_shift<DP>(red);
-    __syncthreads();
-    const int shift = s_shift;
-    if (shift < 0 || shift > 900) {
-        for (int idx = tid; idx < DP * DP; idx += 128) out[idx] = __longlong_as_double(0x7ff8000000000000LL);
-        return;
-    }
-    if (shift > 0) {
-        const double sc = exp2i(-shift);
-        for (int idx = tid; idx < DP * DP; idx += 128) A1[(idx / DP) * LD + idx % DP] *= sc;
-        __syncthreads();
-    }
-    auto mm = [&](double *Cm, const double *X, const double *Y) {      // Cm = X*Y (Cm distinct from X,Y)
-        for (int idx = tid; idx < DP * DP; idx += 128) {
-            int r = idx / DP, c = idx % DP;
-            Cm[r * LD + c] = expm_small_dot<DP, LD>(X, Y, r, c);
-        }
-        __syncthreads();
-    };
-    mm(A2, A1, A1); mm(A3, A2, A1); mm(A4, A2, A2);
-    for (int idx = tid; idx < DP * DP; idx += 128) R[(idx / DP) * LD + idx % DP] = expm_small_poly<LD>(A1, A2, A3, 3, idx / DP, idx % DP);
-    __syncthreads();
-    for (int q = 2; q >= 0; q--) {
-        mm(T, R, A4);
-        for (int idx = tid; idx < DP * DP; idx += 128) { int r = idx / DP, c = idx % DP; R[r * LD + c] = T[r * LD + c] + expm_small_poly<LD>(A1, A2, A3, q, r, c); }
-        __syncthreads();
-    }
-    for (int s = 0; s < shift; s++) {
-        mm(T, R, R);
-        for (int idx = tid; idx < DP * DP; idx += 128) { int o = (idx / DP) * LD + idx % DP; R[o] = T[o]; }
-        __syncthreads();
-    }
-    for (int idx = tid; idx < DP * DP; idx += 128) {
-        int j = idx / DP, k = idx % DP;
-        R[j * LD + k] = expm_small_clamp(R[j * LD + k], j, k, D);
-    }
-    __syncthreads();
-    if (tid < D) R[tid * LD + tid] = expm_small_diag<DP, LD>(R, tid);
-    __syncthreads();
-    for (int idx = tid; idx < DP * DP; idx += 128) out[idx] = R[(idx / DP) * LD + idx % DP];
-}
-
-// ------------------------------------------------------------------------------------------------
-// expm_rates_kernel (hb2_batch_site_rates): P = exp(r_s A_b) for every (set s, branch b) of a chunk, A_b the resident rate
-// matrix of the call's class (d_Qres, row-major D*D), scaled by the set's rate while it is loaded.  A team of
-// expm_rates_team(DP) threads owns one matrix and runs expm_small_kernel's steps entry for entry (same shift, Horner
-// order, fma order, clamping and diagonal repair), so that rate 1 gives the resident path's matrices; 4 and 8
-// states pack 8 and 2 matrices into a CTA, one thread per entry.  Output: PT[s][b][DP*DP], transposed like every P.
-// ------------------------------------------------------------------------------------------------
-struct ExpmRatesArgs {
-    const double *Q;          // [B][D*D] resident rate matrices of the class
-    const double *rate;       // [sets]
-    double *PT;               // [sets][B][DP*DP]
-    int D, B;
-    long long n;              // sets * B matrices
-};
-
-__host__ __device__ constexpr int expm_rates_team(int DP) { return DP * DP < 128 ? DP * DP : 128; }
-constexpr size_t expm_rates_smem_bytes(int DP) { return (size_t)(128 / expm_rates_team(DP)) * expm_small_smem_bytes(DP); }
-
 // Barrier of one team: the CTA, a pair of warps (named barrier 1 + team), or a half-warp.
 template <int T>
 __device__ __forceinline__ void team_sync(int team) {
@@ -960,30 +943,19 @@ __device__ __forceinline__ void team_sync(int team) {
     }
 }
 
-template <int DP>
-__global__ void __launch_bounds__(128) expm_rates_kernel(ExpmRatesArgs a) {
-    constexpr int LD = DP + 1, T = expm_rates_team(DP), M = 128 / T, MS = DP * LD;
-    extern __shared__ __align__(16) double sm[];          // M teams x 6 matrices of DP*LD doubles (expm_rates_smem_bytes)
-    __shared__ double red_all[M][DP];
-    __shared__ int shift_all[M];
-    const int team = threadIdx.x / T, lt = threadIdx.x % T, D = a.D;
-    const long long e = (long long)blockIdx.x * M + team;
-    if (e >= a.n) return;
-    double *A1 = sm + (size_t)team * 6 * MS, *A2 = A1 + MS, *A3 = A2 + MS, *A4 = A3 + MS, *R = A4 + MS, *Tm = R + MS;
-    double *red = red_all[team];
-    const double r = a.rate[e / a.B];
-    const double *Q = a.Q + (size_t)(e % a.B) * D * D;
-    double *out = a.PT + (size_t)e * DP * DP;
-    for (int idx = lt; idx < DP * DP; idx += T) {
-        const int i = idx / DP, j = idx - i * DP;
-        A1[j * LD + i] = (i < D && j < D) ? r * Q[(size_t)i * D + j] : 0.0;
-    }
-    team_sync<T>(team);
+// The small-state exponential of one matrix by a team of T threads (lt = 0..T-1), from the loaded, transposed A1 to the
+// stored result: norm, shift (NaN for a NaN or infinite input or absurd rates), scaling, A^2, A^3, A^4, Horner blocks of
+// degree 15, squarings, clamp, diagonal repair and the store to out.  A1 is the first of the team's 6 matrices of DP*LD
+// doubles; red [DP] and s_shift are the team's shared scratch.  Every exit is team-uniform.
+template <int DP, int T>
+__device__ __forceinline__ void expm_small_body(double *A1, double *red, int &s_shift, int lt, int team, int D, double *out) {
+    constexpr int LD = DP + 1, MS = DP * LD;
+    double *A2 = A1 + MS, *A3 = A2 + MS, *A4 = A3 + MS, *R = A4 + MS, *Tm = R + MS;
     if (lt < DP) red[lt] = expm_small_norm<DP, LD>(A1, lt);
     team_sync<T>(team);
-    if (lt == 0) shift_all[team] = expm_small_shift<DP>(red);
+    if (lt == 0) s_shift = expm_small_shift<DP>(red);
     team_sync<T>(team);
-    const int shift = shift_all[team];
+    const int shift = s_shift;
     if (shift < 0 || shift > 900) {
         for (int idx = lt; idx < DP * DP; idx += T) out[idx] = __longlong_as_double(0x7ff8000000000000LL);
         return;
@@ -993,10 +965,10 @@ __global__ void __launch_bounds__(128) expm_rates_kernel(ExpmRatesArgs a) {
         for (int idx = lt; idx < DP * DP; idx += T) A1[(idx / DP) * LD + idx % DP] *= sc;
         team_sync<T>(team);
     }
-    auto mm = [&](double *Cm, const double *X, const double *Y) {
+    auto mm = [&](double *Cm, const double *X, const double *Y) {      // Cm = X*Y (Cm distinct from X,Y)
         for (int idx = lt; idx < DP * DP; idx += T) {
-            int rr = idx / DP, c = idx % DP;
-            Cm[rr * LD + c] = expm_small_dot<DP, LD>(X, Y, rr, c);
+            int r = idx / DP, c = idx % DP;
+            Cm[r * LD + c] = expm_small_dot<DP, LD>(X, Y, r, c);
         }
         team_sync<T>(team);
     };
@@ -1005,7 +977,7 @@ __global__ void __launch_bounds__(128) expm_rates_kernel(ExpmRatesArgs a) {
     team_sync<T>(team);
     for (int q = 2; q >= 0; q--) {
         mm(Tm, R, A4);
-        for (int idx = lt; idx < DP * DP; idx += T) { int rr = idx / DP, c = idx % DP; R[rr * LD + c] = Tm[rr * LD + c] + expm_small_poly<LD>(A1, A2, A3, q, rr, c); }
+        for (int idx = lt; idx < DP * DP; idx += T) { int r = idx / DP, c = idx % DP; R[r * LD + c] = Tm[r * LD + c] + expm_small_poly<LD>(A1, A2, A3, q, r, c); }
         team_sync<T>(team);
     }
     for (int s = 0; s < shift; s++) {
@@ -1021,6 +993,60 @@ __global__ void __launch_bounds__(128) expm_rates_kernel(ExpmRatesArgs a) {
     if (lt < D) R[lt * LD + lt] = expm_small_diag<DP, LD>(R, lt);
     team_sync<T>(team);
     for (int idx = lt; idx < DP * DP; idx += T) out[idx] = R[(idx / DP) * LD + idx % DP];
+}
+
+template <int DP>
+__global__ void __launch_bounds__(128) expm_small_kernel(ExpmArgs a) {
+    constexpr int LD = DP + 1;
+    extern __shared__ __align__(16) double sm[];          // 6 matrices of DP*LD doubles (expm_small_smem_bytes)
+    __shared__ double red[DP];
+    __shared__ int s_shift;
+    const int tid = threadIdx.x;
+    if (a.dst[blockIdx.x] < 0) return;
+    double *out = a.PT + (size_t)a.dst[blockIdx.x] * DP * DP;
+    load_rate_matrix<DP, LD, 128>(a, sm, tid);
+    if (a.is_trans) {
+        for (int idx = tid; idx < DP * DP; idx += 128) out[idx] = sm[(idx / DP) * LD + idx % DP];
+        return;
+    }
+    expm_small_body<DP, 128>(sm, red, s_shift, tid, 0, a.D, out);
+}
+
+// ------------------------------------------------------------------------------------------------
+// expm_rates_kernel (hb2_batch_site_rates): P = exp(r_s A_b) for every (set s, branch b) of a chunk, A_b the resident rate
+// matrix of the call's class (d_Qres, row-major D*D), scaled by the set's rate while it is loaded.  A team of
+// expm_rates_team(DP) threads owns one matrix and runs expm_small_body as expm_small_kernel does, so that rate 1 gives
+// the resident path's matrices; 4 and 8 states pack 8 and 2 matrices into a CTA, one thread per entry.  Output: PT[s][b][DP*DP], transposed like every P.
+// ------------------------------------------------------------------------------------------------
+struct ExpmRatesArgs {
+    const double *Q;          // [B][D*D] resident rate matrices of the class
+    const double *rate;       // [sets]
+    double *PT;               // [sets][B][DP*DP]
+    int D, B;
+    long long n;              // sets * B matrices
+};
+
+__host__ __device__ constexpr int expm_rates_team(int DP) { return DP * DP < 128 ? DP * DP : 128; }
+constexpr size_t expm_rates_smem_bytes(int DP) { return (size_t)(128 / expm_rates_team(DP)) * expm_small_smem_bytes(DP); }
+
+template <int DP>
+__global__ void __launch_bounds__(128) expm_rates_kernel(ExpmRatesArgs a) {
+    constexpr int LD = DP + 1, T = expm_rates_team(DP), M = 128 / T;
+    extern __shared__ __align__(16) double sm[];          // M teams x 6 matrices of DP*LD doubles (expm_rates_smem_bytes)
+    __shared__ double red_all[M][DP];
+    __shared__ int shift_all[M];
+    const int team = threadIdx.x / T, lt = threadIdx.x % T, D = a.D;
+    const long long e = (long long)blockIdx.x * M + team;
+    if (e >= a.n) return;
+    double *A1 = sm + (size_t)team * 6 * DP * LD;
+    const double r = a.rate[e / a.B];
+    const double *Q = a.Q + (size_t)(e % a.B) * D * D;
+    for (int idx = lt; idx < DP * DP; idx += T) {
+        const int i = idx / DP, j = idx - i * DP;
+        A1[j * LD + i] = (i < D && j < D) ? r * Q[(size_t)i * D + j] : 0.0;
+    }
+    team_sync<T>(team);
+    expm_small_body<DP, T>(A1, red_all[team], shift_all[team], lt, team, D, a.PT + (size_t)e * DP * DP);
 }
 
 
@@ -2143,10 +2169,9 @@ __device__ __forceinline__ bool peer_await(const PeerBuf &b, int src_rank) {
         asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(f) : "memory");
         if (v == b.gen) return true;
         if ((it & 255) == 255) {
-            unsigned long long now;
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
+            const unsigned long long now = globaltimer_ns();
             if (t0 == 0) t0 = now;
-            else if (now - t0 > 20000000000ull) { atomicExch(b.err, 3); return false; }      // 20 s: a rank is gone
+            else if (now - t0 > HB2_PEER_WAIT_LIMIT_NS) { atomicExch(b.err, WAIT_PEER); return false; }
         }
     }
 }

@@ -24,7 +24,7 @@
 // bit.
 #pragma once
 #include "hb2_kernels_fp64.cuh"
-#include "hb2_kernels_tc.cuh"      // step encoding (WALK_*, STEP_*), globaltimer_ns, HB2_WAIT_LIMIT_NS
+#include "hb2_kernels_tc.cuh"      // step encoding (WALK_*, STEP_*)
 
 namespace hb2 {
 
@@ -104,7 +104,7 @@ __global__ void __launch_bounds__(LANES_THREADS, LANES_CTAS_PER_SM) prune64_lane
                 if ((it & 63) == 63) {                                          // never hang the GPU: time-bounded
                     const unsigned long long now = globaltimer_ns();
                     if (t0 == 0) t0 = now;
-                    else if (now - t0 > HB2_WAIT_LIMIT_NS) { atomicExch(w.err, 2); break; }
+                    else if (now - t0 > HB2_WAIT_LIMIT_NS) { atomicExch(w.err, WAIT_LANE); break; }
                 }
             }
         }

@@ -38,9 +38,6 @@
 namespace hb2 {
 
 constexpr int TC_TILE_P = 128;                 // patterns per warpgroup (the wgmma N)
-constexpr int TC_PB_FLOATS = 2 * 4096;         // per (class, branch): Ph tile + Pl tile in canonical layout
-constexpr int TC_PTF_ROW = 68;                 // floats per row of the fp32 P^T table (64 + 4 padding: 272-byte rows)
-constexpr int TC_PTF_FLOATS = 64 * TC_PTF_ROW; // per (class, branch)
 constexpr int TC_X_BYTES = 2 * 16 * 128 * 16;  // B operand: Xh | Xl, [16 chunks][128 patterns][4] fp32 each
 constexpr int TC_D_ROW = 68;                   // floats per pattern row of the shared accumulator read-back buffer
 constexpr int TC_D_BYTES = 128 * TC_D_ROW * 4;
@@ -73,15 +70,6 @@ __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
 __device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ unsigned long long globaltimer_ns() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
-// Device-side waits are bounded by TIME (4 s of globaltimer), not by an iteration count: a slow producer (another
-// partition or process sharing the GPU, fewer co-resident CTAs than planned) only makes the pass slower; a protocol bug
-// still surfaces as an error flag (the host returns an error), never as a hung GPU.
-constexpr unsigned long long HB2_WAIT_LIMIT_NS = 4000000000ull;
 __device__ __forceinline__ bool mbar_wait(uint64_t *bar, uint32_t parity, int *err_flag) {
     const uint32_t addr = smem_u32(bar);
     unsigned long long t0 = 0;
@@ -100,7 +88,7 @@ __device__ __forceinline__ bool mbar_wait(uint64_t *bar, uint32_t parity, int *e
             else if (now - t0 > HB2_WAIT_LIMIT_NS) break;
         }
     }
-    atomicExch(err_flag, 1);
+    atomicExch(err_flag, WAIT_TC_STAGING);
     return false;
 }
 __device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
@@ -112,11 +100,6 @@ __device__ __forceinline__ uint32_t elect_one() {
     uint32_t pred;
     asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}" : "=r"(pred));
     return pred;
-}
-// round-to-nearest (ties away from zero) to tf32, i.e. what cvt.rna.tf32.f32 computes, but with two full-rate integer
-// instructions: the conversion instruction issues at a quarter of the ALU rate and dominated the operand-split phase
-__device__ __forceinline__ float tf32_rn(float x) {
-    return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
 }
 // ---- warpgroup MMA (sm_90a) ----------------------------------------------------------------------------------------
 // Shared-memory matrix descriptor, no swizzle, K-major: start>>4 @0, LBO>>4 @16 (next 16-byte core-matrix column along
@@ -178,37 +161,6 @@ __host__ __device__ constexpr int wg_parent(int x) { return (x & ~15) + ((x & 15
 __device__ __forceinline__ void store_x_chunk(uint8_t *xs, int q, int pattern, const uint32_t *hi, const uint32_t *lo) {
     *reinterpret_cast<uint4 *>(xs + (size_t)q * 2048 + pattern * 16) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
     *reinterpret_cast<uint4 *>(xs + TC_X_BYTES / 2 + (size_t)q * 2048 + pattern * 16) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-}
-
-// Explicit-form mixtures (BS-REL, reference tree.cpp:3047-3089): PT[slot_i] = sum_k w[i][k] * comp[i*K + k], components
-// added in order k = 0..K-1 (deterministic); 64-state tensor partitions also get the split tiles and the fp32 table.
-// One CTA per node; comp = scratch matrices [n*K][Dp*Dp] in the PT layout (transposed).
-__global__ void __launch_bounds__(256) mix_reduce_kernel(const double *__restrict__ comp, const double *__restrict__ w,
-                                                          const int *__restrict__ slots, int K, int Dp, double *__restrict__ PT,
-                                                          float *__restrict__ PB, float *__restrict__ PTf) {
-    const size_t slot = slots[blockIdx.x];
-    const int dpdp = Dp * Dp;
-    double *dst = PT + slot * dpdp;
-    const double *src = comp + (size_t)blockIdx.x * K * dpdp;
-    const double *wk = w + (size_t)blockIdx.x * K;
-    for (int o = threadIdx.x; o < dpdp; o += 256) {
-        double s = 0.0;
-        for (int k = 0; k < K; k++) s += wk[k] * src[(size_t)k * dpdp + o];
-        dst[o] = s;
-    }
-    if (PB && Dp == 64) {
-        __syncthreads();                         // this CTA's own global writes are visible to it after the barrier
-        float *pb = PB + slot * TC_PB_FLOATS;
-        float *pf = PTf + slot * TC_PTF_FLOATS;
-        for (int o = threadIdx.x; o < 4096; o += 256) {
-            const int chunk = o >> 8, n = (o >> 2) & 63, kk = chunk * 4 + (o & 3);
-            const double p = dst[kk * 64 + n];
-            const float hi = tf32_rn((float)p);
-            pb[o] = hi;
-            pb[4096 + o] = tf32_rn((float)(p - (double)hi));
-            pf[(o >> 6) * TC_PTF_ROW + (o & 63)] = (float)dst[o];
-        }
-    }
 }
 
 // Power-of-two renormalisation of a pattern's 64 conditionals: max -> [0.5,1).  `force` = false only rescales when the
@@ -404,7 +356,7 @@ __global__ void __launch_bounds__(256, 1) prune64_tc_walk_kernel(WalkArgs w) {
                 if ((it & 255) == 255) {                                       // never hang the GPU: time-bounded
                     const unsigned long long now = globaltimer_ns();
                     if (t0 == 0) t0 = now;
-                    else if (now - t0 > HB2_WAIT_LIMIT_NS) { atomicExch(a.err, 2); bailed = true; }
+                    else if (now - t0 > HB2_WAIT_LIMIT_NS) { atomicExch(a.err, WAIT_LANE); bailed = true; }
                 }
 #pragma unroll
                 for (int q = 0; q < 16; q++) x4[q] = ld_relaxed_u4(xrow + (size_t)q * 128);
