@@ -249,6 +249,7 @@ struct BatchShape {
     int64_t ent = 0, in = 0;                  // rows per set through launch_expm (R; 0 for site rates) and input doubles per set
     int64_t side = 0;                         // branches per set with outside scratch (branch rows, leaf support: B; else 0)
     int64_t rows = 0, sup = 0;                // doubles per set of row results (branch rows: R) and of support (leaf support: L*D)
+    int64_t joint = 0;                        // internal nodes per set with an argument row and a state (joint ancestors: I)
 };
 
 }  // namespace
@@ -314,6 +315,11 @@ struct hb2_partition {
         // [sets][R] (branch rows) or the leaf support [sets][L][D] (leaf support)
         DeviceBuffer<double> side, rows, sup;
         DeviceBuffer<int> side_ex;
+        // hb2_batch_joint_ancestors only (sh.joint = I; empty for every other call): the argument table [sets][I][64], the
+        // node states [sets][I] and the joint log-likelihoods [sets]
+        DeviceBuffer<unsigned char> arg;
+        DeviceBuffer<long long> states;
+        DeviceBuffer<double> jlnl;
         // Sizes the workspace for chunks of `sh`.  A chunk that does not fit re-sizes the whole workspace for this call,
         // after releasing it, so that memory stays at one call's chunk footprint (~8 GB) instead of adding up the largest
         // buffers of different calls' shapes.
@@ -322,7 +328,8 @@ struct hb2_partition {
             if (sets <= (int64_t)out.size() && ne <= (int64_t)slot.size() && sets * sh.gk <= ex.G && sets * sh.in <= (int64_t)V.size() &&
                 nr * sh.mat <= (int64_t)PT.size() && sets * I * sh.vec <= (int64_t)cond.size() && sets * L <= (int64_t)col.size() &&
                 sets * sh.side * 128 <= (int64_t)side.size() && sets * sh.rows <= (int64_t)rows.size() &&
-                sets * sh.sup <= (int64_t)sup.size())
+                sets * sh.sup <= (int64_t)sup.size() && sets * sh.joint * 64 <= (int64_t)arg.size() &&
+                sets * sh.joint <= (int64_t)states.size() && (sh.joint == 0 || sets <= (int64_t)jlnl.size()))
                 return 0;
             CU(cudaStreamSynchronize(stream));
             *this = BatchWorkspace();
@@ -331,7 +338,8 @@ struct hb2_partition {
                 node_ex.alloc((size_t)sets * I) || row.alloc(sh.row_off.size()) || col.alloc((size_t)sets * L) || pi.alloc(64) ||
                 h_slot.alloc(ne) || h_pat.alloc(sets) || h_col.alloc((size_t)sets * L) ||
                 (sh.side && (side.alloc((size_t)sets * sh.side * 128) || side_ex.alloc((size_t)sets * sh.side * 2))) ||
-                (sh.rows && rows.alloc((size_t)sets * sh.rows)) || (sh.sup && sup.alloc((size_t)sets * sh.sup))) {
+                (sh.rows && rows.alloc((size_t)sets * sh.rows)) || (sh.sup && sup.alloc((size_t)sets * sh.sup)) ||
+                (sh.joint && (arg.alloc((size_t)sets * sh.joint * 64) || states.alloc((size_t)sets * sh.joint) || jlnl.alloc(sets)))) {
                 *this = BatchWorkspace();     // fits nothing: the next call sizes it again
                 return 1;
             }
@@ -1729,7 +1737,10 @@ int hb2_evaluate_classes(hb2_partition *p, const double *weights, int64_t nUpdat
 // branch_rows_kernel; MEME's branch-level empirical Bayes factors).  siteLnL is nullable there.
 // LeafSupport: Sites (weights == nullptr) or MixtureSites, and after its pruning every leaf's support [nSets][L][D]
 // (leaf_support_kernel; MEME's and PRIME's --impute-states).  siteLnL is nullable there.
-enum class BatchEntry { Sites, MixtureSites, Columns, Simulate, Rates, BranchRows, LeafSupport };
+// JointAncestors: Sites (weights == nullptr) or MixtureSites, its pruning only when siteLnL is given, then the joint ML
+// states of every internal node (nodeStates [nSets][I], jointLnL; joint_ancestors_kernel; ancestral.build at every site
+// of FEL, MEME and PRIME).
+enum class BatchEntry { Sites, MixtureSites, Columns, Simulate, Rates, BranchRows, LeafSupport, JointAncestors };
 struct BatchCall {
     BatchEntry entry;
     int64_t templateId, nSets, K;
@@ -1744,6 +1755,7 @@ struct BatchCall {
     const double *rates = nullptr;
     double *rowLnL = nullptr;
     double *support = nullptr;
+    double *jointLnL = nullptr;
 };
 
 // Sets per chunk of hb2_batch_site_rates, whatever the memory rule allows: at 4 states and 256 taxa a chunk of this many
@@ -1753,7 +1765,8 @@ constexpr int64_t RATES_MAX_SETS = 65536;
 // Every refusal of the batch entry points, before anything is launched or written.
 static int check_batch(const hb2_partition *p, const BatchCall &c) {
     const bool rows = c.entry == BatchEntry::BranchRows, leaves = c.entry == BatchEntry::LeafSupport;
-    const bool sites = c.entry == BatchEntry::Sites || c.entry == BatchEntry::MixtureSites || rows || leaves;
+    const bool joint = c.entry == BatchEntry::JointAncestors;
+    const bool sites = c.entry == BatchEntry::Sites || c.entry == BatchEntry::MixtureSites || rows || leaves || joint;
     const bool sim = c.entry == BatchEntry::Simulate;
     const char *fn = sim ? "hb2_batch_site_simulate" : "hb2_batch_column_likelihoods";
     if (!p) return fail(c.entry == BatchEntry::Sites ? "null argument" : "null partition");
@@ -1763,9 +1776,10 @@ static int check_batch(const hb2_partition *p, const BatchCall &c) {
                         "would equal siteLnL)");
         if (rows && !c.rowLnL) return fail("hb2_batch_branch_component_likelihoods: rowLnL must not be null");
         if (leaves && !c.support) return fail("hb2_batch_leaf_support: support must not be null");
+        if (joint && !c.nodeStates) return fail("hb2_batch_joint_ancestors: nodeStates must not be null");
         if (c.entry == BatchEntry::MixtureSites && !c.weights) return fail("weights must not be null");
         if (c.entry == BatchEntry::MixtureSites && !c.formulaValues) return fail("formulaValues must not be null");
-        if (!c.formulaValues || !c.rootFreqs || (!c.siteLnL && !rows && !leaves) || !c.patternOf) return fail("null argument");
+        if (!c.formulaValues || !c.rootFreqs || (!c.siteLnL && !rows && !leaves && !joint) || !c.patternOf) return fail("null argument");
         if (c.nSets < 0) return fail("bad set count");
     } else {
         if (c.nSets < 0) return fail("%s: nSets=%lld is negative", fn, (long long)c.nSets);
@@ -1839,6 +1853,10 @@ static BatchShape batch_shape(const hb2_partition *p, const BatchCall &c) {
         sh.side = B;
         sh.sup = p->L * D;
         per_set += (double)B * 2 * (64 * 8 + 4) + (double)sh.sup * 8;
+    }
+    if (c.entry == BatchEntry::JointAncestors) {    // the argument table and the node states
+        sh.joint = p->I;
+        per_set += (double)p->I * (64 + 8) + 8;
     }
     sh.sets = std::min<int64_t>({c.nSets, std::max<int64_t>(1, (int64_t)(8.0e9 / (per_set + sim_bytes))), 1024});
     sh.ent = sh.R;
@@ -1950,7 +1968,8 @@ static int exponentiate_chunk(hb2_partition *p, const BatchCall &c, const BatchS
 
 // Likelihoods of sets s0 .. s0+nb-1 from the chunk's P area.  Branch rows and leaf support: then branch_rows_kernel or
 // leaf_support_kernel on the inside pass's node vectors (so siteLnL stays the likelihood entry point's bit for bit), and the
-// chunk's rows or support go down.
+// chunk's rows or support go down.  Joint ancestors: the inside pass only when siteLnL is given, then
+// joint_ancestors_kernel, and the chunk's node states and joint log-likelihoods go down.
 static int score_chunk(hb2_partition *p, const BatchCall &c, const BatchShape &sh, int64_t s0, int64_t nb) {
     hb2_partition::BatchWorkspace &ws = p->batch;
     const int64_t L = p->L;
@@ -1964,10 +1983,21 @@ static int score_chunk(hb2_partition *p, const BatchCall &c, const BatchShape &s
     }
     const hb2::BatchPruneArgs ba = batch_prune_args(p, c.columns ? (const int *)ws.col : (const int *)p->d_leaf,
                                                     c.columns ? (int)nb : (int)p->Sp, (int)sh.R);
-    if (c.weights) hb2::prune_batch_kernel<true><<<(unsigned)nb, 64, 0, p->stream>>>(ba);
-    else hb2::prune_batch_kernel<false><<<(unsigned)nb, 64, 0, p->stream>>>(ba);
-    p->launches++;
-    CU(cudaGetLastError());
+    if (c.entry != BatchEntry::JointAncestors || c.siteLnL) {
+        if (c.weights) hb2::prune_batch_kernel<true><<<(unsigned)nb, 64, 0, p->stream>>>(ba);
+        else hb2::prune_batch_kernel<false><<<(unsigned)nb, 64, 0, p->stream>>>(ba);
+        p->launches++;
+        CU(cudaGetLastError());
+    }
+    if (c.entry == BatchEntry::JointAncestors) {   // after the inside pass, whose cond / node_ex it then reuses
+        const hb2::JointArgs g{ba, ws.arg, ws.states, ws.jlnl};
+        if (c.weights) hb2::joint_ancestors_kernel<true><<<(unsigned)nb, 64, 0, p->stream>>>(g);
+        else hb2::joint_ancestors_kernel<false><<<(unsigned)nb, 64, 0, p->stream>>>(g);
+        p->launches++;
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(c.nodeStates + s0 * p->I, ws.states, (size_t)nb * p->I * sizeof(int64_t), cudaMemcpyDeviceToHost, p->stream));
+        if (c.jointLnL) CU(cudaMemcpyAsync(c.jointLnL + s0, ws.jlnl, (size_t)nb * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
+    }
     if (c.rowLnL || c.support) {
         const size_t side = (size_t)nb * p->B;
         hb2::OutsideArgs g{ba, ws.side, ws.side + side * 64, ws.side_ex, ws.side_ex + side, ws.rows, ws.sup};
@@ -2073,6 +2103,17 @@ int hb2_batch_leaf_support(hb2_partition *p, int64_t templateId, int64_t nSets, 
     BatchCall c{BatchEntry::LeafSupport, templateId, nSets, K, branchK, branchGroup, formulaValues, weights, rootFreqs,
                 patternOf, nullptr, siteLnL};
     c.support = support;
+    return batch_sites(p, c);
+}
+
+int hb2_batch_joint_ancestors(hb2_partition *p, int64_t templateId, int64_t nSets, const int64_t *patternOf, int64_t K,
+                              const int64_t *branchK, const double *formulaValues, const double *weights,
+                              const int64_t *branchGroup, const double *rootFreqs, double *siteLnL, double *jointLnL,
+                              int64_t *nodeStates) {
+    BatchCall c{BatchEntry::JointAncestors, templateId, nSets, K, branchK, branchGroup, formulaValues, weights, rootFreqs,
+                patternOf, nullptr, siteLnL};
+    c.nodeStates = nodeStates;
+    c.jointLnL = jointLnL;
     return batch_sites(p, c);
 }
 

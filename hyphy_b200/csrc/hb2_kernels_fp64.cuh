@@ -1402,6 +1402,17 @@ __global__ void __launch_bounds__(256) combine_kernel(CombineArgs a) {
 //   - Padded states (k >= D) stay 0: their table entries are 0, or the kernel masks them (dot's `live`).
 //   - The group sum is one fixed-order xor tree of width G; G = 64 adds the totals of its two warps, red[0] + red[1].  A
 //     pattern's sum * 2^ex goes out through pattern_lnl: a likelihood of 0 gives -inf and NaN stays NaN.
+//   - Joint reconstruction (joint_ancestors_kernel; the reference's RecoverAncestralSequences, tree.cpp:4209-4510):
+//     a max-product replaces each sum.  A child's factor at parent state p is max_c P[p][c] x_c over c ascending, by
+//     strict > against a running maximum that starts at 0 with argument 0 (max_product; tree.cpp:4357-4377): ties go to
+//     the lowest c, a product that is 0 or NaN never wins, and a row with no positive product gives 0 with argument 0.
+//     x is an internal child's vector, or a leaf's 0/1 ambiguity row, which gives the max of P[p][c] over its nonzero
+//     states (ambig_max); a resolved leaf multiplies by P[p][code] with no max (tree.cpp:4315-4327).  A child is
+//     unresolved when it is a leaf whose row is 1 in all D states or an internal node all of whose children are
+//     unresolved: it takes no state and does not multiply its parent (tree.cpp:4350-4356, :4390-4394).  The root state
+//     is the lowest k of the largest positive pi_k J_root[k], 0 when none is positive (argmax; tree.cpp:4448-4457).
+//     Renormalisation by powers of two changes no comparison, so the reference's own rescaling (:4379-4383) is free to
+//     differ.
 // ------------------------------------------------------------------------------------------------
 template <int G>
 struct Group {
@@ -1477,6 +1488,47 @@ struct Group {
             for (int j = 0; j < D; j++) { const double w = amb[j]; if (w != 0.0) m = fma(w, entry(j), m); }
         }
         return m;
+    }
+    // max_j x_j entry(j) over j < D for a staged x, and its argument, by the joint reconstruction's strict-> scan; `bad` is
+    // set by a NaN product.  A thread that is not `live` reads no entry and returns 0 with argument 0.
+    template <typename Entry>
+    __device__ __forceinline__ double max_product(double staged, int D, bool live, Entry entry, int &arg, bool &bad) const {
+        double best = 0.0;
+        int c = 0;
+        bool nan = false;
+        if (G == 64 && !live) { arg = 0; return 0.0; }
+        for (int j = 0; j < D; j++) {
+            const double t = at(staged, j) * (live ? entry(j) : 0.0);
+            if (t > best) { best = t; c = j; }
+            nan |= t != t;
+        }
+        arg = c;
+        bad |= live && nan;
+        return best;
+    }
+    // max_j entry(j) over the nonzero states j < D of a 0/1 ambiguity row (0 when none is positive); `all` tells whether
+    // every state is nonzero (an unresolved leaf); `bad` is set by a NaN entry read.
+    template <typename Entry>
+    __device__ __forceinline__ double ambig_max(const double *row, int D, bool live, Entry entry, bool &all, bool &bad) const {
+        double best = 0.0;
+        bool full = true, nan = false;
+        for (int j = 0; j < D; j++) {
+            if (row[j] == 0.0) { full = false; continue; }
+            if (!live) continue;
+            const double t = entry(j);
+            if (t > best) best = t;
+            nan |= t != t;
+        }
+        all = full;
+        bad |= nan;
+        return best;
+    }
+    // The lowest k whose x_k is the group's largest positive value, and that value in `best`; 0 and 0.0 when no x_k is
+    // positive (a NaN never wins).
+    __device__ __forceinline__ int argmax(double x, double &best) const {
+        const double v = x > 0.0 ? x : 0.0;
+        best = max(v);
+        return G - (int)max(v == best ? (double)(G - k) : 0.0);
     }
 };
 
@@ -1902,6 +1954,113 @@ __global__ void __launch_bounds__(64) branch_rows_kernel(OutsideArgs g) { outsid
 // north-star FEL / MEME-all / MEME-third shapes (tools/bench_leaf_support.py, alternating runs, identical output).
 template <bool MIX>
 __global__ void __launch_bounds__(64, 8) leaf_support_kernel(OutsideArgs g) { outside_pass<OutsideEmit::LeafSupport, MIX>(g); }
+
+// ------------------------------------------------------------------------------------------------
+// joint_ancestors_kernel<MIX> (hb2_batch_joint_ancestors, both layouts): the joint maximum-likelihood states of every
+// internal node of a set (Pupko's max-product recursion, the reference's RecoverAncestralSequences).  One CTA of 64
+// threads per set, thread p = parent state p, under the group toolkit's rules for joint reconstruction.
+//   1. Internal nodes in flat (post-) order, exactly as prune_batch_kernel walks them, with the same BranchP reads of the
+//      transposed table, the same wide-node rescale and the same renormalisation at each node's end: J_par[p] is the
+//      product over its resolved children of P[p][code] (a resolved leaf), ambig_max (an ambiguous leaf) or max_product
+//      over the child's staged J (an internal child), whose argument goes to arg[child][p].  An unresolved internal child's
+//      row of arg is 0xFF, and an unresolved node's exponent is JOINT_UNRESOLVED.
+//   2. The root state r = argmax of pi_k J_root[k].
+//   3. Traceback by thread 0 in reverse flat order (a pre-order): an internal child's state is arg[child][state of its
+//      parent], or -1 below an unresolved parent or for an unresolved child.
+// The chunk's cond / node_ex hold the joint vectors (the inside pass, when it ran, is done with them).  jointLnL is
+// pattern_lnl of pi_r J_root[r] 2^ex, 0.0 for an unresolved root, and NaN when any thread of the set multiplied or compared
+// a NaN (one flag per thread, combined by the group at the root).
+// ------------------------------------------------------------------------------------------------
+constexpr int JOINT_UNRESOLVED = INT_MIN;
+
+// A minimum of 8 CTAs per SM, as leaf_support_kernel (a chunk of at most 1024 sets puts no more on any of the 132 SMs),
+// lets ptxas use 56 / 80 registers instead of 42 / 32; on one H100 at 700 W the kernel then took 9.7-9.9 / 16.8 / 12.9 ms
+// instead of 9.9 / 42.4 / 33.5-34.0 ms on the north-star FEL / MEME-all / MEME-third shapes (tools/bench_joint_ancestors.py,
+// alternating runs, identical output).
+
+struct JointArgs {
+    BatchPruneArgs in;        // the chunk's sets: PT, pat, leaf, ambig, pi, tree (MIX: mix_w, row_off); cond / node_ex scratch
+    unsigned char *arg;       // [nSets][I][64] state of internal node i given its parent's state; 0xFF: i is unresolved
+    long long *states;        // [nSets][I] the reconstruction: a state 0..D-1, or -1
+    double *lnl;              // [nSets] jointLnL
+};
+
+template <bool MIX>
+__global__ void __launch_bounds__(64, 8) joint_ancestors_kernel(JointArgs g) {
+    __shared__ double xs[64];
+    __shared__ double red[2];
+    const BatchPruneArgs &a = g.in;
+    const int s = blockIdx.x, k = threadIdx.x;
+    const Group<64> grp{xs, red, 0xffffffffu, k};
+    const bool live = k < a.D;
+    const int pattern = a.pat[s];
+    const double *PTs = a.PT + (size_t)s * (MIX ? a.R : a.B) * 4096;
+    const double *mw = MIX ? a.mix_w + (size_t)s * a.R : nullptr;
+    double *cs = a.cond + (size_t)s * a.I * 64;
+    int *node_ex = a.node_ex + (size_t)s * a.I;
+    unsigned char *arg = g.arg + (size_t)s * a.I * 64;
+    bool bad = false, open = true;               // a NaN was met; the node has no resolved child yet
+    double v = 0.0;
+    int ex = 0;
+    for (int par = 0; par < a.I; par++) {
+        v = live ? 1.0 : 0.0;
+        ex = 0;
+        open = true;
+        const int c_begin = a.tree.child_start[par], c_end = a.tree.child_start[par + 1];
+        for (int ci = c_begin; ci < c_end; ci++) {
+            if (ci - c_begin >= 2) grp.renorm(v, ex, RESCALE_BELOW);
+            const int child = a.tree.child_ids[ci];
+            BranchP<MIX> P(a, PTs, child);
+            P.load_weights(mw);
+            auto entry = [&](int j) { return P(j * 64 + k); };
+            double m;
+            if (child < a.L) {
+                const int code = a.leaf[(size_t)child * a.Sp + pattern];
+                if (code >= 0) {
+                    m = live ? entry(code) : 0.0;
+                    bad |= m != m;
+                } else {
+                    bool all;
+                    m = grp.ambig_max(a.ambig + (size_t)(-code - 1) * 64, a.D, live, entry, all, bad);
+                    if (all) continue;
+                }
+            } else {
+                const int cin = child - a.L;
+                if (node_ex[cin] == JOINT_UNRESOLVED) { arg[(size_t)cin * 64 + k] = 0xFF; continue; }
+                int c;
+                m = grp.max_product(grp.stage(cs[(size_t)cin * 64 + k]), a.D, live, entry, c, bad);
+                arg[(size_t)cin * 64 + k] = (unsigned char)c;
+                ex += node_ex[cin];
+            }
+            v *= m;
+            open = false;
+        }
+        grp.renorm(v, ex);
+        cs[(size_t)par * 64 + k] = v;
+        if (k == 0) node_ex[par] = open ? JOINT_UNRESOLVED : ex;
+        __syncthreads();                         // node_ex and arg rows visible to the block
+    }
+    // the root (par = I - 1): v, ex and open are its own
+    const double x = live ? v * a.pi[k] : 0.0;
+    bad |= x != x;
+    const bool nan = grp.max(bad ? 1.0 : 0.0) > 0.0;
+    double best;
+    const int r = grp.argmax(x, best);
+    if (k == 0) {
+        long long *st = g.states + (size_t)s * a.I;
+        st[a.I - 1] = open ? -1 : r;
+        for (int n = a.I - 1; n >= 0; n--) {
+            const long long sn = st[n];
+            for (int ci = a.tree.child_start[n]; ci < a.tree.child_start[n + 1]; ci++) {
+                const int child = a.tree.child_ids[ci];
+                if (child < a.L) continue;
+                const int c = sn < 0 ? 0xFF : arg[(size_t)(child - a.L) * 64 + sn];
+                st[child - a.L] = c == 0xFF ? -1 : c;
+            }
+        }
+        g.lnl[s] = open ? 0.0 : nan ? (double)NAN : pattern_lnl(best, ex, [] {});
+    }
+}
 
 // ------------------------------------------------------------------------------------------------
 // prune_rates_kernel (hb2_batch_site_rates): prune_batch_kernel<false>'s recursion for 4..32 padded states.  A group of

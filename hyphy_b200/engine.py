@@ -47,6 +47,8 @@ ABI = [
     ("hb2_batch_branch_component_likelihoods", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, C.c_int64, _ip, _dp, _dp, _ip,
                                                          _dp, _dp, _dp]),
     ("hb2_batch_leaf_support", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, C.c_int64, _ip, _dp, _dp, _ip, _dp, _dp, _dp]),
+    ("hb2_batch_joint_ancestors", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, C.c_int64, _ip, _dp, _dp, _ip, _dp, _dp, _dp,
+                                            _ip]),
     ("hb2_batch_column_likelihoods", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, C.c_int64, _ip, _dp, _dp, _ip, _dp, _dp]),
     ("hb2_batch_site_rates", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _ip, _dp, _dp, _dp]),
     ("hb2_read_conditionals", C.c_int, [C.c_void_p, C.c_int64, C.c_int64, _dp, _i32p]),
@@ -315,6 +317,22 @@ class Partition:
         _check(self._lib.hb2_batch_leaf_support(self._h, int(template), len(po), ppo, K, pbk, pv, pw, pbg, ppi,
                                                 site.ctypes.data_as(_dp) if want_site else None, sup.ctypes.data_as(_dp)))
         return (sup, site) if want_site else sup
+
+    def batch_joint_ancestors(self, pattern_of, formula_values, root_freqs, weights=None, branch_k=None, branch_group=None,
+                              template=0, want_site=False):
+        """Joint maximum-likelihood ancestral states (hb2_batch_joint_ancestors): sets as batch_leaf_support.  Returns
+        (node_states [nSets, I], joint_lnl [nSets]), node_states[s][i] being internal node i's state or -1 (unresolved);
+        with want_site also the nSets site log-likelihoods, as (node_states, joint_lnl, site_lnl)."""
+        po, ppo = _i(pattern_of)
+        K, pbk, pv, pw, pbg, keep = self._batch_rows(len(po), formula_values, weights, branch_k, branch_group)
+        pi, ppi = _d(root_freqs)
+        site = np.empty(len(po)) if want_site else None
+        jl = np.empty(len(po))
+        st = np.empty((len(po), self.I), dtype=np.int64)
+        _check(self._lib.hb2_batch_joint_ancestors(self._h, int(template), len(po), ppo, K, pbk, pv, pw, pbg, ppi,
+                                                   site.ctypes.data_as(_dp) if want_site else None, jl.ctypes.data_as(_dp),
+                                                   st.ctypes.data_as(_ip)))
+        return (st, jl, site) if want_site else (st, jl)
 
     def _batch_rows(self, n_sets, formula_values, weights, branch_k, branch_group):
         """Checked arguments of the batch entry points that take both set layouts: weights None means one row per branch

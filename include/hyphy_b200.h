@@ -227,6 +227,44 @@ int hb2_batch_leaf_support(hb2_partition *p, int64_t templateId, int64_t nSets, 
                            int64_t K, const int64_t *branchK, const double *formulaValues, const double *weights,
                            const int64_t *branchGroup, const double *rootFreqs, double *siteLnL, double *support);
 
+/* Joint maximum-likelihood ancestral states for FEL's, MEME's and PRIME's per-site reconstruction (ancestral.build(lf, 0,
+ * FALSE) at every site, FEL.bf:798-801, MEME.bf:1359-1363, PRIME.bf:975 and :1013): what ReconstructAncestors(lf, {{0}})
+ * reports for the internal nodes of a site, for every set in one call.  The reference's procedure is Pupko's max-product
+ * recursion (_LikelihoodFunction::ReconstructAncestors, likefunc2.cpp:309-480; _TheTree::RecoverAncestralSequences,
+ * tree.cpp:4209-4510) without category variables, every branch under its one transition matrix (an explicit-form
+ * mixture's mixed matrix):
+ *   children in increasing flat id, each parent vector starting at 1 (:4253, :4266-4271); a resolved leaf in state a
+ *   multiplies it by P[p][a] (:4315-4327); an ambiguous leaf or internal child with vector x (its 0/1 row, or the child's
+ *   joint vector) multiplies it by max_c P[p][c] x[c], the scan over ascending c by strict > against a running maximum
+ *   that starts at 0 with index 0, so ties go to the lowest c and a row with no positive product gives 0 with index 0
+ *   (:4357-4377); an unresolved child -- a leaf whose row is 1 in all D states, or an internal node all of whose children
+ *   are unresolved -- takes state -1 and does not multiply its parent (:4350-4356, :4390-4394); the root state is argmax_c
+ *   pi_c J_root[c] by the same rule, -1 when the root is unresolved (:4448-4457, :4484-4486); traceback takes each internal
+ *   node's argument at its parent's state, -1 below a -1 (:4458-4470).  The reference's unresolved test compares values
+ *   with 1.0; the engine's is structural, which agrees except when a resolved subtree's vector is exactly 1 in all D
+ *   states (DESIGN §4.13).
+ * Sets as hb2_batch_leaf_support, on partition patterns: weights == NULL gives one row per branch (K must be 1 and branchK
+ * NULL; FEL's and PRIME's site models), otherwise MEME's mixture rows.  Outputs:
+ *   nodeStates [nSets][I]: entry i is internal node i (root at I-1, as hb2_batch_site_simulate's nodeStates): a state
+ *              0..D-1, or -1 for an unresolved node.
+ *   jointLnL   nullable [nSets]: log(pi_r J_root[r]) at the returned root state r; -inf for a product of 0, 0.0 for a fully
+ *              unresolved column, NaN for a set whose recursion multiplied or compared a NaN (its states are still those
+ *              the comparisons give).
+ *   siteLnL    nullable [nSets]: bit for bit what hb2_batch_site_likelihoods (weights == NULL) or
+ *              hb2_batch_site_mixture_likelihoods returns for the same arguments; its inside pass runs only when given.
+ * Plain sets give, bit for bit, the states and jointLnL of the mixture layout with one component of weight 1.0 per branch.
+ * A NaN weight or formula value affects its own set only.  fp64 throughout, every joint vector renormalised by exact
+ * powers of two (which changes no comparison).
+ * Refusals before anything is launched or written (the partition stays usable): everything the corresponding likelihood
+ * entry point refuses; nodeStates == NULL; K != 1 or a non-NULL branchK without weights.  nSets == 0 after these checks
+ * does nothing.  33..64 states only; not available in class-group mode.
+ * Nothing an evaluation reads is touched: conditionals, scalers, walk plans and tags, the branch cache, the staged root
+ * vector, the P cache and the resident rate matrices. */
+int hb2_batch_joint_ancestors(hb2_partition *p, int64_t templateId, int64_t nSets, const int64_t *patternOf,
+                              int64_t K, const int64_t *branchK, const double *formulaValues, const double *weights,
+                              const int64_t *branchGroup, const double *rootFreqs,
+                              double *siteLnL, double *jointLnL, int64_t *nodeStates);
+
 /* The batch likelihoods of caller-given columns instead of partition patterns (the refits of a parametric bootstrap score
  * columns simulated by hb2_batch_site_simulate, which are not patterns of the partition): set s scores
  * columns[s][0..L-1], in hb2_create's leafState codes (>= 0: a state < D; < 0: ambiguity row -(code+1) < nAmb).

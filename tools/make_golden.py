@@ -9,7 +9,9 @@ with (the final lnL of an evaluation stream, joint ML ancestral sequences).
 (meme.compute_branch_EBF, MEME.bf:886-944) on every site at once -- see pinned_fixture.
 `--impute` writes tests/golden/<case>_impute.npz for IMPUTE_CASES: leaf state imputation
 (ReconstructAncestors(MARGINAL, DOLEAVES), MEME's and PRIME's --impute-states) on every site -- see impute_fixture.
-Run where the reference binary was built:  python tools/make_golden.py [--runs | --pinned | --impute | name ...]
+`--joint` writes tests/golden/<case>_joint.npz for JOINT_CASES: the joint maximum-likelihood ancestral states
+(ReconstructAncestors, as FEL, MEME and PRIME run it per site through ancestral.build) on every site -- see joint_fixture.
+Run where the reference binary was built:  python tools/make_golden.py [--runs | --pinned | --impute | --joint | name ...]
 """
 import hashlib
 import json
@@ -178,6 +180,67 @@ def impute_fixture(out, name):
     print(f"{name}_impute: lnL={lnL!r} leaves={L} sites={n} filter patterns={n_pat}", flush=True)
 
 
+# mixture layout (K = 3 on every branch), plain layout, and a gap-rich plain case ('---', N and R/Y codons, unresolved
+# cherries) that nothing but its fixture builds or loads
+JOINT_CASES = {"bsrel_12x80_k3": CASES["bsrel_12x80_k3"], "mg94_8x60_c1": CASES["mg94_8x60_c1"],
+               "mg94_8x60_c1_gaps": lambda: synth.codon_workload(8, 60, 1, ambig_frac=0.5)}
+
+
+def joint_script(w, path_bf, path_fas):
+    """The case's script of ref_harness.write_hbl, followed by the joint reconstruction: `NAMES` the reconstructed data
+    set's sequence names, `DUP` the filter's site-to-pattern map, then one `ANC k sequence` line per internal node."""
+    rh.write_hbl(w, path_bf, path_fas, per_site=False)
+    lines = ["DataSet anc = ReconstructAncestors (lf);",
+             "GetString (nms, anc, -1);",
+             'for (k = 0; k < Columns (nms); k += 1) { fprintf (stdout, "NAMES ", k, " ", nms[k], "\n"); }',
+             "GetDataInfo (dup, flt);",
+             'fprintf (stdout, "DUP");',
+             'for (k = 0; k < Columns (dup); k += 1) { fprintf (stdout, " ", dup[k]); }',
+             'fprintf (stdout, "\n");',
+             "DataSetFilter ancf = CreateFilter (anc, 1);",
+             'for (k = 0; k < ancf.species; k += 1) { GetDataInfo (aSeq, ancf, k); fprintf (stdout, "ANC ", k, " ", aSeq, "\n"); }']
+    with open(path_bf, "a") as f:
+        f.write("\n".join(lines) + "\n")
+
+
+def joint_fixture(out, name):
+    """tests/golden/<name>_joint.npz: states [sites][I] -- entry i of a site is the reference's joint ML state of internal
+    node i (mapped by name) as a sense-codon index of synth's codon table, -1 for '---' -- and the workload checksum."""
+    w = JOINT_CASES[name]()
+    L, I, n = w.tree.n_leaves, w.tree.n_internal, len(w.site_to_pattern)
+    tmp = tempfile.mkdtemp(prefix="hb2ref_")
+    bf, fas = os.path.join(tmp, "job.bf"), os.path.join(tmp, "job.fas")
+    joint_script(w, bf, fas)
+    proc = subprocess.run([rh.REF_BIN, "CPU=1", bf], cwd=tmp, stdin=subprocess.DEVNULL, capture_output=True, text=True, check=True)
+    names, dup, seqs = {}, None, {}
+    for line in proc.stdout.splitlines():
+        f = line.split()
+        if f and f[0] == "NAMES":
+            names[int(f[1])] = f[2]
+        elif f and f[0] == "DUP":
+            dup = np.array([int(x) for x in f[1:]], dtype=np.int64)
+        elif f and f[0] == "ANC":
+            seqs[int(f[1])] = f[2]
+    assert dup is not None and len(dup) == n and len(seqs) == I == len(names), proc.stdout[-2000:]
+    node_of = {nm: i for i, nm in enumerate(w.tree.names[L:L + I - 1])}
+    unnamed = [nm for nm in names.values() if nm not in node_of]
+    assert len(unnamed) == 1, unnamed           # the newick leaves the root unnamed: the binary names it itself
+    node_of[unnamed[0]] = I - 1
+    code = {synth.codon_str(c): k for k, c in enumerate(synth.SENSE)}
+    code["---"] = -1
+    states = np.full((n, I), -2, dtype=np.int64)
+    for k, seq in seqs.items():
+        assert len(seq) == 3 * n, (k, len(seq))
+        states[:, node_of[names[k]]] = [code[seq[3 * j:3 * j + 3]] for j in range(n)]
+    assert np.all(states >= -1)
+    for p in range(w.S):                        # sites of one pattern of the engine's compression share their states
+        sites = np.nonzero(w.site_to_pattern == p)[0]
+        assert np.all(states[sites] == states[sites[:1]]), p
+    np.savez_compressed(os.path.join(out, name + "_joint.npz"), states=states, checksum=np.array(checksum(w)),
+                        S=np.int64(w.S), sites=np.int64(n))
+    print(f"{name}_joint: internal nodes={I} sites={n} unresolved={int((states < 0).sum())}", flush=True)
+
+
 def main():
     out = os.path.join(ROOT, "tests", "golden")
     os.makedirs(out, exist_ok=True)
@@ -187,6 +250,10 @@ def main():
         return
     if only == ["--pinned"]:
         pinned_fixture(out)
+        return
+    if only == ["--joint"]:
+        for name in JOINT_CASES:
+            joint_fixture(out, name)
         return
     if only == ["--impute"]:
         for name in IMPUTE_CASES:
